@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native video hot path (driver contract, see DESIGN.md §7).
+"""bench.py — headline benchmark of the H100-native video hot path (see DESIGN.md §7).
 
 Workload (BASELINE.json metric "4K frames/sec encoded per GPU", configs[2]): synthetic desktop-like
 3840x2160 BGRA frames -> fused BT.709 CSC -> H.264 Constrained-Baseline (one IDR, then P pictures with
@@ -9,11 +9,16 @@ A STEP is one batch of FRAMES_PER_STEP frames through one session (one session p
   value  frames/s with the BGRA inputs already resident in HBM (b2v_submit_resident), device-timed
   e2e    frames/s through the host-buffer API: pinned host ring -> cudaMemcpyAsync H2D -> CSC -> encode
          -> D2H of every access unit -> Python callback, wall-clock + device timer inside the timed region
-  roofline       the fused CSC kernel: algorithmic bytes (5.5 B/px) / CUDA-event time per launch, in-step
+  roofline       the fused CSC kernel: algorithmic bytes (5.5 B/px) / CUDA-event time per launch, in-step, as a fraction of
+                 the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s)
   cpu_baseline   the CPU restatement (oracle/) on the host cores, bounded sample (rank 0, N=1 only)
 
 `--impl reference` times the CPU path only (the reference's own videoconvert+x264enc pipeline cannot
 run here — SURVEY.md §8c — so the arm runs the oracle port, all host threads, labelled kind="port").
+
+`--dump-outputs DIR` writes what the timed leg delivered in its last step — the access units of its FRAMES_PER_STEP pictures —
+as DIR/*.npy (float32 / float64), so that two builds can be compared output for output on identical inputs.  Capturing them
+needs a Python callback on the timed session, which slows and spreads `value`: take timings from a run without it.
 """
 from __future__ import annotations
 
@@ -35,9 +40,11 @@ W, H = 3840, 2160
 FPS_NOMINAL = 60.0
 BITRATE_KBPS = 20000
 FRAMES_PER_STEP = 64      # one step = one batch of 64 pictures through the hot path (long enough that host scheduling jitter averages out)
-N_DISTINCT = 16           # distinct input frames cycled (the scroll restarts every 16 pictures): 16 x 33.2 MB = 531 MB > 126 MB of L2
+N_DISTINCT = 16           # distinct input frames cycled (the scroll restarts every 16 pictures): 16 x 33.2 MB = 531 MB > 50 MB of L2
 N_SIDE = 256              # pictures in each side measurement (device-timer pass, striped mode)
 ALG_BYTES_PER_PX = 5.5    # 4 B BGRA read + 1 B Y + 0.5 B CbCr written (SURVEY.md §8d)
+HBM_PEAK_GBS = 3350.0     # H100 SXM data sheet (HBM3, 700 W card); a roofline fraction is achieved / this, never a measured peak
+DUMP_MAX_BYTES = 16 << 20 # --dump-outputs: at most 16 Mi access-unit bytes (64 MB as float32); more is sampled with a fixed seed
 
 
 def synth_frames(n, w=W, h=H):
@@ -46,7 +53,7 @@ def synth_frames(n, w=W, h=H):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md clocks line).  One nvidia-smi process
+    """nvidia-smi clocks + throttle reasons DURING the timed region.  One nvidia-smi process
     (rank 0 only, all GPUs of the job, 100 ms period) is started before the warm-up so that it is already streaming when the
     timed region begins; `mark()` / `stop()` delimit the rows that fall inside it."""
 
@@ -103,13 +110,6 @@ class ClockSampler:
                 "samples": len(sm), "window": window, "gpus_sampled": self.n_gpus}
 
 
-def measured_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
 def cpu_quota():
     """CPUs this container may actually use (cgroup v2 cpu.max), or None when unlimited/unknown."""
     try:
@@ -138,27 +138,6 @@ def bind_to_gpu_numa_node(torch, device: int):
         return node
     except Exception:
         return None
-
-
-def csc_dram_traffic():
-    """(total, read, write, file) DRAM bytes of one 4K CSC launch from the newest committed `ncu --set full` capture under
-    profiles/.  The read side is exactly the 33.2 MB BGRA input (no re-reads); the 12.4 MB NV12 output stays in L2 for the
-    encoder kernels that follow (write side: a few KB), so traffic < algorithmic bytes."""
-    try:
-        import csv, glob
-        files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_full_v*_raw.csv")), key=lambda p: os.path.basename(p).split("_raw")[0][:len("r1_ncu_full_v9")])
-        scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        for path in reversed(files):              # newest capture that holds a CSC launch
-            rows = list(csv.reader(open(path)))
-            hdr, units = rows[0], rows[1]
-            ik, ir, iw = hdr.index("Kernel Name"), hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-            for r in rows[2:]:
-                if "csc_bgra_nv12" in r[ik]:
-                    rd, wr = float(r[ir]) * scale.get(units[ir], 1), float(r[iw]) * scale.get(units[iw], 1)
-                    return rd + wr, rd, wr, os.path.basename(path)
-    except Exception:
-        pass
-    return None, None, None, None
 
 
 def usable_threads() -> int:
@@ -331,28 +310,19 @@ def python_surface_leg(frames, device, seconds=2.0):
                     "into the pinned slot per frame (single Python thread), H2D, encode, D2H"}
 
 
-def live_csc_traffic(timeout_s=240):
-    """dram__bytes_read/write of one 4K CSC launch, measured NOW on this box with this build: a short ncu run (separate process,
-    CSC-only session, outside every timed region).  None when ncu cannot run here."""
-    import csv, io, shutil
-    ncu = shutil.which("ncu") or "/usr/local/cuda/bin/ncu"
-    if not os.path.exists(ncu):
-        return None
-    try:
-        out = subprocess.run([ncu, "--metrics", "dram__bytes_read.sum,dram__bytes_write.sum", "--clock-control", "none", "-k", "regex:csc_bgra_nv12",
-                              "-s", "4", "-c", "4", "--csv", sys.executable, os.path.join(ROOT, "tools", "csc_once.py")],
-                             capture_output=True, text=True, timeout=timeout_s, cwd=ROOT)
-        rows = [r for r in csv.reader(io.StringIO(out.stdout)) if len(r) > 10]
-        hdr = rows[0]
-        im, iv, iu = hdr.index("Metric Name"), hdr.index("Metric Value"), hdr.index("Metric Unit")
-        scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        rd = [float(r[iv].replace(",", "")) * scale.get(r[iu], 1) for r in rows[1:] if r[im] == "dram__bytes_read.sum"]
-        wr = [float(r[iv].replace(",", "")) * scale.get(r[iu], 1) for r in rows[1:] if r[im] == "dram__bytes_write.sum"]
-        if not rd or not wr:
-            return None
-        return {"read": sum(rd) / len(rd), "write": sum(wr) / len(wr), "launches": len(rd), "source": "live ncu run inside bench.py (tools/csc_once.py)"}
-    except Exception:
-        return None
+def dump_outputs(out_dir, aus):
+    """The access units a caller of the timed path received in its last step: their bytes concatenated (float32; a seeded sample
+    when longer than DUMP_MAX_BYTES), and per picture the size, QP and key-frame flag (float64)."""
+    if len(aus) != FRAMES_PER_STEP:
+        raise RuntimeError(f"--dump-outputs: {len(aus)} access units captured from the last step, expected {FRAMES_PER_STEP}")
+    os.makedirs(out_dir, exist_ok=True)
+    data = np.frombuffer(b"".join(a for a, _, _ in aus), np.uint8)
+    if data.size > DUMP_MAX_BYTES:
+        data = data[np.sort(np.random.default_rng(0).choice(data.size, DUMP_MAX_BYTES, replace=False))]
+    np.save(os.path.join(out_dir, "access_unit_bytes.npy"), data.astype(np.float32))
+    np.save(os.path.join(out_dir, "access_unit_sizes.npy"), np.array([len(a) for a, _, _ in aus], np.float64))
+    np.save(os.path.join(out_dir, "access_unit_qp.npy"), np.array([q for _, _, q in aus], np.float64))
+    np.save(os.path.join(out_dir, "access_unit_is_key.npy"), np.array([k for _, k, _ in aus], np.float64))
 
 
 def workload_config(frames_per_step):
@@ -388,7 +358,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the access units of the last timed step to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
     rank = int(os.environ.get("RANK", "0"))
@@ -443,22 +416,28 @@ def main():
         return float(t.item())
 
     frames = synth_frames(N_DISTINCT)
-    peak, peak_src = measured_peak()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet, HBM3 3.35 TB/s"
     # leg 1 (`value`, inputs resident) and leg 2 (`e2e`) run with no instrumentation; the CUDA-event pairs around the CSC launches
     # that `roofline` is computed from sit in leg 1b: the same resident-input steps, timed the same way, with
     # B2V_FLAG_TIMING_CSC on (an event pair around the CSC launch of every 4th picture).  The events cost a GPU-bound step 4-5 %,
     # which is why `value` is not quoted from that leg; in the PCIe-bound e2e leg the GPU idles between pictures and an event
     # pair there mostly measures wake-up latency (29 us around a 9 us kernel)
-    sess = Session(W, H, fps=FPS_NOMINAL, device=local_rank, rc_mode=N.B2V_RC_CBR, bitrate_kbps=BITRATE_KBPS,
-                   ring_slots=N_DISTINCT, flags=0, collect=False)
-    out_bytes = [0]
-    sample_aus = []
+    # leg 1 registers no Python callback: a per-picture callback has to take the GIL from the submitting thread on every picture,
+    # and that hand-off, not the GPU, then sets the pace and the run-to-run spread.  Its byte counts come from the session's
+    # stats.  Only --dump-outputs adds a callback, which copies the access units of the last timed step.
+    # The session delivers one access unit per picture, in order; the pictures of the last timed step are delivered pictures
+    # [first, first + FRAMES_PER_STEP) counted from the session's start.
+    n_delivered = [0]
+    dump_first = (args.warmup + args.steps - 1) * FRAMES_PER_STEP
+    dump_aus = []
 
-    def on_frame(fptr):
-        out_bytes[0] += fptr.contents.size
-        if len(sample_aus) < 8 and not fptr.contents.is_key:
-            sample_aus.append(ctypes.string_at(fptr.contents.data, fptr.contents.size))
-    sess._on_frame = on_frame
+    def capture_last_step(fptr):
+        if dump_first <= n_delivered[0] < dump_first + FRAMES_PER_STEP:
+            f = fptr.contents
+            dump_aus.append((ctypes.string_at(f.data, f.size), f.is_key, f.qp))
+        n_delivered[0] += 1
+    sess = Session(W, H, fps=FPS_NOMINAL, device=local_rank, rc_mode=N.B2V_RC_CBR, bitrate_kbps=BITRATE_KBPS,
+                   ring_slots=N_DISTINCT, flags=0, collect=False, on_frame=capture_last_step if args.dump_outputs else None)
 
     # ---------------- leg 1: inputs resident in HBM ----------------------------------------------------
     for i, f in enumerate(frames):
@@ -518,33 +497,43 @@ def main():
 
     # ---------------- leg 2: end to end from pinned host buffers -----------------------------------------
     # pre-fill the pinned ring once (the producer — XShm grab in the reference — writes into these slots);
-    # every frame is then copied H2D inside the timed region and every access unit copied back D2H.
+    # every frame is then copied H2D inside the timed region and every access unit copied back D2H to a Python callback.
+    out_bytes = [0]
+    sample_aus = []
+
+    def on_frame(fptr):
+        out_bytes[0] += fptr.contents.size
+        if len(sample_aus) < 8 and not fptr.contents.is_key:
+            sample_aus.append(ctypes.string_at(fptr.contents.data, fptr.contents.size))
+    se = Session(W, H, fps=FPS_NOMINAL, device=local_rank, rc_mode=N.B2V_RC_CBR, bitrate_kbps=BITRATE_KBPS,
+                 ring_slots=N_DISTINCT, flags=0, collect=False, on_frame=on_frame)
     for i in range(N_DISTINCT):
-        slot, view = sess.acquire()
+        slot, view = se.acquire()
         view[...] = frames[i]
-        sess.submit_slot(slot)
-    sess.flush()
+        se.submit_slot(slot)
+    se.flush()
 
     def step_host():
         for _ in range(FRAMES_PER_STEP):
-            slot, _view = sess.acquire()       # round-robin: slot i still holds distinct frame i
-            sess.submit_slot(slot)
+            slot, _view = se.acquire()       # round-robin: slot i still holds distinct frame i
+            se.submit_slot(slot)
 
     for _ in range(args.warmup):
         step_host()
-    sess.flush()
-    st0 = sess.stats()
+    se.flush()
+    st0 = se.stats()
     out_bytes[0] = 0
     barrier()
-    sess.timer_start()
+    se.timer_start()
     t0 = time.perf_counter()
     for _ in range(args.steps):
         step_host()
-    e2e_dev_ms = sess.timer_stop()
+    e2e_dev_ms = se.timer_stop()
     e2e_wall_ms = 1000 * (time.perf_counter() - t0)
     barrier()
     clk = clocks.stop() if clocks else None
-    st1 = sess.stats()
+    st1 = se.stats()
+    se.close()
     e2e_ms = max_over_ranks(max(e2e_wall_ms, e2e_dev_ms))
     e2e_value = sum_over_ranks(float(n_frames)) / (e2e_ms / 1000.0)
     per_rank_e2e_ms = gather_over_ranks(max(e2e_wall_ms, e2e_dev_ms))
@@ -557,19 +546,13 @@ def main():
     csc_ms = st_roof["ms_csc"] / max(1, st_roof["n_csc"])       # event pairs of the instrumented resident leg (1b)
     achieved = alg / (csc_ms * 1e-3) / 1e9 if csc_ms > 0 else 0.0
     burst_ms = sess.bench_csc_burst(N_DISTINCT, 200)
-    traffic = csc_dram_traffic()
-    if rank == 0 and world == 1:
-        live = live_csc_traffic()
-        if live:
-            traffic = (live["read"] + live["write"], live["read"], live["write"], live["source"])
     roofline = {"bound": "hbm", "kernel": "csc_bgra_nv12_fast", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "peak_source": peak_src, "traffic": traffic[0], "traffic_read": traffic[1], "traffic_write": traffic[2], "traffic_source": traffic[3],
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg, "us_per_launch": csc_ms * 1e3,
                 "timed_launches": int(st_roof["n_csc"]),
                 "where": "CUDA-event pair around the CSC launch of every 4th picture of leg 1b: the resident-input steps of `value`, re-run with the events on "
                          f"({n_frames / (roof_ms / 1000.0):.0f} frames/s with them)",
                 "device_timer": None,
-                "frac_of_8TBps_nominal": achieved / 8000.0,
                 "burst": {"note": f"200 back-to-back launches between one event pair, same {N_DISTINCT} cycled frames",
                           "us_per_launch": burst_ms * 1e3, "achieved": alg / (burst_ms * 1e-3) / 1e9,
                           "frac": alg / (burst_ms * 1e-3) / 1e9 / peak}}
@@ -592,8 +575,7 @@ def main():
             if sdt["n_csc_device"]:
                 us = sdt["ms_csc_device"] / sdt["n_csc_device"] * 1e3
                 roofline["device_timer"] = {"note": "in-step launches timed by the kernel itself (%globaltimer), 256 pictures, separate instrumented pass",
-                                            "us_per_launch": us, "achieved": alg / (us * 1e-6) / 1e9, "frac": alg / (us * 1e-6) / 1e9 / peak,
-                                            "frac_of_8TBps_nominal": alg / (us * 1e-6) / 1e9 / 8000.0}
+                                            "us_per_launch": us, "achieved": alg / (us * 1e-6) / 1e9, "frac": alg / (us * 1e-6) / 1e9 / peak}
         except Exception as e:
             roofline["device_timer"] = {"error": repr(e)}
     # per-kernel breakdown: separate pass with every stage bracketed by events (those extra event commands cost the step 4-5 %,
@@ -630,7 +612,6 @@ def main():
                 ms8b = s8.bench_csc_burst(4, 60)
             alg8 = w8 * h8 * ALG_BYTES_PER_PX
             roofline["c4_8k_stress"] = {"us_per_launch": ms8 * 1e3, "achieved": alg8 / (ms8 * 1e-3) / 1e9, "frac": alg8 / (ms8 * 1e-3) / 1e9 / peak,
-                                        "frac_of_8TBps_nominal": alg8 / (ms8 * 1e-3) / 1e9 / 8000.0,
                                         "burst_us_per_launch": ms8b * 1e3, "burst_frac": alg8 / (ms8b * 1e-3) / 1e9 / peak,
                                         "algorithmic_bytes_per_launch": alg8, "note": "one CUDA-event pair per launch; 4 resident frames cycled (531 MB > L2)"}
         except Exception as e:
@@ -741,6 +722,9 @@ def main():
                    "x264_anchor": x264_anchor(cores)}
         except Exception as e:  # the checker failing must not hide the GPU number
             cpu = {"value": None, "error": repr(e)}
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dump_aus)
 
     if rank == 0:
         line = {

@@ -1,5 +1,5 @@
 /*
- * b2video.h — C-ABI of libb2video.so, the B200-native video-frame hot path.
+ * b2video.h — C-ABI of libb2video.so, the H100-native (sm_90a) video-frame hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point replaces one
  * call the selkies reference makes into its out-of-tree native module

@@ -1,7 +1,7 @@
-"""selkies_b200 — the B200-native video-frame hot path behind the selkies video-pipeline surface.
+"""selkies_b200 — the H100-native video-frame hot path behind the selkies video-pipeline surface.
 
 Only what the hot path needs lives here:
-  csrc/               hand-written sm_100a CUDA kernels + the C-ABI (include/b2video.h)
+  csrc/               hand-written sm_90a CUDA kernels + the C-ABI (include/b2video.h)
   _native.py          ctypes binding (no CPU fallback)
   pixelflux_compat.py CaptureSettings / ScreenCapture / StripeCallback (the module the reference imports)
   media_pipeline.py   MediaPipeline ABC + MediaPipelineB200 (mirror of src/selkies/media_pipeline.py)

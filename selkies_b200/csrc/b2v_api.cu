@@ -86,7 +86,7 @@ enum : uint8_t { SLOT_FREE = 0, SLOT_ACQUIRED = 1, SLOT_IN_FLIGHT = 2 };
 
 struct Session {
   b2v_settings cfg{};
-  int device = 0, sm_count = 148;
+  int device = 0, sm_count = 132;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
   bool encode = true, timing = false, timing_csc_only = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;

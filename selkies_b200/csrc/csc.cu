@@ -1,4 +1,4 @@
-// csc.cu — fused BGRA -> BT.709 limited-range NV12 colour conversion (+ bilinear scale), sm_100a.
+// csc.cu — fused BGRA -> BT.709 limited-range NV12 colour conversion (+ bilinear scale), sm_90a.
 //
 // Replaces the colour-conversion stage of the reference's native capture module
 // (pixelflux, call site src/selkies/media_pipeline.py:299-300; legacy GStreamer
@@ -12,7 +12,7 @@
 //              issued back to back so 2U 16-byte loads are in flight per thread.
 //   arithmetic: dp2a (two 16-bit coefficient x 8-bit pixel MACs per instruction); rounding
 //              constant and the +16 / +128 offsets are folded into the accumulator seed.
-//   TMA path   (1:1, the default on sm_100a): persistent grid of 2 CTAs per SM; one elected thread streams 256 px x 16 row
+//   TMA path   (1:1, opt-in with B2V_CSC=tma; the fast path is the default): persistent grid of 2 CTAs per SM; one elected thread streams 256 px x 16 row
 //              BGRA tiles (16 KB) into a 4-stage shared-memory ring with cp.async.bulk.tensor.2d (SASS: UTMALDG) completing on
 //              mbarriers, so 128 KB of reads per SM are in flight with no load instruction in the compute warps' issue slots;
 //              the 256 threads convert from shared memory (conflict-free LDS.128) and store Y/CbCr straight to HBM.

@@ -1,5 +1,5 @@
 // h264_encoder.h — interface between the session layer (b2v_api.cu) and the H.264 Baseline
-// encoder kernels (h264_*.cu).  B200 carries no NVENC block, so stage (c) of the hot path is a
+// encoder kernels (h264_*.cu).  H100 carries no NVENC block, so stage (c) of the hot path is a
 // software encoder made of CUDA kernels: one warp per macroblock.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 // h264_inter.cu — P pictures: one warp per macroblock, P_L0_16x16 (ITU-T H.264 8.4).
 //
 //  1. the 16x16 source block and a 48x48 window of the previous reconstruction (L2-resident: a 4K
-//     NV12 frame is 12.4 MB against 126 MB of L2) are staged in shared memory;
+//     NV12 frame is 12.4 MB against 50 MB of L2) are staged in shared memory;
 //  2. exhaustive full-sample search, dx in [-16,15] (one candidate column per LANE), dy in [-16,16]:
 //     every window row is byte-aligned once per lane with funnel shifts and then feeds the 16 (row, dy)
 //     pairs it belongs to — 33 SAD accumulators live in registers, VABSDIFF4.U8.ACC does 4 pixels per

@@ -55,7 +55,7 @@ class GSTWebRTCApp:
         if self.capture is not None:
             raise GSTWebRTCAppError("video pipeline already built")
         if self.encoder not in ("x264enc", "nvh264enc", "b200h264enc"):
-            raise GSTWebRTCAppError(f"unsupported encoder {self.encoder!r} for the B200 video branch")
+            raise GSTWebRTCAppError(f"unsupported encoder {self.encoder!r} for the CUDA video branch")
         cs = CaptureSettings()
         cs.capture_width, cs.capture_height = self.width, self.height
         cs.target_fps = float(self.framerate)

@@ -1,4 +1,4 @@
-"""Video side of the selkies media-pipeline interface, backed by the B200 encoder.
+"""Video side of the selkies media-pipeline interface, backed by the CUDA encoder of this package.
 
 The rest of selkies talks to an object with ten methods (the abstract class at src/selkies/media_pipeline.py:41-80) and two
 callback attributes (`produce_data(buf, pts, kind)`, `send_data_channel_message(msg)`).  `MediaPipelineB200` offers that

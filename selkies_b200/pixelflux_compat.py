@@ -200,7 +200,7 @@ class ScreenCapture:
                 # selkies-ws-core.js:475-496), under which a Constrained-Baseline 4:2:0 stream decodes as well: the stream stays
                 # 4:2:0 (chroma at half resolution) instead of the capture failing.
                 import warnings
-                warnings.warn("h264_fullcolor: the B200 pipeline encodes 4:2:0 (Constrained Baseline); the stream decodes under the 4:4:4 decoder "
+                warnings.warn("h264_fullcolor: this pipeline encodes 4:2:0 (Constrained Baseline); the stream decodes under the 4:4:4 decoder "
                               "configuration the client selects, with chroma at half resolution", RuntimeWarning, stacklevel=2)
             w, h = int(settings.capture_width), int(settings.capture_height)
             w -= w & 1

@@ -47,7 +47,9 @@ class Session:
         s.gop, s.slice_rows, s.header_mode, s.ring_slots, s.flags = gop, slice_rows, header_mode, ring_slots, flags
         s.paintover_trigger_frames, s.paintover_crf, s.stripe_rows = paintover_trigger_frames, paintover_crf, stripe_rows
         s.paintover_burst_frames, s.idr_slice_mbs = paintover_burst_frames, idr_slice_mbs
-        self._cb = N.FRAME_CB(self._callback)        # keep alive for the lifetime of the handle
+        # keep alive for the lifetime of the handle.  With nothing to deliver to Python the library gets no callback at all: a
+        # ctypes callback takes the GIL on the output thread for every picture, which costs the submitting thread its pace.
+        self._cb = N.FRAME_CB(self._callback) if (on_frame is not None or collect) else N.FRAME_CB()
         h = C.c_void_p()
         N.check(self._lib.b2v_create(C.byref(s), self._cb, None, C.byref(h)))
         self._h = h

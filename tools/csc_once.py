@@ -1,5 +1,4 @@
-"""A dozen 4K CSC launches over distinct resident frames (CSC-only session) — the target of bench.py's live ncu traffic probe
-and of the `ncu --set full` captures under profiles/.  CSC_KERNEL=ldg|tma1|tma2 selects the kernel (default: the library's)."""
+"""A dozen 4K CSC launches over distinct resident frames (CSC-only session), as a target for a profiler.  CSC_KERNEL=ldg|tma1|tma2 selects the kernel (default: the library's)."""
 import os
 import sys
 

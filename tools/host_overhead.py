@@ -10,8 +10,7 @@ from tests import synth
 W, H = 3840, 2160
 frames = [synth.desktop(W, H, t) for t in range(4)]
 for flags, name in ((0, "plain"), (N.B2V_FLAG_TIMING, "timing")):
-    with Session(W, H, rc_mode=N.B2V_RC_CBR, bitrate_kbps=20000, ring_slots=8, flags=flags, collect=False) as s:
-        s._on_frame = lambda fptr: None
+    with Session(W, H, rc_mode=N.B2V_RC_CBR, bitrate_kbps=20000, ring_slots=8, flags=flags, collect=False, on_frame=lambda fptr: None) as s:
         for i, f in enumerate(frames):
             s.resident_upload(i, f)
         for k in range(32):

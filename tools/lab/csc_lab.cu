@@ -1,5 +1,5 @@
 // csc_lab.cu — standalone timing harness for the CSC kernels (tools only; not part of libb2video.so).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -DCSC_TRACE -o tools/lab/csc_lab tools/lab/csc_lab.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -DCSC_TRACE -o tools/lab/csc_lab tools/lab/csc_lab.cu
 // Run on the GPU box: tools/lab/csc_lab [w h]
 #include <algorithm>
 #include <cstdio>
@@ -74,7 +74,7 @@ int main(int argc, char** argv) {
     for (int mode = 1; mode <= 2; mode++) {
       cudaMemset(d_tr, 0, MAXC * 4 * 8);
       cudaDeviceSynchronize();
-      k_pollute<<<148 * 8, 256, 0, st>>>(pol, pol_bytes / 16);
+      k_pollute<<<prop.multiProcessorCount * 8, 256, 0, st>>>(pol, pol_bytes / 16);
       if (mode == 2) { cudaStreamSynchronize(st); }
       launch_csc(params(5), prop.multiProcessorCount, st);
       cudaStreamSynchronize(st);

@@ -1,5 +1,5 @@
 // read_lab.cu — what does a pure 33 MB read cost on this GPU?  (floor for the CSC kernel's input side)
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/lab/read_lab tools/lab/read_lab.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/lab/read_lab tools/lab/read_lab.cu
 #include <cstdio>
 #include <cstdint>
 #include <vector>
@@ -67,12 +67,13 @@ int main() {
     printf("%-28s burst %.2f us/launch (%.0f GB/s read)   in-kernel span %.2f us (%.0f GB/s)  %s\n", name, ms * 1e3 / 200, fb / (ms * 1e-3 / 200) * 1e-9, span / 16, fb / (span / 16 * 1e-6) * 1e-9, cudaGetErrorString(cudaGetLastError()));
   };
   const size_t n16 = fb / 16;
-  for (int ctas : {148, 296, 592, 1184, 2368}) {
+  int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  for (int ctas : {sms, 2 * sms, 4 * sms, 8 * sms, 16 * sms}) {
     char nm[64];
     snprintf(nm, 64, "read U4 %d x 256", ctas); run(nm, [&](int i, unsigned long long* t) { k_read<4><<<ctas, 256>>>(in[i], n16, sink, t); });
     snprintf(nm, 64, "read U8 %d x 256", ctas); run(nm, [&](int i, unsigned long long* t) { k_read<8><<<ctas, 256>>>(in[i], n16, sink, t); });
   }
-  for (int ctas : {296, 592, 1184}) {
+  for (int ctas : {2 * sms, 4 * sms, 8 * sms}) {
     char nm[64];
     snprintf(nm, 64, "read U8 %d x 512", ctas); run(nm, [&](int i, unsigned long long* t) { k_read<8><<<ctas, 512>>>(in[i], n16, sink, t); });
     snprintf(nm, 64, "read+write U4 %d x 256", ctas); run(nm, [&](int i, unsigned long long* t) { k_read_write<4><<<ctas, 256>>>(in[i], n16, dst, t); });

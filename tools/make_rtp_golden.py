@@ -1,6 +1,6 @@
 """Generate tests/golden/rtp_h264_golden.json from the UNMODIFIED reference packetiser.
 
-Runs only in the build container (needs /root/reference).  The reference module
+Needs a checkout of the reference project: REF_ROOT=<selkies checkout> python tools/make_rtp_golden.py.  The reference module
 src/selkies/webrtc/codecs/h264.py imports PyAV and sibling modules that are absent here, but its packetiser
 (`H264Encoder._split_bitstream / _packetize / _packetize_fu_a / _packetize_stap_a`, h264.py:165-279) is pure
 Python: the script stubs the unused imports, executes the reference file as-is and records, for a set of
@@ -15,7 +15,7 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/src/selkies/webrtc/codecs/h264.py"
+REF = os.path.join(os.environ.get("REF_ROOT", "."), "src", "selkies", "webrtc", "codecs", "h264.py")
 
 
 def load_reference():

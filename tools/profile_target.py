@@ -1,4 +1,4 @@
-"""Short 4K run of the headline workload for ncu (profiles/README.md lists the command lines):
+"""Short 4K run of the headline workload, as a target for a profiler:
 python tools/profile_target.py [n_pictures] [gop]   — CBR 20 Mbit/s, inputs resident, two-stream schedule as in bench.py."""
 import os
 import sys
