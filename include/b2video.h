@@ -162,7 +162,14 @@ int   b2v_flush(void* h);                                /* wait until every sub
 
 /* ---- live control: ScreenCapture.update_framerate (media_pipeline.py:236),
  *      update_video_bitrate (:195), request_idr_frame (:244); set_resolution is
- *      WebRTCApp.on_resize_handler → width/height (webrtc_mode.py:383-426). --- */
+ *      WebRTCApp.on_resize_handler → width/height (webrtc_mode.py:383-426).
+ * When a call takes effect: every setting is read when a picture is submitted, so a control call made after submit k and
+ * before submit k+1 applies from picture k+1 on, whether or not pictures are still in flight; nothing already submitted
+ * changes.  b2v_request_idr makes picture k+1 an IDR; with b2v_set_gop(frames > 0), picture k+1 is an IDR when
+ * `frames` or more pictures, the last IDR included, were coded since that IDR.  b2v_set_resolution first drains the pictures in flight, then restarts the encoder:
+ * picture k+1 is an IDR with parameter sets of the new size, the rate controller starts afresh, frame ids continue.  In CBR
+ * mode the controller sees a new bitrate or frame rate as a new per-picture target (bitrate * 1000 / fps bits); its QP
+ * decisions reach the pictures two after the one they were made from. --- */
 int  b2v_set_framerate(void* h, double fps);
 int  b2v_set_bitrate_kbps(void* h, int32_t kbps);
 int  b2v_set_qp(void* h, int32_t qp);                    /* CQP mode (restart-free set_crf) */

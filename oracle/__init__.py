@@ -162,6 +162,15 @@ class RefEncoder:
     def last_qp(self):
         return self.L.b2v_ref_enc_last_qp(self.h)
 
+    def rc_state(self) -> dict:
+        """The rate-control / paint-over record written after the last picture: fullness (bits), qp (decided for a later
+        picture), static_run, remaining (paint-over pictures still to schedule), paint, debt (the debt rule raised the QP)."""
+        v = np.zeros(6, np.int64)
+        self.L.b2v_ref_enc_rc_state.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+        if self.L.b2v_ref_enc_rc_state(self.h, v.ctypes.data_as(C.POINTER(C.c_int64))) != 0:
+            raise ValueError("no picture encoded yet")
+        return dict(zip(("fullness", "qp", "static_run", "remaining", "paint", "debt"), (int(x) for x in v)))
+
     def close(self):
         if self.h:
             self.L.b2v_ref_enc_destroy(self.h)

@@ -110,7 +110,7 @@ typedef struct {
   int frame_num, idr_count;
   /* rate controller / paint-over scheduler: fb[k & 1] is the feedback record written after picture k; picture k is coded from
    * fb[k & 1] as it stood BEFORE that, i.e. the state after picture k-2 (see rc_step) */
-  struct rcfb { int32_t qp, static_run, remaining, paint; int64_t fullness, X; } fb[2];
+  struct rcfb { int32_t qp, static_run, remaining, paint, debt; int64_t fullness, X; } fb[2];
   int64_t pic;            /* pictures encoded so far */
   int paint_trigger, paint_qp, paint_burst;   /* paint-over: `paint_burst` finer pictures after `paint_trigger` all-skipped pictures */
   int last_qp; int64_t last_bits;
@@ -1128,6 +1128,7 @@ static int rc_frame_qp(const enc_t* e, const struct rcfb* fb, int idr, int rc_mo
 static void rc_step(const enc_t* e, struct rcfb* out, const struct rcfb* prev, const struct rcfb* used, int64_t bits, int qp_used,
                     int idr, int coded, int rc_mode, int64_t target) {
   struct rcfb n = *prev;
+  n.debt = 0;
   const int was_paint = e->paint_trigger > 0 && !idr && used->paint;
   /* paint-over scheduler: count all-skipped pictures; at `paint_trigger` schedule `paint_burst` pictures at the paint-over QP
    * (each step schedules the picture two ahead); real motion cancels what is left of the burst */
@@ -1173,7 +1174,7 @@ static void rc_step(const enc_t* e, struct rcfb* out, const struct rcfb* prev, c
       /* debt: spikes the two-picture rule lets through (a scroll that restarts every N pictures, recurring cuts) pile up in the
        * bucket; while it holds more than RC_DEBT_PICTURES pictures' worth, a picture that coded anything makes the quantiser one
        * step coarser whatever the last two pictures say — and (rule above) it gets finer again only once the bucket is empty */
-      if (full > RC_DEBT_PICTURES * T && coded && qt <= qp_used) qt = qp_used + 1;
+      if (full > RC_DEBT_PICTURES * T && coded && qt <= qp_used) { qt = qp_used + 1; n.debt = 1; }
       q = clip3(base - 2, base + 4, qt);
     }
     n.qp = clip3(RC_QP_MIN, RC_QP_MAX, q);
@@ -1213,6 +1214,15 @@ int b2v_ref_enc_coded_w(void* h) { return ((enc_t*)h)->cw; }
 int b2v_ref_enc_coded_h(void* h) { return ((enc_t*)h)->ch; }
 const uint8_t* b2v_ref_enc_recon(void* h) { enc_t* e = (enc_t*)h; return e->recon[e->cur]; }
 int b2v_ref_enc_last_qp(void* h) { return ((enc_t*)h)->last_qp; }
+/* the feedback record written after the last picture (test hook: which rate-control and paint-over branches a stream reaches):
+ * out = {fullness, qp, static_run, remaining, paint, debt}; returns 0, or -1 before the first picture */
+int b2v_ref_enc_rc_state(void* h, int64_t* out) {
+  enc_t* e = (enc_t*)h;
+  if (e->pic == 0) return -1;
+  const struct rcfb* r = &e->fb[(e->pic - 1) & 1];
+  out[0] = r->fullness; out[1] = r->qp; out[2] = r->static_run; out[3] = r->remaining; out[4] = r->paint; out[5] = r->debt;
+  return 0;
+}
 void b2v_ref_enc_set_paintover(void* h, int trigger_frames, int qp) { enc_t* e = (enc_t*)h; e->paint_trigger = trigger_frames; e->paint_qp = qp; }
 /* slices of IDR pictures: n > 0 macroblocks per slice inside a row, n < 0 slices of slice_rows whole rows as in P pictures, 0 = the default rule */
 void b2v_ref_enc_set_idr_slice_mbs(void* h, int n) {

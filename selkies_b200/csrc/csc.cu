@@ -450,6 +450,20 @@ void* csc_make_tensor_map(const uint8_t* d_bgra, int w, int h, int stride) {
 }
 void csc_free_tensor_map(void* d) { if (d) cudaFree(d); }
 
+// Opt-in dynamic shared memory above 48 KB.  cudaFuncSetAttribute applies to the CURRENT device only, so the size already
+// granted is remembered per device (a session on a second GPU needs its own call), and submitters of several sessions may
+// get here at once: the record is guarded.
+constexpr int kAttrDevices = 64;
+static std::mutex g_attr_mu;
+static int g_attr_tma[kAttrDevices], g_attr_scaled[kAttrDevices];
+static void opt_in_smem(const void* fn, int* granted, int smem) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lk(g_attr_mu);
+  if (dev >= 0 && dev < kAttrDevices && smem <= granted[dev]) return;
+  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess && dev >= 0 && dev < kAttrDevices) granted[dev] = smem;
+}
+
 int launch_csc(const CscParams& p, int sm_count, cudaStream_t st) {
   csc_env_once();
   const bool fast = p.tx == nullptr && p.ty == nullptr && p.dst_w == p.src_w && p.dst_h == p.src_h && p.coded_w == p.dst_w &&
@@ -457,8 +471,7 @@ int launch_csc(const CscParams& p, int sm_count, cudaStream_t st) {
                     ((uintptr_t)p.out_y % 4) == 0 && ((uintptr_t)p.out_uv % 4) == 0;
   if (fast && p.matrix == 0 && g_csc_tma && p.tmap && (p.src_h % 2) == 0 && p.coded_h >= p.src_h) {
     const int stages = g_csc_tma_stages, smem = stages * TMA_TILE_BYTES;
-    static int attr_smem = 0;
-    if (smem > attr_smem) { cudaFuncSetAttribute(csc_bgra_nv12_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_smem = smem; }
+    opt_in_smem((const void*)csc_bgra_nv12_tma, g_attr_tma, smem);
     const int tiles_x = (p.src_w + TMA_TW - 1) / TMA_TW, tiles_y = (p.src_h + TMA_TH - 1) / TMA_TH, n_tiles = tiles_x * tiles_y;
     int grid = sm_count * g_csc_tma_ctas_per_sm;
     if (grid > n_tiles) grid = n_tiles;
@@ -501,8 +514,7 @@ int launch_csc(const CscParams& p, int sm_count, cudaStream_t st) {
       const int fw_cap = (int)((fw + 3) & ~3LL), fh_cap = (int)fh;
       const long long smem = (long long)fw_cap * fh_cap * 4;
       if (smem <= 96 * 1024) {
-        static int attr = 0;
-        if (smem > 48 * 1024 && smem > attr) { cudaFuncSetAttribute(csc_bgra_nv12_scaled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = (int)smem; }
+        if (smem > 48 * 1024) opt_in_smem((const void*)csc_bgra_nv12_scaled, g_attr_scaled, (int)smem);
         dim3 grid((p.coded_w + SC_TW - 1) / SC_TW, (p.coded_h + SC_TH - 1) / SC_TH);
         csc_bgra_nv12_scaled<<<grid, SC_THREADS, (size_t)smem, st>>>(p, fw_cap, fh_cap);
         return 1;

@@ -116,6 +116,10 @@ class Session:
         self.width, self.height = width, height
         self.dst_width, self.dst_height = dst_width or width, dst_height or height
 
+    def set_gop(self, frames: int) -> None:
+        """Key-frame distance in pictures from the next submit on (<= 0: key frames only on request)."""
+        N.check(self._lib.b2v_set_gop(self._h, int(frames)))
+
     def request_idr(self) -> None:
         N.check(self._lib.b2v_request_idr(self._h))
 

@@ -67,6 +67,18 @@ def test_csc_scaled_tiled_bit_exact_large(sw, sh, dw, dh):
     assert np.array_equal(uv, ouv)
 
 
+@pytest.mark.parametrize("sw,sh,dw,dh", [(1920, 1080, 320, 180), (7680, 4320, 1280, 720)])
+def test_csc_scaled_tiled_opt_in_shared_memory_tier(sw, sh, dw, dh):
+    """Downscales by 6: the tiled kernel's source footprint is 392 x 51 pixels (80 KB), above the 48 KB a launch gets without
+    the opt-in attribute."""
+    f = synth.noise(sw, sh, 9)
+    with Session(sw, sh, dst_width=dw, dst_height=dh, flags=N.B2V_FLAG_NO_ENCODE) as s:
+        y, uv = s.csc_nv12(f)
+    oy, ouv = oracle.csc_nv12(f, dst_w=dw, dst_h=dh)
+    assert np.array_equal(y, oy)
+    assert np.array_equal(uv, ouv)
+
+
 def test_csc_scaled_close_to_cv2_resize():
     """SURVEY §8c.3: the fused bilinear scale stays within rounding distance of cv2.resize(INTER_LINEAR) followed by the 1:1
     conversion (cv2 blends with 11-bit weights, this spec with 8-bit ones: +-1 per channel before the matrix)."""
