@@ -15,7 +15,6 @@ struct EncoderConfig {
   int slice_rows;          // macroblock rows per slice
   int stripe_rows;         // macroblock rows per band (multiple of slice_rows); 0 = full-frame
   int idr_slice_mbs;       // IDR pictures: macroblocks per slice inside a row (needs slice_rows == 1); 0 = default rule, < 0 = whole rows
-  int sm_count;
 };
 
 // 64-byte record the pack kernel writes in front of the access unit in HBM; travels to the host

@@ -17,7 +17,7 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(b2v_[a-z0-9_]+)\s*\(", src)) - {"b2v_cb"})
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_4():
     from selkies_b200 import _native
     lib = ctypes.CDLL(_native.LIB_PATH)
     declared = header_symbols()
@@ -26,7 +26,9 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in include/b2video.h but not exported"
     bound = {n for n, _, _ in _native.SYMBOLS}
     assert set(declared) == bound, set(declared) ^ bound
-    assert _native.lib().b2v_abi_version() == 3          # no compute call: safe without a GPU
+    header_abi = re.search(r"#define\s+B2V_ABI_VERSION\s+(\d+)", open(os.path.join(ROOT, "include", "b2video.h")).read())
+    assert header_abi and int(header_abi.group(1)) == 4
+    assert _native.lib().b2v_abi_version() == 4          # no compute call: safe without a GPU
 
 
 def test_struct_layouts_match_header():
