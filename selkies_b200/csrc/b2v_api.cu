@@ -7,11 +7,12 @@
 //
 // Per-frame flow (four streams, events in between; nothing on the host blocks except ring back-pressure):
 //   st_copy : cudaMemcpyAsync  pinned slot -> device BGRA slot                      (a) ingest
-//   st_enc  : fused CSC(+scale) -> NV12 cur ; analysis (k_intra_rows / k_inter_mb)          (b),(c)
+//   st_enc  : fused CSC(+scale) -> NV12 cur ; analysis (k_intra_rows / k_inter_mb), or the whole JPEG encode   (b),(c)
 //   st_pack : entropy coding of the same picture (k_cavlc_mb -> k_slice_build, which runs the rate-control step -> k_pack_au)
 //             -> AU in HBM, overlapping the analysis of the next picture on st_enc (h264_encoder.cu)
 //   st_out  : cudaMemcpyAsync  AU head (size + first chunk) -> pinned output slot
-//   output thread: waits the D2H event, fetches the tail of oversized AUs, runs the callback in order.
+//   output thread: waits the D2H event, fetches the tail of oversized AUs, runs the callback in order: one call per band
+//   that carries data (striped H.264, JPEG stripes); a full frame is delivered as the one band of the picture.
 #include <condition_variable>
 #include <cstdarg>
 #include <cstdio>
@@ -95,7 +96,7 @@ struct Session {
   int n_slots = 4;
   uint8_t* host_slot[kMaxSlots] = {};
   uint8_t* dev_slot[kMaxSlots] = {};
-  cudaEvent_t ev_h2d[kMaxSlots] = {}, ev_csc[kMaxSlots] = {};
+  cudaEvent_t ev_h2d[kMaxSlots] = {};
   uint8_t slot_state[kMaxSlots] = {};   // SLOT_*
   size_t frame_bytes = 0;
   // resident frames (bench `value` leg)
@@ -113,8 +114,7 @@ struct Session {
   uint8_t* h_out[kMaxSlots] = {};
   cudaEvent_t ev_enc[kMaxSlots] = {}, ev_out[kMaxSlots] = {};
   bool out_free[kMaxSlots] = {};
-  size_t au_cap = 0;
-  int au_data_off = 64, n_bands = 0;   // bytes in front of the first NAL in d_au (AuHeader [+ band table]); bands when striped
+  AuLayout lay{};                // shape of d_au[i] (the encoder's); all zero without encoding
   int out_next = 0;
   int ring_next = 0;
   cudaEvent_t ev_timer[2] = {};
@@ -128,8 +128,8 @@ struct Session {
   int bitrate_kbps = 8000;
   int qp_fixed = 26;
 
-  // timing events (B2V_FLAG_TIMING): 8 per output slot, read back by the output thread
-  cudaEvent_t ev_t[kMaxSlots][8] = {};
+  // timing events (B2V_FLAG_TIMING): 6 per output slot, read back by the output thread
+  cudaEvent_t ev_t[kMaxSlots][6] = {};
 
   b2v_cb cb = nullptr; void* user = nullptr;
   std::mutex mu;                 // guards everything below + sequencing state
@@ -145,6 +145,9 @@ struct Session {
 };
 
 int round16(int v) { return (v + 15) & ~15; }
+
+// frame sizes a session takes, source and encoded alike: even, 16..7680 x 16..4320
+bool size_ok(int w, int h) { return w >= 16 && h >= 16 && w <= 7680 && h <= 4320 && !(w & 1) && !(h & 1); }
 
 int alloc_geometry(Session* s) {
   // (re)allocate everything that depends on the frame size
@@ -174,13 +177,7 @@ int alloc_geometry(Session* s) {
     jc.paint_trigger = s->cfg.paintover_trigger_frames > 0 ? s->cfg.paintover_trigger_frames : 0;
     int rc = jpeg_create(&jc, &s->jenc);
     if (rc) return fail(rc, "jpeg_create failed: %s", jpeg_last_error());
-    s->au_cap = jpeg_au_capacity(s->jenc);
-    s->au_data_off = jpeg_au_data_offset(s->jenc);
-    s->n_bands = jpeg_stripe_count(s->jenc);
-    for (int i = 0; i < s->n_slots; i++) {
-      CK(cudaMalloc((void**)&s->d_au[i], s->au_cap));
-      CK(cudaHostAlloc((void**)&s->h_out[i], s->au_cap + kOutHead, cudaHostAllocDefault));
-    }
+    s->lay = jpeg_layout(s->jenc);
   } else if (s->encode) {
     EncoderConfig ec{};
     ec.width = s->dst_w; ec.height = s->dst_h; ec.coded_w = s->coded_w; ec.coded_h = s->coded_h;
@@ -189,15 +186,15 @@ int alloc_geometry(Session* s) {
     ec.idr_slice_mbs = s->cfg.idr_slice_mbs;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
-    s->au_cap = encoder_au_capacity(s->enc);
-    s->au_data_off = encoder_au_data_offset(s->enc);
-    s->n_bands = encoder_band_count(s->enc);
-    for (int i = 0; i < s->n_slots; i++) {
-      CK(cudaMalloc((void**)&s->d_au[i], s->au_cap));
-      CK(cudaHostAlloc((void**)&s->h_out[i], s->au_cap + kOutHead, cudaHostAllocDefault));
-    }
+    s->lay = encoder_layout(s->enc);
   }
-  for (int i = 0; i < s->n_slots; i++) s->out_free[i] = true;
+  for (int i = 0; i < s->n_slots; i++) {
+    if (s->encode) {
+      CK(cudaMalloc((void**)&s->d_au[i], s->lay.cap));
+      CK(cudaHostAlloc((void**)&s->h_out[i], s->lay.cap + kOutHead, cudaHostAllocDefault));
+    }
+    s->out_free[i] = true;
+  }
   return 0;
 }
 
@@ -229,9 +226,117 @@ CscParams csc_params(Session* s, const uint8_t* d_bgra, int stride, uint8_t* d_n
   return p;
 }
 
+// Waits for the access unit of job j and checks it; fetches the tail of an oversized one.  Returns its size in bytes, 0 when
+// the picture failed or nothing was encoded (B2V_FLAG_NO_ENCODE).
+int wait_au(Session* s, const Job& j, int64_t* ns_event, bool* slept) {
+  const int64_t tw = now_ns();
+  const cudaError_t se = wait_event_polling(s->encode ? s->ev_out[j.out_idx] : s->ev_enc[j.out_idx], slept);
+  *ns_event = now_ns() - tw;
+  if (!s->encode) return 0;
+  uint8_t* base = s->h_out[j.out_idx];
+  const AuHeader* ah = (const AuHeader*)base;     // device wrote the AU header at the start of the buffer
+  const int size = ah->size;
+  const size_t doff = (size_t)s->lay.data_off;
+  if (se != cudaSuccess || size < 0 || (size_t)size + doff > s->lay.cap || ah->overflow) {
+    // a kernel faulted or produced an impossible access unit: fail loudly — nothing is delivered, every later
+    // call on this session returns B2V_ECUDA with this message
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (!s->failed) snprintf(s->fail_msg, sizeof s->fail_msg, "encode pipeline failed on frame %d: %s (size %d, overflow %d)", j.frame_id,
+                             se != cudaSuccess ? cudaGetErrorString(se) : "invalid access unit", size, ah->overflow);
+    s->failed = true;
+    return 0;
+  }
+  if ((size_t)size + doff > kFirstChunk && size > 0) {   // oversized AU: fetch the tail
+    size_t have = kFirstChunk;
+    cudaMemcpyAsync(base + have, s->d_au[j.out_idx] + have, doff + (size_t)size - have, cudaMemcpyDeviceToHost, s->st_out);
+    cudaStreamSynchronize(s->st_out);
+    std::lock_guard<std::mutex> lk(s->mu);
+    s->stats.d2h_bytes += (int64_t)(doff + size - have);
+  }
+  return size;
+}
+
+// B2V_FLAG_TIMING / B2V_FLAG_TIMING_CSC: adds the stage times of job j (and the CSC's device stamps, when it has an AU) to the stats
+void add_timing(Session* s, const Job& j, bool have_au) {
+  cudaEvent_t* ev = s->ev_t[j.out_idx];
+  float ms[6] = {0, 0, 0, 0, 0, 0};
+  cudaEventElapsedTime(&ms[0], ev[0], ev[1]);
+  const bool stages = s->encode && !s->timing_csc_only;
+  if (stages) {
+    for (int k = 1; k < 5; k++) cudaEventElapsedTime(&ms[k], ev[k], ev[k + 1]);
+    cudaEventElapsedTime(&ms[5], ev[0], ev[5]);
+  } else ms[5] = ms[0];
+  std::lock_guard<std::mutex> lk(s->mu);
+  s->stats.ms_csc += ms[0]; s->stats.n_csc++;
+  if (have_au) {
+    const AuHeader* ah = (const AuHeader*)s->h_out[j.out_idx];
+    if (ah->csc_t1 > ah->csc_t0 && ah->csc_t0 != 0) { s->stats.ms_csc_device += (double)(ah->csc_t1 - ah->csc_t0) * 1e-6; s->stats.n_csc_device++; }
+  }
+  if (stages) {
+    if (j.is_key) { s->stats.ms_intra += ms[1]; s->stats.n_intra++; }
+    else { s->stats.ms_inter += ms[1]; s->stats.n_inter++; }
+    s->stats.ms_cavlc += ms[2]; s->stats.n_cavlc++;
+    s->stats.ms_slice += ms[3]; s->stats.n_slice++;
+    s->stats.ms_pack += ms[4]; s->stats.n_pack++;
+  }
+  s->stats.ms_total_gpu += ms[5];
+}
+
+// pixelflux's 10-byte stripe header: 04 | is_key | frame_id u16be | y_start u16be | width u16be | height u16be
+void put_pixelflux_header(uint8_t* h, const Job& j, int y0, int bh) {
+  h[0] = 0x04; h[1] = j.is_key ? 1 : 0;
+  h[2] = (uint8_t)(j.frame_id >> 8); h[3] = (uint8_t)j.frame_id;
+  h[4] = (uint8_t)(y0 >> 8); h[5] = (uint8_t)y0;
+  h[6] = (uint8_t)(j.hdr_w >> 8); h[7] = (uint8_t)j.hdr_w;
+  h[8] = (uint8_t)(bh >> 8); h[9] = (uint8_t)bh;
+}
+
+// Runs the callback once per band of job j's access unit (`size` bytes) that carries data, in picture order; a full frame is the
+// one band {off 0, size, coded} of height hdr_h.  The band table is copied into `tab` first: the header of band k is written
+// over the tail of band k-1 (already delivered) or the table slack (the AuHeader, already read, for a full frame).
+// Returns the bytes delivered, headers included.
+int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab, int64_t* ns_cb) {
+  uint8_t* base = s->h_out[j.out_idx];
+  uint8_t* au = base + s->lay.data_off;
+  const int qp = ((const AuHeader*)base)->qp;
+  int rows = j.hdr_h;
+  if (s->lay.n_bands == 0) {
+    tab.assign(1, BandEntry{0, size, 1, 0});
+  } else {
+    tab.resize(s->lay.n_bands);
+    memcpy(tab.data(), base + sizeof(AuHeader), sizeof(BandEntry) * s->lay.n_bands);
+    rows = s->lay.band_rows * 16;
+  }
+  const bool hdr = s->cfg.header_mode == B2V_HDR_PIXELFLUX;
+  int64_t bytes = 0;
+  for (int b = 0; b < (int)tab.size(); b++) {
+    const BandEntry& be = tab[b];
+    if (!be.coded || be.size <= 0 || (long long)be.off + be.size > size) continue;
+    const int y0 = b * rows, bh = (y0 + rows <= j.hdr_h) ? rows : j.hdr_h - y0;
+    b2v_frame f{};
+    f.data = au + be.off; f.size = be.size;
+    if (hdr && s->jpeg) {
+      // JPEG stripe: frame_id u16be | y_start u16be | JFIF file (the reference prepends 03 00, selkies.py:3118; the client reads the
+      // frame id at offset 2 and y_start at offset 4, selkies-ws-core.js:3166-3172)
+      uint8_t* h = au + be.off - 4;
+      h[0] = (uint8_t)(j.frame_id >> 8); h[1] = (uint8_t)j.frame_id; h[2] = (uint8_t)(y0 >> 8); h[3] = (uint8_t)y0;
+      f.data = h; f.size += 4;
+    } else if (hdr) {
+      put_pixelflux_header(au + be.off - 10, j, y0, bh);
+      f.data = au + be.off - 10; f.size += 10;
+    }
+    f.frame_id = j.frame_id; f.is_key = j.is_key; f.qp = qp; f.pts90k = j.pts; f.capture_ns = j.capture_ns;
+    f.y_start = y0; f.height = bh;
+    bytes += f.size;
+    if (s->cb) { const int64_t tc = now_ns(); s->cb(&f, s->user); *ns_cb += now_ns() - tc; }
+  }
+  return bytes;
+}
+
 void output_loop(Session* s) {
   cudaSetDevice(s->device);
   prctl(PR_SET_TIMERSLACK, 1000UL, 0, 0, 0);     // this thread's short sleeps (wait_event_polling) are not rounded up by 50 us
+  std::vector<BandEntry> tab;                    // deliver()'s copy of the band table, kept across pictures
   for (;;) {
     Job j;
     {
@@ -244,122 +349,17 @@ void output_loop(Session* s) {
       if (s->jobs.empty()) { if (s->stopping) return; continue; }
       j = s->jobs.front(); s->jobs.pop_front();
     }
-    int size = 0, qp = 0;
-    const uint8_t* data = nullptr;
-    int64_t ns_event = 0, ns_cb = 0; bool slept = false;
-    if (s->encode) {
-      const int64_t tw = now_ns();
-      const cudaError_t se = wait_event_polling(s->ev_out[j.out_idx], &slept);
-      ns_event = now_ns() - tw;
-      uint8_t* base = s->h_out[j.out_idx];
-      const AuHeader* ah = (const AuHeader*)base;     // device wrote the AU header at the start of the buffer
-      size = ah->size; qp = ah->qp;
-      const size_t doff = (size_t)s->au_data_off;
-      if (se != cudaSuccess || size < 0 || (size_t)size + doff > s->au_cap || ah->overflow) {
-        // a kernel faulted or produced an impossible access unit: fail loudly — nothing is delivered, every later
-        // call on this session returns B2V_ECUDA with this message
-        std::lock_guard<std::mutex> lk(s->mu);
-        if (!s->failed) snprintf(s->fail_msg, sizeof s->fail_msg, "encode pipeline failed on frame %d: %s (size %d, overflow %d)", j.frame_id,
-                                 se != cudaSuccess ? cudaGetErrorString(se) : "invalid access unit", size, ah->overflow);
-        s->failed = true;
-        size = 0;
-      }
-      if ((size_t)size + doff > kFirstChunk && size > 0) {   // oversized AU: fetch the tail
-        size_t have = kFirstChunk;
-        cudaMemcpyAsync(base + have, s->d_au[j.out_idx] + have, doff + (size_t)size - have, cudaMemcpyDeviceToHost, s->st_out);
-        cudaStreamSynchronize(s->st_out);
-        std::lock_guard<std::mutex> lk(s->mu);
-        s->stats.d2h_bytes += (int64_t)(doff + size - have);
-      }
-      uint8_t* au = base + doff;
-      data = au;
-      if (s->n_bands == 0 && s->cfg.header_mode == B2V_HDR_PIXELFLUX) {
-        // 10-byte stripe header written into the slack in front of the AU (AuHeader is 64 bytes; already consumed)
-        uint8_t* h = au - 10;
-        h[0] = 0x04; h[1] = j.is_key ? 1 : 0;
-        h[2] = (uint8_t)(j.frame_id >> 8); h[3] = (uint8_t)j.frame_id;
-        h[4] = 0; h[5] = 0;
-        h[6] = (uint8_t)(j.hdr_w >> 8); h[7] = (uint8_t)j.hdr_w;
-        h[8] = (uint8_t)(j.hdr_h >> 8); h[9] = (uint8_t)j.hdr_h;
-        data = h; size += 10;
-      }
-    } else {
-      const int64_t tw = now_ns();
-      wait_event_polling(s->ev_enc[j.out_idx], &slept);
-      ns_event = now_ns() - tw;
-    }
-    if (j.timing) {
-      cudaEvent_t* ev = s->ev_t[j.out_idx];
-      float ms[6] = {0, 0, 0, 0, 0, 0};
-      cudaEventElapsedTime(&ms[0], ev[0], ev[1]);
-      const bool stages = s->encode && !s->timing_csc_only;
-      if (stages) {
-        for (int k = 1; k < 5; k++) cudaEventElapsedTime(&ms[k], ev[k], ev[k + 1]);
-        cudaEventElapsedTime(&ms[5], ev[0], ev[5]);
-      } else ms[5] = ms[0];
-      std::lock_guard<std::mutex> lk(s->mu);
-      s->stats.ms_csc += ms[0]; s->stats.n_csc++;
-      if (s->encode && size > 0) {
-        const AuHeader* ah2 = (const AuHeader*)s->h_out[j.out_idx];
-        if (ah2->csc_t1 > ah2->csc_t0 && ah2->csc_t0 != 0) { s->stats.ms_csc_device += (double)(ah2->csc_t1 - ah2->csc_t0) * 1e-6; s->stats.n_csc_device++; }
-      }
-      if (stages) {
-        if (j.is_key) { s->stats.ms_intra += ms[1]; s->stats.n_intra++; }
-        else { s->stats.ms_inter += ms[1]; s->stats.n_inter++; }
-        s->stats.ms_cavlc += ms[2]; s->stats.n_cavlc++;
-        s->stats.ms_slice += ms[3]; s->stats.n_slice++;
-        s->stats.ms_pack += ms[4]; s->stats.n_pack++;
-      }
-      s->stats.ms_total_gpu += ms[5];
-    }
-    if (s->encode && size > 0 && s->n_bands > 0) {
-      // striped mode: one callback per band that carries data, in picture order.  The band table is copied out first:
-      // the 10-byte header of band k is written over the tail of band k-1 (already delivered) or the table slack.
-      std::vector<BandEntry> tab(s->n_bands);
-      memcpy(tab.data(), s->h_out[j.out_idx] + sizeof(AuHeader), sizeof(BandEntry) * s->n_bands);
-      uint8_t* au = s->h_out[j.out_idx] + s->au_data_off;
-      const int rows = (s->jpeg ? jpeg_stripe_rows(s->jenc) : s->cfg.stripe_rows) * 16;
-      int delivered_bytes = 0;
-      for (int b = 0; b < s->n_bands; b++) {
-        const BandEntry& be = tab[b];
-        if (!be.coded || be.size <= 0 || (long long)be.off + be.size > size) continue;
-        const int y0 = b * rows, bh = (y0 + rows <= j.hdr_h) ? rows : j.hdr_h - y0;
-        b2v_frame f{};
-        f.data = au + be.off; f.size = be.size;
-        if (s->jpeg && s->cfg.header_mode == B2V_HDR_PIXELFLUX) {
-          // JPEG stripe: frame_id u16be | y_start u16be | JFIF file (the reference prepends 03 00, selkies.py:3118; the client reads the
-          // frame id at offset 2 and y_start at offset 4, selkies-ws-core.js:3166-3172)
-          uint8_t* h = au + be.off - 4;
-          h[0] = (uint8_t)(j.frame_id >> 8); h[1] = (uint8_t)j.frame_id; h[2] = (uint8_t)(y0 >> 8); h[3] = (uint8_t)y0;
-          f.data = h; f.size += 4;
-        } else if (s->cfg.header_mode == B2V_HDR_PIXELFLUX) {
-          uint8_t* h = au + be.off - 10;
-          h[0] = 0x04; h[1] = j.is_key ? 1 : 0;
-          h[2] = (uint8_t)(j.frame_id >> 8); h[3] = (uint8_t)j.frame_id;
-          h[4] = (uint8_t)(y0 >> 8); h[5] = (uint8_t)y0;
-          h[6] = (uint8_t)(j.hdr_w >> 8); h[7] = (uint8_t)j.hdr_w;
-          h[8] = (uint8_t)(bh >> 8); h[9] = (uint8_t)bh;
-          f.data = h; f.size += 10;
-        }
-        f.frame_id = j.frame_id; f.is_key = j.is_key; f.qp = qp; f.pts90k = j.pts; f.capture_ns = j.capture_ns;
-        f.y_start = y0; f.height = bh;
-        delivered_bytes += f.size;
-        if (s->cb) { const int64_t tc = now_ns(); s->cb(&f, s->user); ns_cb += now_ns() - tc; }
-      }
-      size = delivered_bytes;
-    } else if (s->cb && s->encode && size > 0) {
-      b2v_frame f{};
-      f.data = data; f.size = size; f.frame_id = j.frame_id; f.is_key = j.is_key; f.qp = qp;
-      f.pts90k = j.pts; f.capture_ns = j.capture_ns; f.y_start = 0; f.height = j.hdr_h;
-      const int64_t tc = now_ns(); s->cb(&f, s->user); ns_cb = now_ns() - tc;
-    }
+    int64_t ns_event = 0, ns_cb = 0, bytes = 0; bool slept = false;
+    const int size = wait_au(s, j, &ns_event, &slept);
+    if (j.timing) add_timing(s, j, size > 0);
+    if (size > 0) bytes = deliver(s, j, size, tab, &ns_cb);
     {
       std::lock_guard<std::mutex> lk(s->mu);
       if (j.in_slot >= 0) s->slot_state[j.in_slot] = SLOT_FREE;
       s->out_free[j.out_idx] = true;
       s->delivered++;
       s->stats.frames_delivered++;
-      s->stats.bytes_out += size;
+      s->stats.bytes_out += bytes;
       if (j.is_key) s->stats.key_frames++;
       s->stats.ns_wait_event += ns_event; s->stats.ns_callback += ns_cb;
       if (ns_event > s->stats.ns_wait_event_max) s->stats.ns_wait_event_max = ns_event;
@@ -440,24 +440,19 @@ int submit_common(Session* s, const uint8_t* d_bgra, int stride, int in_slot, in
   if (ev) cudaEventRecord(ev[0], s->st_enc);
   int nl = launch_csc(cp, s->st_enc);
   if (ev) cudaEventRecord(ev[1], s->st_enc);
-  if (in_slot >= 0) CKS(cudaEventRecord(s->ev_csc[in_slot], s->st_enc));
-  CKS(cudaEventRecord(s->ev_enc[out_idx], s->st_enc));
+  cudaStream_t st_done = s->st_enc;     // where the access unit (without encoding: the NV12 picture) is complete
   if (s->encode && s->jpeg) {
     nl += jpeg_encode(s->jenc, s->d_cur, s->d_au[out_idx], j.is_key, s->st_enc);
-    CKS(cudaEventRecord(s->ev_enc[out_idx], s->st_enc));
-    CKS(cudaStreamWaitEvent(s->st_out, s->ev_enc[out_idx], 0));
-    size_t first = s->au_cap < kFirstChunk ? s->au_cap : kFirstChunk;
-    CKS(cudaMemcpyAsync(s->h_out[out_idx], s->d_au[out_idx], first, cudaMemcpyDeviceToHost, s->st_out));
-    CKS(cudaEventRecord(s->ev_out[out_idx], s->st_out));
-    std::lock_guard<std::mutex> lk(s->mu);
-    s->stats.d2h_bytes += (int64_t)first;
   } else if (s->encode) {
     fp.cur = s->d_cur; fp.au = s->d_au[out_idx]; fp.ev = s->timing_csc_only ? nullptr : ev; fp.csc_ts = cp.ts;
     fp.st_pack = fp.ev ? nullptr : s->st_pack;      // per-stage events need the serial schedule
     nl += encoder_encode(s->enc, &fp, s->st_enc);
-    CKS(cudaEventRecord(s->ev_enc[out_idx], fp.st_pack ? fp.st_pack : s->st_enc));      // the access unit is complete here
+    if (fp.st_pack) st_done = fp.st_pack;
+  }
+  CKS(cudaEventRecord(s->ev_enc[out_idx], st_done));
+  if (s->encode) {
     CKS(cudaStreamWaitEvent(s->st_out, s->ev_enc[out_idx], 0));
-    size_t first = s->au_cap < kFirstChunk ? s->au_cap : kFirstChunk;
+    const size_t first = s->lay.cap < kFirstChunk ? s->lay.cap : kFirstChunk;
     CKS(cudaMemcpyAsync(s->h_out[out_idx], s->d_au[out_idx], first, cudaMemcpyDeviceToHost, s->st_out));
     CKS(cudaEventRecord(s->ev_out[out_idx], s->st_out));
     std::lock_guard<std::mutex> lk(s->mu);
@@ -481,10 +476,9 @@ void release_session(Session* s) {
   free_geometry(s);
   for (int i = 0; i < kMaxSlots; i++) {
     if (s->ev_h2d[i]) cudaEventDestroy(s->ev_h2d[i]);
-    if (s->ev_csc[i]) cudaEventDestroy(s->ev_csc[i]);
     if (s->ev_enc[i]) cudaEventDestroy(s->ev_enc[i]);
     if (s->ev_out[i]) cudaEventDestroy(s->ev_out[i]);
-    for (int k = 0; k < 8; k++) if (s->ev_t[i][k]) cudaEventDestroy(s->ev_t[i][k]);
+    for (cudaEvent_t e : s->ev_t[i]) if (e) cudaEventDestroy(e);
   }
   if (s->ev_timer[0]) cudaEventDestroy(s->ev_timer[0]);
   if (s->ev_timer[1]) cudaEventDestroy(s->ev_timer[1]);
@@ -494,6 +488,40 @@ void release_session(Session* s) {
   if (s->st_out) cudaStreamDestroy(s->st_out);
   if (s->st_pack) cudaStreamDestroy(s->st_pack);
   delete s;
+}
+
+// b2v_bench_csc (burst = false: each launch bracketed by its own event pair, the sum excludes host launch gaps) and
+// b2v_bench_csc_burst (one event pair around all launches)
+int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launch, bool burst) {
+  if (!s || n_resident <= 0 || n_resident > (int)s->resident.size() || iters <= 0 || !ms_per_launch) return fail(B2V_EINVAL, "bad argument");
+  int rc = b2v_flush(s);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> sub(s->submit_mu);
+  CK(cudaSetDevice(s->device));
+  // one NV12 target per resident frame so that reads AND writes cycle through > L2 of memory
+  std::vector<uint8_t*> outs(n_resident, nullptr);
+  size_t ob = (size_t)s->coded_w * s->coded_h * 3 / 2;
+  for (auto& o : outs) CK(cudaMalloc((void**)&o, ob));
+  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, s->resident[i], s->src_w * 4, outs[i]), s->st_enc);   // warm-up
+  CK(cudaStreamSynchronize(s->st_enc));
+  const int pairs = burst ? 1 : iters;
+  std::vector<cudaEvent_t> e0(pairs), e1(pairs);
+  for (int i = 0; i < pairs; i++) { cudaEventCreate(&e0[i]); cudaEventCreate(&e1[i]); }
+  if (burst) cudaEventRecord(e0[0], s->st_enc);
+  for (int i = 0; i < iters; i++) {
+    int k = i % n_resident;
+    if (!burst) cudaEventRecord(e0[i], s->st_enc);
+    launch_csc(csc_params(s, s->resident[k], s->src_w * 4, outs[k]), s->st_enc);
+    if (!burst) cudaEventRecord(e1[i], s->st_enc);
+  }
+  if (burst) cudaEventRecord(e1[0], s->st_enc);
+  CK(cudaStreamSynchronize(s->st_enc));
+  double total = 0;
+  for (int i = 0; i < pairs; i++) { float ms = 0; cudaEventElapsedTime(&ms, e0[i], e1[i]); total += ms; cudaEventDestroy(e0[i]); cudaEventDestroy(e1[i]); }
+  for (auto o : outs) cudaFree(o);
+  CK(cudaGetLastError());
+  *ms_per_launch = (float)(total / iters);
+  return 0;
 }
 
 }  // namespace
@@ -513,10 +541,8 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if (!cfg || !out) return fail(B2V_EINVAL, "null argument");
   int sw = cfg->src_w, sh = cfg->src_h;
   int dw = cfg->dst_w > 0 ? cfg->dst_w : sw, dh = cfg->dst_h > 0 ? cfg->dst_h : sh;
-  if (sw < 16 || sh < 16 || sw > 7680 || sh > 4320 || (sw & 1) || (sh & 1))
-    return fail(B2V_EINVAL, "source size %dx%d unsupported (even, 16..7680 x 16..4320)", sw, sh);
-  if (dw < 16 || dh < 16 || dw > 7680 || dh > 4320 || (dw & 1) || (dh & 1))
-    return fail(B2V_EINVAL, "encoded size %dx%d unsupported", dw, dh);
+  if (!size_ok(sw, sh)) return fail(B2V_EINVAL, "source size %dx%d unsupported (even, 16..7680 x 16..4320)", sw, sh);
+  if (!size_ok(dw, dh)) return fail(B2V_EINVAL, "encoded size %dx%d unsupported", dw, dh);
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(B2V_EINVAL, "device %d out of range (%d devices)", cfg->device, ndev);
@@ -543,12 +569,11 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   cudaStreamCreateWithFlags(&s->st_pack, cudaStreamNonBlocking);
   for (int i = 0; i < kMaxSlots; i++) {
     cudaEventCreateWithFlags(&s->ev_h2d[i], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&s->ev_csc[i], cudaEventDisableTiming);
     // the output thread polls these from user mode (wait_event_polling): no interrupt-driven wait, no spinning core either
     cudaEventCreateWithFlags(&s->ev_enc[i], cudaEventDisableTiming);
     cudaEventCreateWithFlags(&s->ev_out[i], cudaEventDisableTiming);
   }
-  for (int i = 0; i < kMaxSlots; i++) for (int k = 0; k < 8; k++) cudaEventCreate(&s->ev_t[i][k]);
+  for (auto& evs : s->ev_t) for (cudaEvent_t& e : evs) cudaEventCreate(&e);
   cudaEventCreate(&s->ev_timer[0]); cudaEventCreate(&s->ev_timer[1]);
   if (s->timing && (cfg->flags & B2V_FLAG_DEVICE_TIMER)) cudaMalloc((void**)&s->d_csc_ts, sizeof(unsigned long long) * 2 * kMaxSlots);
   int rc = alloc_geometry(s);
@@ -698,8 +723,7 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   if (!s) return fail(B2V_EINVAL, "null handle");
   if (dw <= 0) dw = sw;
   if (dh <= 0) dh = sh;
-  if (sw < 16 || sh < 16 || sw > 7680 || sh > 4320 || (sw & 1) || (sh & 1) || dw < 16 || dh < 16 || dw > 7680 || dh > 4320 || (dw & 1) || (dh & 1))
-    return fail(B2V_EINVAL, "size unsupported");
+  if (!size_ok(sw, sh) || !size_ok(dw, dh)) return fail(B2V_EINVAL, "size unsupported");
   // Submitters are locked out FIRST; then everything in flight drains (the output thread needs `mu`, not `submit_mu`, so it
   // keeps delivering); a producer still holding an acquired slot would be writing into memory about to be freed: refuse.
   std::lock_guard<std::mutex> sub(s->submit_mu);
@@ -788,38 +812,7 @@ int b2v_get_recon(void* h, void* nv12) {
 }
 
 int b2v_bench_csc(void* h, int32_t n_resident, int32_t iters, float* ms_per_launch) {
-  Session* s = (Session*)h;
-  if (!s || n_resident <= 0 || n_resident > (int)s->resident.size() || iters <= 0 || !ms_per_launch) return fail(B2V_EINVAL, "bad argument");
-  int rc = b2v_flush(h);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> sub(s->submit_mu);
-  CK(cudaSetDevice(s->device));
-  // one NV12 target per resident frame so that reads AND writes cycle through > L2 of memory
-  std::vector<uint8_t*> outs(n_resident, nullptr);
-  size_t ob = (size_t)s->coded_w * s->coded_h * 3 / 2;
-  for (auto& o : outs) CK(cudaMalloc((void**)&o, ob));
-  for (int i = 0; i < n_resident; i++) {   // warm-up: one pass over every frame
-    CscParams p = csc_params(s, s->resident[i], s->src_w * 4, outs[i]);
-    launch_csc(p, s->st_enc);
-  }
-  CK(cudaStreamSynchronize(s->st_enc));
-  // each launch is bracketed by its own event pair; the sum excludes host launch gaps
-  std::vector<cudaEvent_t> e0(iters), e1(iters);
-  for (int i = 0; i < iters; i++) { cudaEventCreate(&e0[i]); cudaEventCreate(&e1[i]); }
-  for (int i = 0; i < iters; i++) {
-    int k = i % n_resident;
-    CscParams p = csc_params(s, s->resident[k], s->src_w * 4, outs[k]);
-    cudaEventRecord(e0[i], s->st_enc);
-    launch_csc(p, s->st_enc);
-    cudaEventRecord(e1[i], s->st_enc);
-  }
-  CK(cudaStreamSynchronize(s->st_enc));
-  double total = 0;
-  for (int i = 0; i < iters; i++) { float ms = 0; cudaEventElapsedTime(&ms, e0[i], e1[i]); total += ms; cudaEventDestroy(e0[i]); cudaEventDestroy(e1[i]); }
-  for (auto o : outs) cudaFree(o);
-  CK(cudaGetLastError());
-  *ms_per_launch = (float)(total / iters);
-  return 0;
+  return bench_csc((Session*)h, n_resident, iters, ms_per_launch, false);
 }
 
 int b2v_timer_start(void* h) {
@@ -848,28 +841,7 @@ int b2v_timer_stop(void* h, float* ms) {
 }
 
 int b2v_bench_csc_burst(void* h, int32_t n_resident, int32_t iters, float* ms_per_launch) {
-  Session* s = (Session*)h;
-  if (!s || n_resident <= 0 || n_resident > (int)s->resident.size() || iters <= 0 || !ms_per_launch) return fail(B2V_EINVAL, "bad argument");
-  int rc = b2v_flush(h);
-  if (rc) return rc;
-  std::lock_guard<std::mutex> sub(s->submit_mu);
-  CK(cudaSetDevice(s->device));
-  std::vector<uint8_t*> outs(n_resident, nullptr);
-  size_t ob = (size_t)s->coded_w * s->coded_h * 3 / 2;
-  for (auto& o : outs) CK(cudaMalloc((void**)&o, ob));
-  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, s->resident[i], s->src_w * 4, outs[i]), s->st_enc);
-  CK(cudaStreamSynchronize(s->st_enc));
-  cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-  cudaEventRecord(e0, s->st_enc);
-  for (int i = 0; i < iters; i++) { int k = i % n_resident; launch_csc(csc_params(s, s->resident[k], s->src_w * 4, outs[k]), s->st_enc); }
-  cudaEventRecord(e1, s->st_enc);
-  CK(cudaStreamSynchronize(s->st_enc));
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  for (auto o : outs) cudaFree(o);
-  CK(cudaGetLastError());
-  *ms_per_launch = ms / iters;
-  return 0;
+  return bench_csc((Session*)h, n_resident, iters, ms_per_launch, true);
 }
 
 }  // extern "C"

@@ -1,9 +1,37 @@
 // b2v_internal.h — shared declarations between the C-ABI (b2v_api.cu) and the kernels.
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace b2v {
+
+// ---- access-unit container: both encoders write it into HBM, the session's output thread reads it ----
+// 64-byte record the pack kernel writes in front of the access unit in HBM; travels to the host
+// with the first D2H chunk.
+struct AuHeader {
+  int32_t size;            // bytes of data following the header (and band table)
+  int32_t qp;              // slice QP used
+  int32_t is_idr;
+  int32_t n_slices;
+  int64_t total_bits;      // before emulation prevention
+  int32_t next_qp;         // rate controller output for the next frame
+  int32_t overflow;        // non-zero if a macroblock exceeded its scratch budget (must never happen)
+  uint64_t csc_t0, csc_t1;  // %globaltimer stamps of the CSC launch of this picture (0 when timing is off)
+  int32_t pad[4];
+};
+static_assert(sizeof(AuHeader) == 64, "AuHeader must be 64 bytes");
+
+// banded output (striped H.264, JPEG stripes): one record per band right after the AuHeader (offsets relative to the first data byte)
+struct BandEntry { int32_t off, size, coded, frame_num; };
+
+// shape of an encoder's access-unit buffers
+struct AuLayout {
+  size_t cap;              // bytes of one buffer
+  int data_off;            // bytes in front of the first data byte: AuHeader [+ band table] (+ slack for an in-place stripe header)
+  int n_bands;             // band table entries; 0 = full frame, no band table
+  int band_rows;           // macroblock rows (16 luma rows) per band; 0 when n_bands == 0
+};
 
 // ---- colour conversion spec (DESIGN.md §3; BT.709 limited range, 14-bit coefficients) ----
 constexpr int KYR = 2991, KYG = 10064, KYB = 1016;

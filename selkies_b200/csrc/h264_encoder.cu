@@ -237,9 +237,9 @@ void encoder_destroy(Encoder* e) {
   delete e;
 }
 
-size_t encoder_au_capacity(const Encoder* e) { return e->au_cap; }
-int encoder_au_data_offset(const Encoder* e) { return e->au_data_off; }
-int encoder_band_count(const Encoder* e) { return e->striped ? e->n_bands : 0; }
+AuLayout encoder_layout(const Encoder* e) {
+  return {e->au_cap, e->au_data_off, e->striped ? e->n_bands : 0, e->striped ? e->band_rows : 0};
+}
 const uint8_t* encoder_recon(const Encoder* e) { return e->recon[e->cur]; }
 
 int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {

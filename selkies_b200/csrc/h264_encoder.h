@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "b2v_internal.h"
+
 namespace b2v {
 
 struct Encoder;
@@ -17,33 +19,15 @@ struct EncoderConfig {
   int idr_slice_mbs;       // IDR pictures: macroblocks per slice inside a row (needs slice_rows == 1); 0 = default rule, < 0 = whole rows
 };
 
-// 64-byte record the pack kernel writes in front of the access unit in HBM; travels to the host
-// with the first D2H chunk.
-struct AuHeader {
-  int32_t size;            // bytes of Annex-B data following this header
-  int32_t qp;              // slice QP used
-  int32_t is_idr;
-  int32_t n_slices;
-  int64_t total_bits;      // before emulation prevention
-  int32_t next_qp;         // rate controller output for the next frame
-  int32_t overflow;        // non-zero if a macroblock exceeded its scratch budget (must never happen)
-  uint64_t csc_t0, csc_t1;  // %globaltimer stamps of the CSC launch of this picture (0 when timing is off)
-  int32_t pad[4];
-};
-static_assert(sizeof(AuHeader) == 64, "AuHeader must be 64 bytes");
-
-// striped mode: one record per band right after the AuHeader (offsets relative to the first NAL byte)
-struct BandEntry { int32_t off, size, coded, frame_num; };
-
 struct EncodeFrameParams {
   const uint8_t* cur;      // NV12, coded size, device
-  uint8_t* au;             // device buffer, encoder_au_capacity() bytes; AuHeader first
+  uint8_t* au;             // device buffer, encoder_layout().cap bytes; AuHeader first
   int idr;
   int rc_mode;             // B2V_RC_CBR | B2V_RC_CQP
   int qp_fixed;
   int paint_trigger, paint_qp, paint_burst;   // paint-over: `paint_burst` pictures at paint_qp after `paint_trigger` all-skipped pictures (0 = off)
   int64_t target_bits;     // per frame, CBR
-  cudaEvent_t* ev;         // null, or 8 timing events: encoder records ev[2..5] after each stage (forces the serial schedule)
+  cudaEvent_t* ev;         // null, or 6 timing events: encoder records ev[2..5] after each stage (forces the serial schedule)
   cudaStream_t st_pack;    // null = everything on `st`; else the entropy coding of this picture (k_cavlc_mb ... k_pack_au) runs here,
                            // overlapping the analysis of the next picture on `st`.  The access unit is complete on st_pack.
   const unsigned long long* csc_ts;   // null, or the CSC launch's device stamps to forward in the AuHeader
@@ -51,9 +35,7 @@ struct EncodeFrameParams {
 
 int  encoder_create(const EncoderConfig* cfg, Encoder** out);
 void encoder_destroy(Encoder* e);
-size_t encoder_au_capacity(const Encoder* e);
-int  encoder_au_data_offset(const Encoder* e);   // AuHeader + band table (+ slack for an in-place stripe header)
-int  encoder_band_count(const Encoder* e);       // 0 when full-frame
+AuLayout encoder_layout(const Encoder* e);       // n_bands == 0 when full-frame
 // enqueue one frame on `st` (and `p->st_pack`); returns the number of kernel launches issued
 int  encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st);
 const uint8_t* encoder_recon(const Encoder* e);   // NV12 reconstruction of the last encoded frame

@@ -19,7 +19,6 @@
 #include <cstring>
 #include <vector>
 
-#include "h264_encoder.h"     // AuHeader, BandEntry: the JPEG mode reuses the access-unit container of the striped H.264 mode
 #include "jpeg.h"
 
 namespace b2v {
@@ -471,10 +470,7 @@ void jpeg_destroy(JpegEncoder* e) {
   for (void* p : ptrs) if (p) cudaFree(p);
   delete e;
 }
-size_t jpeg_au_capacity(const JpegEncoder* e) { return e->au_cap; }
-int jpeg_au_data_offset(const JpegEncoder* e) { return e->au_data_off; }
-int jpeg_stripe_count(const JpegEncoder* e) { return e->n_stripes; }
-int jpeg_stripe_rows(const JpegEncoder* e) { return e->stripe_rows; }
+AuLayout jpeg_layout(const JpegEncoder* e) { return {e->au_cap, e->au_data_off, e->n_stripes, e->stripe_rows}; }
 
 int jpeg_encode(JpegEncoder* e, const uint8_t* cur_nv12, uint8_t* au, int force_all, cudaStream_t st) {
   JpegCtx c{};

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "b2v_internal.h"    // AuHeader, BandEntry, AuLayout: the access-unit container of the striped H.264 mode
+
 namespace b2v {
 
 struct JpegEncoder;
@@ -18,10 +20,7 @@ struct JpegConfig {
 
 int  jpeg_create(const JpegConfig* cfg, JpegEncoder** out);
 void jpeg_destroy(JpegEncoder* e);
-size_t jpeg_au_capacity(const JpegEncoder* e);
-int  jpeg_au_data_offset(const JpegEncoder* e);   // AuHeader + stripe table (+ slack for an in-place stripe header)
-int  jpeg_stripe_count(const JpegEncoder* e);
-int  jpeg_stripe_rows(const JpegEncoder* e);
+AuLayout jpeg_layout(const JpegEncoder* e);       // always banded: n_bands >= 1 stripes
 // enqueue one picture (NV12 in the JFIF matrix, coded size) on `st`; the output buffer gets AuHeader | BandEntry[n_stripes] | the
 // JFIF files of the delivered stripes back to back.  force_all: deliver every stripe (first picture, refresh request).
 // Returns the number of kernel launches issued.

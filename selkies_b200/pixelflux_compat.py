@@ -25,11 +25,13 @@ from __future__ import annotations
 import ctypes as C
 import threading
 import time
+from types import SimpleNamespace
 from typing import Callable, Optional
 
 import numpy as np
 
 from . import _native as N
+from .session import Session
 
 
 class CaptureSettings:
@@ -174,9 +176,7 @@ class ScreenCapture:
 
     def __init__(self, frame_source: Optional[FrameSource] = None):
         self._source = frame_source
-        self._lib = None
-        self._h = None
-        self._cb_native = None
+        self._session: Optional[Session] = None
         self._user_cb = None
         self._thread = None
         self._stop = threading.Event()
@@ -190,7 +190,7 @@ class ScreenCapture:
     # -- lifecycle ----------------------------------------------------------------------------------
     def start_capture(self, settings: CaptureSettings, callback) -> None:
         with self._lock:
-            if self._h is not None:
+            if self._session is not None:
                 raise RuntimeError("capture already running")
             jpeg = int(getattr(settings, "output_mode", 1)) == 0        # the reference's "jpeg" encoder (selkies.py:3209-3212)
             if not callable(callback):
@@ -205,10 +205,8 @@ class ScreenCapture:
             w, h = int(settings.capture_width), int(settings.capture_height)
             w -= w & 1
             h -= h & 1                                # the reference forces even sizes (webrtc_mode.py:397-402)
-            self._lib = N.lib()                      # raises if the CUDA library is missing: no CPU fallback
-            s = N.B2VSettings()
-            s.src_w, s.src_h = w, h
-            s.dst_w, s.dst_h = int(getattr(settings, "output_width", 0) or 0), int(getattr(settings, "output_height", 0) or 0)
+            s = SimpleNamespace(paintover_trigger_frames=0, paintover_crf=0, paintover_burst_frames=0)      # Session keyword arguments; paint-over off
+            s.dst_width, s.dst_height = int(getattr(settings, "output_width", 0) or 0), int(getattr(settings, "output_height", 0) or 0)
             s.fps = float(settings.target_fps) if float(settings.target_fps) > 0 else 60.0
             s.device = int(getattr(settings, "gpu_id", 0) or 0)
             s.rc_mode = N.B2V_RC_CBR if bool(settings.h264_cbr_mode) else N.B2V_RC_CQP
@@ -231,7 +229,7 @@ class ScreenCapture:
                 sl = max(1, s.slice_rows)
                 rows = int(getattr(settings, "h264_stripe_rows", 0) or 0)
                 if rows <= 0:
-                    mbh = ((int(s.dst_h) or h) + 15) // 16
+                    mbh = ((s.dst_height or h) + 15) // 16
                     rows = -(-mbh // 8)
                 s.stripe_rows = -(-rows // sl) * sl
             if jpeg:
@@ -244,11 +242,8 @@ class ScreenCapture:
                 s.paintover_trigger_frames = int(getattr(settings, "paint_over_trigger_frames", 15) or 0) if bool(getattr(settings, "use_paint_over_quality", False)) else 0
                 s.stripe_rows = int(getattr(settings, "h264_stripe_rows", 0) or 0)
             self._user_cb = callback
-            self._cb_native = N.FRAME_CB(self._on_frame)
-            handle = C.c_void_p()
-            N.check(self._lib.b2v_create(C.byref(s), self._cb_native, None, C.byref(handle)))
-            self._h = handle
-            self._w, self._h_px = w, h
+            # raises if the CUDA library is missing: no CPU fallback
+            self._session = Session(w, h, collect=False, on_frame=self._on_frame, **vars(s))
             self._fps = s.fps
             if self._source is None:
                 self._source = SyntheticDesktopSource()
@@ -260,55 +255,54 @@ class ScreenCapture:
     def stop_capture(self) -> None:
         """Blocking: joins the capture thread and drains the encoder (media_pipeline.py:313)."""
         with self._lock:
-            h, t = self._h, self._thread
-            if h is None:
+            t = self._thread
+            if self._session is None:
                 return
             self._stop.set()
         if t is not None and t is not threading.current_thread():
             t.join()
         with self._lock:
-            if self._h is not None:
-                self._lib.b2v_destroy(self._h)
-                self._h = None
+            if self._session is not None:
+                self._session.close()
+                self._session = None
             self._thread = None
 
     @staticmethod
     def _gop_frames(seconds: float, fps: float) -> int:
-        """keyframe_distance is in SECONDS (settings.py:163); b2v_settings.gop is in frames."""
+        """keyframe_distance is in SECONDS (settings.py:163); the session's gop is in frames."""
         return -1 if seconds <= 0 else max(1, int(round(seconds * fps)))
 
     # -- live control ----------------------------------------------------------------------------------
     def update_framerate(self, fps: float) -> None:
         with self._lock:
-            if self._h is None:
+            if self._session is None:
                 return
-            N.check(self._lib.b2v_set_framerate(self._h, float(fps)))
+            self._session.set_framerate(fps)
             self._fps = float(fps)
             if self._kf_seconds > 0:               # the key-frame interval is a time: keep it across the rate change
-                N.check(self._lib.b2v_set_gop(self._h, self._gop_frames(self._kf_seconds, self._fps)))
+                self._session.set_gop(self._gop_frames(self._kf_seconds, self._fps))
 
     def update_video_bitrate(self, kbps: int) -> None:
         with self._lock:
-            if self._h is None:
+            if self._session is None:
                 return
-            N.check(self._lib.b2v_set_bitrate_kbps(self._h, int(kbps)))
+            self._session.set_bitrate_kbps(kbps)
 
     def request_idr_frame(self) -> None:
         with self._lock:
-            if self._h is None:
+            if self._session is None:
                 return
-            N.check(self._lib.b2v_request_idr(self._h))
+            self._session.request_idr()
 
     def update_resolution(self, width: int, height: int) -> None:
         """Follow a display resize (what auto_adjust_screen_capture_size does in the reference)."""
         with self._resize_lock:                  # the capture loop holds no ring slot while we are in here
             with self._lock:
-                if self._h is None:
+                if self._session is None:
                     return
                 width -= width & 1
                 height -= height & 1
-                N.check(self._lib.b2v_set_resolution(self._h, width, height, 0, 0))
-                self._w, self._h_px = width, height
+                self._session.set_resolution(width, height)
                 self._source.configure(width, height)
 
     def set_cursor_callback(self, fn) -> None:       # selkies.py:3166-3167 (guarded by hasattr)
@@ -321,22 +315,20 @@ class ScreenCapture:
         while not self._stop.is_set():
             # The control lock is held only for the snapshot: acquire (blocks while the ring is full), fill (tens of ms at 4K) and
             # submit run outside it, so request_idr_frame / update_* never queue behind a frame and a callback that calls them
-            # while the ring is full cannot deadlock.  The handle stays valid: stop_capture joins this thread before destroying it.
+            # while the ring is full cannot deadlock.  The session stays open: stop_capture joins this thread before closing it.
             with self._lock:
-                handle, fps = self._h, self._fps
-            if handle is None:
+                session, fps = self._session, self._fps
+            if session is None:
                 break
             with self._resize_lock:
-                w, h = self._w, self._h_px
-                slot = C.c_int32(-1)
-                p = self._lib.b2v_ring_acquire(handle, C.byref(slot))
-                if not p:
-                    break
-                view = np.frombuffer((C.c_ubyte * (w * h * 4)).from_address(p), np.uint8).reshape(h, w, 4)
+                try:
+                    slot, view = session.acquire()
+                except N.B2VError:
+                    break                         # the session is stopping
                 if not self._source.fill(view, index):
-                    self._lib.b2v_ring_release(handle, slot.value)      # end of the source: nothing to encode
+                    session.release_slot(slot)    # end of the source: nothing to encode
                     break
-                N.check(self._lib.b2v_ring_submit(handle, slot.value, w * 4, time.monotonic_ns()))
+                session.submit_slot(slot, time.monotonic_ns())
             index += 1
             next_t += 1.0 / max(1e-3, fps)
             delay = next_t - time.perf_counter()
@@ -345,7 +337,7 @@ class ScreenCapture:
             else:
                 next_t = time.perf_counter()      # fell behind: do not burst
 
-    def _on_frame(self, fptr, _user):
+    def _on_frame(self, fptr):
         f = fptr.contents
         r = _Result()
         # zero-copy view of the native buffer, valid for the duration of the callback only
