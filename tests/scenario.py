@@ -1,15 +1,19 @@
 """Scripted two-sided driver: one event list applied to a GPU `Session` and to `oracle.RefEncoder`, compared picture by picture.
+Every H.264 parity test that drives a `Session` runs through it.
 
 Events (plain tuples, built by the helpers below): picture(frame), set_bitrate(kbps), set_fps(fps), set_qp(qp), request_idr(),
-set_gop(n), resize(src_w, src_h, dst_w, dst_h).  The GPU side submits without flushing, so pictures stay in flight on both
-streams as they do in a live session; control calls land between two submits (include/b2video.h: a call made after submit k
-applies from picture k+1).  The oracle side restates the host rules of b2v_api.cu: the per-picture target
-int(kbps * 1000 / fps), the IDR decision `want_idr or (gop > 0 and frames_since_idr >= gop)`, and a resize = a fresh encoder
-at the new size fed the oracle's CSC(+scale), starting with an IDR.
+set_gop(n), resize(src_w, src_h, dst_w, dst_h), flush().  The GPU side submits without flushing unless a flush() event asks
+for it, so pictures stay in flight on both streams as they do in a live session; control calls land between two submits
+(include/b2video.h: a call made after submit k applies from picture k+1).  Pictures enter through the host ring
+(Config.entry "ring") or, as bench.py feeds them, as frames resident on the device ("resident": each distinct frame object is
+uploaded once).  The oracle side restates the host rules of b2v_api.cu: the per-picture target int(kbps * 1000 / fps), the IDR
+decision `want_idr or (gop > 0 and frames_since_idr >= gop)`, and a resize = a fresh encoder at the new size fed the oracle's
+CSC(+scale), starting with an IDR.
 
-Per picture the access unit (in striped mode: the (y_start, bytes) of every delivered band), is_key, qp and frame_id must be
-equal.  At the end of every segment (the pictures between two resizes) the reconstructions must be equal and libavcodec must
-decode the segment's stream (every band's stream on its own in striped mode) to that reconstruction."""
+Per picture, every delivered band (one band at y_start 0 in full-frame mode) must equal the oracle's: bytes, is_key, qp,
+frame_id, y_start and height, and in pixelflux header mode the 10-byte header that carries them.  At the end of every segment
+(the pictures between two resizes) the reconstructions must be equal and libavcodec must decode the segment's stream (every
+band's stream on its own in striped mode) to that reconstruction."""
 from __future__ import annotations
 
 from dataclasses import dataclass, field
@@ -49,11 +53,26 @@ def resize(src_w, src_h, dst_w=0, dst_h=0):
     return ("resize", int(src_w), int(src_h), int(dst_w or src_w), int(dst_h or src_h))
 
 
+def flush():
+    return ("flush",)
+
+
+def stream(frames, idr_at=()) -> list:
+    """Pictures of `frames` in order, with flush() and request_idr() before every picture index in idr_at except 0."""
+    events = []
+    for i, f in enumerate(frames):
+        if i in idr_at and i > 0:
+            events += [flush(), request_idr()]
+        events.append(picture(f))
+    return events
+
+
 def describe(ev) -> str:
     return ev[0] + "(" + ", ".join(str(a) for a in ev[1:]) + ")"
 
 
-CBR, CQP = 0, 1          # = selkies_b200._native.B2V_RC_CBR / B2V_RC_CQP (the oracle side needs no library)
+CBR, CQP = 0, 1                  # = selkies_b200._native.B2V_RC_CBR / B2V_RC_CQP (the oracle side needs no library)
+HDR_NONE, HDR_PIXELFLUX = 0, 1   # = selkies_b200._native.B2V_HDR_NONE / B2V_HDR_PIXELFLUX
 
 
 @dataclass
@@ -69,7 +88,12 @@ class Config:
     gop: int = -1
     paint: tuple = (0, 18, 1)          # (trigger pictures, paint-over QP, burst pictures); trigger 0 = off
     stripe_rows: int = 0
+    slice_rows: int = 0                # 0 = the default rule (8-row slices), as in Session and RefEncoder
+    idr_slice_mbs: int = 0
+    header_mode: int = HDR_NONE
+    flags: int = 0                     # B2V_FLAG_* bits of the GPU session
     ring_slots: int = 4
+    entry: str = "ring"                # "ring" (b2v_ring_submit) or "resident" (b2v_resident_upload + b2v_submit_resident)
 
 
 @dataclass
@@ -81,6 +105,12 @@ class Expected:
     bands: list                        # [(y_start, bytes)]: one entry at y_start 0 in full-frame mode
     rc: dict                           # oracle rate-control record after this picture (RefEncoder.rc_state)
     after: str                         # the control event just before this picture (or "start")
+
+    @property
+    def au(self) -> bytes:
+        """The access unit of a full-frame picture."""
+        (_, au), = self.bands
+        return au
 
 
 @dataclass
@@ -99,7 +129,8 @@ class OracleSide:
 
     def _new_encoder(self, sw, sh, dw, dh):
         self.src, self.dst = (sw, sh), (dw, dh)
-        self.enc = oracle.RefEncoder(dw, dh)
+        self.enc = oracle.RefEncoder(dw, dh, self.cfg.slice_rows)
+        self.enc.set_idr_slice_mbs(self.cfg.idr_slice_mbs)
         if self.cfg.stripe_rows:
             self.enc.set_stripes(self.cfg.stripe_rows)
         if self.cfg.paint[0] > 0:
@@ -120,7 +151,7 @@ class OracleSide:
         elif kind == "resize":
             self._new_encoder(*ev[1:])
             self.want_idr = True
-        else:
+        elif kind != "flush":          # the oracle has nothing in flight
             raise ValueError(f"unknown event {ev!r}")
 
     def picture(self, frame, after: str) -> Expected:
@@ -144,10 +175,15 @@ class OracleSide:
 class GpuSide:
     def __init__(self, cfg: Config, device: int = 0):
         from selkies_b200.session import Session
+        assert cfg.entry in ("ring", "resident"), cfg.entry
         p = cfg.paint
+        self.resident = cfg.entry == "resident"
+        self.uploaded = {}                 # id(frame) -> (resident index, frame); the frame is held so that its id stays unique
         self.s = Session(cfg.width, cfg.height, dst_width=cfg.dst_width, dst_height=cfg.dst_height, fps=cfg.fps, device=device,
-                         rc_mode=cfg.rc_mode, bitrate_kbps=cfg.kbps, crf=cfg.qp, gop=cfg.gop, stripe_rows=cfg.stripe_rows,
-                         paintover_trigger_frames=p[0], paintover_crf=p[1], paintover_burst_frames=p[2], ring_slots=cfg.ring_slots)
+                         rc_mode=cfg.rc_mode, bitrate_kbps=cfg.kbps, crf=cfg.qp, gop=cfg.gop, slice_rows=cfg.slice_rows,
+                         idr_slice_mbs=cfg.idr_slice_mbs, stripe_rows=cfg.stripe_rows, header_mode=cfg.header_mode,
+                         paintover_trigger_frames=p[0], paintover_crf=p[1], paintover_burst_frames=p[2], ring_slots=cfg.ring_slots,
+                         flags=cfg.flags)
 
     def control(self, ev):
         kind, s = ev[0], self.s
@@ -161,11 +197,21 @@ class GpuSide:
             s.set_gop(ev[1])
         elif kind == "request_idr":
             s.request_idr()
+        elif kind == "flush":
+            s.flush()
         elif kind == "resize":
             s.set_resolution(*ev[1:])
+            self.uploaded.clear()          # the library frees its resident frames on a resize
 
     def picture(self, frame):
-        self.s.submit(frame)              # no flush: the picture stays in flight
+        if not self.resident:
+            self.s.submit(frame)           # no flush: the picture stays in flight
+            return
+        if id(frame) not in self.uploaded:
+            k = len(self.uploaded)
+            self.s.resident_upload(k, frame)
+            self.uploaded[id(frame)] = (k, frame)
+        self.s.submit_resident(self.uploaded[id(frame)][0])
 
 
 def _first_diff(a: bytes, b: bytes) -> int:
@@ -175,6 +221,10 @@ def _first_diff(a: bytes, b: bytes) -> int:
 
 def _where(x: Expected) -> str:
     return f"picture {x.index} (after {x.after})"
+
+
+def _band_height(cfg: Config, h: int, y0: int) -> int:
+    return min(h, y0 + cfg.stripe_rows * 16) - y0 if cfg.stripe_rows else h
 
 
 def _check_segment(cfg: Config, seg: Segment, got: list, grec, rrec, decode: bool):
@@ -192,13 +242,21 @@ def _check_segment(cfg: Config, seg: Segment, got: list, grec, rrec, decode: boo
         where = _where(x)
         assert len(gs) == len(x.bands), f"{where}: {len(gs)} bands delivered, oracle codes {len(x.bands)} (y_start {[y for y, _ in x.bands]})"
         for g, (y0, ref) in zip(gs, x.bands):
+            bh = _band_height(cfg, h, y0)
             assert g.frame_id == x.index, f"{where}: frame_id {g.frame_id}"
             assert g.is_key == x.is_key, f"{where}: is_key gpu {g.is_key} oracle {x.is_key}"
             assert g.qp == x.qp, f"{where}: qp gpu {g.qp} oracle {x.qp}"
             assert g.y_start == y0, f"{where}: band y_start gpu {g.y_start} oracle {y0}"
-            if g.data != ref:
-                raise AssertionError(f"{where}, band y_start {y0}: AU differs at byte {_first_diff(g.data, ref)} "
-                                     f"(gpu {len(g.data)} B, oracle {len(ref)} B, qp {g.qp})")
+            assert g.height == bh, f"{where}, band y_start {y0}: height gpu {g.height}, expected {bh}"
+            data = g.data
+            if cfg.header_mode == HDR_PIXELFLUX:
+                # 04 | is_key | frame_id u16be | y_start u16be | width u16be | band height u16be
+                hdr = bytes([4, x.is_key]) + b"".join(v.to_bytes(2, "big") for v in (x.index & 0xFFFF, y0, w, bh))
+                assert data[:10] == hdr, f"{where}, band y_start {y0}: header {data[:10].hex()}, expected {hdr.hex()}"
+                data = data[10:]
+            if data != ref:
+                raise AssertionError(f"{where}, band y_start {y0}: AU differs at byte {_first_diff(data, ref)} "
+                                     f"(gpu {len(data)} B, oracle {len(ref)} B, qp {g.qp})")
     first = seg.pictures[0]
     assert first.is_key, f"segment at picture {seg.first} does not start with an IDR"
     for _, au in first.bands:
@@ -208,7 +266,7 @@ def _check_segment(cfg: Config, seg: Segment, got: list, grec, rrec, decode: boo
         return
     bands = sorted({y0 for x in seg.pictures for y0, _ in x.bands})
     for y0 in bands:
-        y1 = min(h, y0 + cfg.stripe_rows * 16) if cfg.stripe_rows else h
+        y1 = y0 + _band_height(cfg, h, y0)
         aus = [au for x in seg.pictures for yb, au in x.bands if yb == y0]
         dec = avdec.decode_stream(aus, quiet=True)
         assert len(dec) == len(aus), f"segment at picture {seg.first}, band {y0}: {len(dec)} pictures decoded of {len(aus)}"

@@ -3,9 +3,8 @@ content mixes (edge cases: one-macroblock-wide pictures, cropped sizes, search w
 import numpy as np
 import pytest
 
-from selkies_b200 import _native as N
+from tests import scenario as S
 from tests import synth
-from tests.test_encode_gpu import assert_same, encode_both
 
 pytestmark = pytest.mark.gpu
 
@@ -41,18 +40,15 @@ def test_random_configuration(seed):
     frames = make_frames(rng, w, h, n)
     idr_at = tuple(sorted({0} | {int(i) for i in rng.integers(1, n, size=int(rng.integers(0, 2)))}))
     if rng.integers(0, 3) == 0:
-        kbps = int(rng.choice([100, 400, 2000, 20000]))
-        got, ref, grec, rrec = encode_both(w, h, frames, slice_rows=slice_rows, idr_at=idr_at, rc_mode=N.B2V_RC_CBR, kbps=kbps, fps=30.0)
+        cfg = S.Config(w, h, rc_mode=S.CBR, kbps=int(rng.choice([100, 400, 2000, 20000])), fps=30.0, slice_rows=slice_rows)
     else:
-        qp = int(rng.choice([0, 8, 18, 24, 30, 37, 45, 51]))
-        got, ref, grec, rrec = encode_both(w, h, frames, qp=qp, slice_rows=slice_rows, idr_at=idr_at)
-    assert_same(got, ref, grec, rrec)
+        cfg = S.Config(w, h, qp=int(rng.choice([0, 8, 18, 24, 30, 37, 45, 51])), slice_rows=slice_rows)
+    S.run(cfg, S.stream(frames, idr_at))
 
 
 @pytest.mark.parametrize("seed", range(12))
 def test_random_striped_configuration(seed):
     """Same, in striped mode (random band height) with paint-over switched on in the constant-QP runs and still pictures mixed in."""
-    from tests.test_stripes_gpu import group, run_both
     rng = np.random.default_rng(5000 + seed)
     w = int(rng.choice([32, 66, 130, 160, 258, 322])) & ~1
     h = int(rng.choice([48, 70, 96, 130, 176, 226])) & ~1
@@ -67,11 +63,9 @@ def test_random_striped_configuration(seed):
         else:
             frames[t][: h // 3] = frames[0][: h // 3]         # static top third
     idr_at = tuple(sorted({0} | {int(i) for i in rng.integers(1, n, size=int(rng.integers(0, 2)))}))
+    layout = dict(stripe_rows=stripe_rows, slice_rows=slice_rows)
     if rng.integers(0, 3) == 0:
-        got, ref, grec, rrec = run_both(w, h, frames, stripe_rows, slice_rows, rc_mode=N.B2V_RC_CBR, kbps=int(rng.choice([200, 1500, 20000])), idr_at=idr_at)
+        cfg = S.Config(w, h, rc_mode=S.CBR, kbps=int(rng.choice([200, 1500, 20000])), fps=30.0, **layout)
     else:
-        got, ref, grec, rrec = run_both(w, h, frames, stripe_rows, slice_rows, qp=int(rng.choice([10, 24, 30, 38, 47])), idr_at=idr_at,
-                                         paint=(int(rng.integers(1, 3)), int(rng.choice([8, 16, 22]))))
-    for i, (gp, rp) in enumerate(zip(group(got, n), ref)):
-        assert [(g.y_start, g.data) for g in gp] == rp, f"picture {i}"
-    assert np.array_equal(grec[0], rrec[0]) and np.array_equal(grec[1], rrec[1])
+        cfg = S.Config(w, h, qp=int(rng.choice([10, 24, 30, 38, 47])), paint=(int(rng.integers(1, 3)), int(rng.choice([8, 16, 22])), 1), **layout)
+    S.run(cfg, S.stream(frames, idr_at))

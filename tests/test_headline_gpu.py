@@ -5,85 +5,43 @@ full frame).  bench.py: 3840x2160 synthetic desktop, CBR 20 Mbit/s @ 60 fps nomi
 and the 16-picture scroll cycle — picture 16 is the scroll RESTART, the one picture of the cycle in which nothing is
 predictable and every macroblock runs the exhaustive search + refinement.  The pictures go through the same entry point as
 the timed legs (b2v_submit_resident, B2V_FLAG_TIMING_CSC, two-stream schedule, several pictures in flight) and every access
-unit AND the final reconstruction must equal the oracle's, byte for byte."""
-import numpy as np
+unit AND the final reconstruction must equal the oracle's, byte for byte (tests/scenario.py)."""
+import dataclasses
+
 import pytest
 
 import oracle
 from selkies_b200 import _native as N
-from selkies_b200.session import Session
+from tests import scenario as S
 from tests import synth
 
 pytestmark = pytest.mark.gpu
 
-W, H, FPS, KBPS, N_DISTINCT, N_PICS = 3840, 2160, 60.0, 20000, 16, 18
+W, H, N_DISTINCT, N_PICS = 3840, 2160, 16, 18
+HEADLINE = S.Config(W, H, rc_mode=S.CBR, kbps=20000, fps=60.0, ring_slots=N_DISTINCT, flags=N.B2V_FLAG_TIMING_CSC, entry="resident")
 
 
 @pytest.fixture(scope="module")
-def c2_frames():
-    return [synth.desktop(W, H, t) for t in range(N_DISTINCT)]
-
-
-def oracle_stream(frames, n, stripe_rows=0):
+def c2_events():
     oracle.set_threads(0)
-    enc = oracle.RefEncoder(W, H)            # default slicing, as the session's: 8-row slices (one per stripe in striped mode), IDR pictures sub-row
-    if stripe_rows:
-        enc.set_stripes(stripe_rows)
-    target = int(KBPS * 1000 / FPS)
-    aus, tables = [], []
-    for i in range(n):
-        aus.append(enc.encode_bgra(frames[i % len(frames)], i == 0, rc_mode=0, target_bits=target))
-        tables.append(enc.stripe_table() if stripe_rows else None)
-    return aus, tables, enc.recon()
+    frames = [synth.desktop(W, H, t) for t in range(N_DISTINCT)]
+    return [S.picture(frames[i % N_DISTINCT]) for i in range(N_PICS)]
 
 
-def first_diff(a: bytes, b: bytes) -> int:
-    n = min(len(a), len(b))
-    return next((k for k in range(n) if a[k] != b[k]), n)
-
-
-def gpu_stream(frames, n, device=0, **kw):
-    with Session(W, H, fps=FPS, device=device, rc_mode=N.B2V_RC_CBR, bitrate_kbps=KBPS, ring_slots=N_DISTINCT,
-                 flags=N.B2V_FLAG_TIMING_CSC, **kw) as s:
-        for i, f in enumerate(frames):
-            s.resident_upload(i, f)
-        for i in range(n):                       # free-running, like the timed leg: no flush between pictures
-            s.submit_resident(i % len(frames))
-        s.flush()
-        return s.take_frames(), s.recon()
-
-
-def test_c2_4k_cbr20_idr_plus_17p_bit_exact(c2_frames):
-    got, grec = gpu_stream(c2_frames, N_PICS)
-    ref, _, rrec = oracle_stream(c2_frames, N_PICS)
-    assert len(got) == N_PICS and got[0].is_key and not any(g.is_key for g in got[1:])
-    for i, (g, r) in enumerate(zip(got, ref)):
-        assert g.data == r, f"picture {i}: AU differs at byte {first_diff(g.data, r)} (gpu {len(g.data)} B, oracle {len(r)} B, qp {g.qp})"
-    assert np.array_equal(grec[0], rrec[0]) and np.array_equal(grec[1], rrec[1])
+def test_c2_4k_cbr20_idr_plus_17p_bit_exact(c2_events):
+    xs = S.pictures(S.run(HEADLINE, c2_events))
+    assert [x.is_key for x in xs] == [True] + [False] * (N_PICS - 1)
     # the scroll restart (picture 16) is the expensive one: it must be much larger than a steady scroll picture
-    assert len(got[16].data) > 2 * len(got[15].data)
+    assert len(xs[16].au) > 2 * len(xs[15].au)
 
 
-def test_c2_4k_striped_8_bands_bit_exact(c2_frames):
+def test_c2_4k_striped_8_bands_bit_exact(c2_events):
     rows = -(-(H // 16) // 8)                    # 17 macroblock rows per stripe, as bench.py's striped leg
-    got, grec = gpu_stream(c2_frames, N_PICS, stripe_rows=rows)
-    ref, tables, rrec = oracle_stream(c2_frames, N_PICS, stripe_rows=rows)
-    k = 0
-    for i, (au, tab) in enumerate(zip(ref, tables)):
-        for b, (off, size, coded) in enumerate(tab):
-            if not coded:
-                continue
-            g = got[k]; k += 1
-            assert g.frame_id == i and g.y_start == b * rows * 16
-            assert g.data == au[off: off + size], f"picture {i} stripe {b}: differs at byte {first_diff(g.data, au[off: off + size])}"
-    assert k == len(got)
-    assert np.array_equal(grec[0], rrec[0]) and np.array_equal(grec[1], rrec[1])
+    S.run(dataclasses.replace(HEADLINE, stripe_rows=rows), c2_events)
 
 
-def test_c3_second_gpu_same_stream(c2_frames):
-    """configs[3]: one session per GPU.  A session on device 1 (when the box has one) produces the same bytes as device 0."""
+def test_c3_second_gpu_same_stream(c2_events):
+    """configs[3]: one session per GPU.  A session on device 1 (when the box has one) produces the oracle's stream too."""
     if N.lib().b2v_device_count() < 2:
         pytest.skip("one GPU visible")
-    a, _ = gpu_stream(c2_frames, 6, device=0)
-    b, _ = gpu_stream(c2_frames, 6, device=1)
-    assert [x.data for x in a] == [x.data for x in b]
+    S.run(HEADLINE, c2_events[:6], device=1)

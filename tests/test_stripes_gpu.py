@@ -1,44 +1,15 @@
 """GPU parity, striped mode ("x264enc-striped", CaptureSettings.h264_fullframe = False, selkies.py:3219): the CUDA encoder's
-stripes vs oracle/h264_ref.c, bit-exact, through the C-ABI; every stripe stream decodes on its own (libavcodec)."""
+stripes vs oracle/h264_ref.c, bit-exact, through the C-ABI (tests/scenario.py); every stripe stream decodes on its own (libavcodec)."""
 import numpy as np
 import pytest
 
-import oracle
 from oracle import avdec
 from selkies_b200 import _native as N
 from selkies_b200.session import Session
+from tests import scenario as S
 from tests import synth
 
 pytestmark = pytest.mark.gpu
-
-
-def run_both(w, h, frames, stripe_rows, slice_rows, *, qp=28, rc_mode=N.B2V_RC_CQP, kbps=0, fps=30.0, idr_at=(0,), header_mode=N.B2V_HDR_NONE, paint=(0, 18)):
-    enc = oracle.RefEncoder(w, h, slice_rows)
-    enc.set_stripes(stripe_rows)
-    enc.set_paintover(*paint)
-    target = int(kbps * 1000 / fps) if kbps else 0
-    ref = []                       # per picture: [(y_start, bytes)] of the coded bands
-    for i, f in enumerate(frames):
-        au = enc.encode_bgra(f, i in idr_at, rc_mode=1 if rc_mode == N.B2V_RC_CQP else 0, qp=qp, target_bits=target)
-        ref.append([(k * stripe_rows * 16, au[o:o + sz]) for k, (o, sz, c) in enumerate(enc.stripe_table()) if c])
-    with Session(w, h, rc_mode=rc_mode, crf=qp, bitrate_kbps=kbps or 8000, fps=fps, slice_rows=slice_rows, gop=-1,
-                 stripe_rows=stripe_rows, header_mode=header_mode, paintover_trigger_frames=paint[0], paintover_crf=paint[1]) as s:
-        for i, f in enumerate(frames):
-            if i in idr_at and i > 0:
-                s.flush()
-                s.request_idr()
-            s.submit(f)
-        s.flush()
-        got = s.take_frames()
-        grec = s.recon()
-    return got, ref, grec, enc.recon()
-
-
-def group(got, n_pictures):
-    per = [[] for _ in range(n_pictures)]
-    for g in got:
-        per[g.frame_id].append(g)
-    return per
 
 
 def frames_with_static_top(w, h, n):
@@ -48,24 +19,19 @@ def frames_with_static_top(w, h, n):
     return frames
 
 
+def encode(w, h, frames, stripe_rows, slice_rows, idr_at=(), **cfg):
+    """Both encoders over `frames` in striped mode; returns the oracle's Expected records."""
+    cfg = S.Config(w, h, stripe_rows=stripe_rows, slice_rows=slice_rows, **cfg)
+    return S.pictures(S.run(cfg, S.stream(frames, idr_at)))
+
+
 @pytest.mark.parametrize("w,h,stripe_rows,slice_rows", [(320, 200, 4, 1), (320, 200, 4, 2), (320, 200, 6, 3), (192, 112, 1, 1), (640, 360, 8, 1), (320, 200, 4, 0), (640, 360, 6, 0)])
 def test_stripes_bit_exact(w, h, stripe_rows, slice_rows):
-    frames = frames_with_static_top(w, h, 5)
-    got, ref, grec, rrec = run_both(w, h, frames, stripe_rows, slice_rows, idr_at=(0, 3))
-    per = group(got, len(frames))
-    for i, (gp, rp) in enumerate(zip(per, ref)):
-        assert [(g.y_start, g.data) for g in gp] == rp, f"picture {i}"
-        for g in gp:
-            assert g.height == min(h, g.y_start + stripe_rows * 16) - g.y_start and g.is_key == (i in (0, 3))
-    assert np.array_equal(grec[0], rrec[0]) and np.array_equal(grec[1], rrec[1])
+    """Every band's bytes, height and key flag; every band's stream decodes on its own (checked by the driver)."""
+    xs = encode(w, h, frames_with_static_top(w, h, 5), stripe_rows, slice_rows, idr_at=(3,))
+    assert [x.is_key for x in xs] == [True, False, False, True, False]
     if (w, stripe_rows) == (320, 4):
-        assert all(g.y_start >= 64 for g in per[1])           # the static band is not sent
-    # every stripe is a stream of its own
-    for y0 in sorted({g.y_start for g in got}):
-        st = [g.data for g in got if g.y_start == y0]
-        Y, U, V = avdec.decode_stream(st, quiet=True)[-1]
-        y1 = min(h, y0 + stripe_rows * 16)
-        assert np.array_equal(Y, grec[0][y0:y1, :w]) and np.array_equal(U, grec[1][y0 // 2: y1 // 2, 0:w:2])
+        assert all(y0 >= 64 for y0, _ in xs[1].bands)          # the static band is not sent
 
 
 def test_stripes_subpel_motion_stays_inside_the_band():
@@ -78,29 +44,13 @@ def test_stripes_subpel_motion_stays_inside_the_band():
     for t in range(4):
         a = cv2.warpAffine(big, np.float32([[1, 0, -(24 + 0.75 * t)], [0, 1, -(24 + 3.25 * t)]]), (w, h), flags=cv2.INTER_CUBIC)
         frames.append(np.dstack([np.clip(a, 0, 255).astype(np.uint8), np.full((h, w), 255, np.uint8)]))
-    got, ref, grec, rrec = run_both(w, h, frames, rows, 1, qp=26)
-    per = group(got, len(frames))
-    for gp, rp in zip(per, ref):
-        assert [(g.y_start, g.data) for g in gp] == rp
-    assert np.array_equal(grec[0], rrec[0]) and np.array_equal(grec[1], rrec[1])
-    for y0 in range(0, h, rows * 16):
-        Y, _, _ = avdec.decode_stream([g.data for g in got if g.y_start == y0], quiet=True)[-1]
-        assert np.array_equal(Y, grec[0][y0: y0 + rows * 16, :w])
+    encode(w, h, frames, rows, 1, qp=26)
 
 
 def test_stripes_cbr_and_pixelflux_header():
     w, h, rows = 320, 200, 4
-    frames = frames_with_static_top(w, h, 8)
-    got, ref, grec, rrec = run_both(w, h, frames, rows, 1, rc_mode=N.B2V_RC_CBR, kbps=900, header_mode=N.B2V_HDR_PIXELFLUX)
-    per = group(got, len(frames))
-    for i, (gp, rp) in enumerate(zip(per, ref)):
-        assert [(g.y_start, g.data[10:]) for g in gp] == rp, f"picture {i}"
-        for g in gp:
-            d = g.data
-            assert d[0] == 0x04 and d[1] == (1 if i == 0 else 0) and int.from_bytes(d[2:4], "big") == i
-            assert int.from_bytes(d[4:6], "big") == g.y_start and int.from_bytes(d[6:8], "big") == w and int.from_bytes(d[8:10], "big") == g.height
-    assert np.array_equal(grec[0], rrec[0])
-    assert len({g.qp for g in got}) > 1
+    xs = encode(w, h, frames_with_static_top(w, h, 8), rows, 1, rc_mode=S.CBR, kbps=900, fps=30.0, header_mode=S.HDR_PIXELFLUX)
+    assert [x.is_key for x in xs] == [True] + [False] * 7 and len({x.qp for x in xs}) > 1
 
 
 def test_stripe_rows_must_be_a_multiple_of_slice_rows():

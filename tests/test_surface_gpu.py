@@ -14,6 +14,7 @@ from selkies_b200.media_pipeline import MediaPipelineB200, RateControlMode
 from selkies_b200.pixelflux_compat import ArraySource, CaptureSettings, ScreenCapture, StripeCallback
 from selkies_b200 import _native as N
 from selkies_b200.session import Session
+from tests import scenario as S
 from tests import synth
 from tests.test_h264_oracle import split_nals
 
@@ -125,19 +126,7 @@ def test_gst_webrtc_app_facade():
 
 
 def test_scaled_encode_matches_oracle():
-    sw, sh, dw, dh = 640, 360, 320, 180
-    from selkies_b200 import _native as N
-    from selkies_b200.session import Session
-    frames = [synth.desktop(sw, sh, t) for t in range(3)]
-    enc = oracle.RefEncoder(dw, dh)
-    with Session(sw, sh, dst_width=dw, dst_height=dh, rc_mode=N.B2V_RC_CQP, crf=29) as s:
-        for f in frames:
-            s.submit(f)
-        s.flush()
-        got = s.take_frames()
-    for i, f in enumerate(frames):
-        y, uv = oracle.csc_nv12(f, dst_w=dw, dst_h=dh, coded_w=enc.cw, coded_h=enc.ch)
-        assert got[i].data == enc.encode_nv12(y, uv, i == 0, qp=29)
+    S.run(S.Config(640, 360, 320, 180, qp=29), [S.picture(synth.desktop(640, 360, t)) for t in range(3)])
 
 
 def test_two_concurrent_sessions_are_independent():
