@@ -82,8 +82,10 @@ typedef struct b2v_settings {
                                delivered.  0 or >= picture rows = full frame */
   int32_t idr_slice_mbs;    /* IDR pictures only (whatever slice_rows is): macroblocks per slice INSIDE a row.  The macroblocks of an
                                intra slice are a serial chain (left-neighbour prediction), so shorter slices shorten the chain the
-                               GPU has to walk (a 4K key frame: 3.3 ms with whole rows).  0 = default (about 540 slices per
-                               picture, none under 30 macroblocks: 60 at 4K, 30 at 1080p), < 0 = whole rows, n = n macroblocks */
+                               GPU has to walk.  0 = default (about 540 slices per picture, none under 30 macroblocks: 60 at 4K,
+                               30 at 1080p), n > 0 = n macroblocks per slice (n >= the picture's width in macroblocks: one slice
+                               per row).  Negative values are rejected: b2v_create fails with B2V_EINVAL.  (Earlier builds of
+                               this ABI version took a negative value to mean slices of whole rows.) */
   int32_t paintover_burst_frames;   /* CaptureSettings.h264_paintover_burst_frames (selkies.py:3217): how many consecutive
                                        pictures are coded at paintover_crf once the trigger is reached; <= 0 = 1 */
 } b2v_settings;

@@ -133,9 +133,10 @@ class RefEncoder:
         return [tuple(int(v) for v in t[3 * i: 3 * i + 3]) for i in range(n)]
 
     def set_idr_slice_mbs(self, n: int) -> None:
-        """Slices of IDR pictures: n > 0 macroblocks per slice inside a row, n < 0 whole rows, 0 = the default rule."""
+        """Slices of IDR pictures: n > 0 macroblocks per slice inside a row, 0 = the default rule."""
         self.L.b2v_ref_enc_set_idr_slice_mbs.argtypes = [C.c_void_p, C.c_int]
-        self.L.b2v_ref_enc_set_idr_slice_mbs(self.h, n)
+        if self.L.b2v_ref_enc_set_idr_slice_mbs(self.h, n) < 0:
+            raise ValueError("idr_slice_mbs must be >= 0")
 
     def set_paintover(self, trigger_frames: int, qp: int, burst_frames: int = 1) -> None:
         self.L.b2v_ref_enc_set_paintover(self.h, trigger_frames, qp)

@@ -99,11 +99,12 @@ typedef struct {
 #define MAX_STRIPES 512
 #define DEFAULT_SLICE_ROWS 8
 typedef struct {
-  int width, height, cw, ch, mbw, mbh, slice_rows, n_slices, auto_rows;
-  /* IDR pictures may be cut finer than rows: slices of `seg_cols` macroblocks inside a row (whatever slice_rows is: that one governs P pictures).  The
+  int width, height, cw, ch, mbw, mbh, slice_rows, auto_rows;
+  /* IDR pictures are cut into slices of `seg_cols` macroblocks inside a row (whatever slice_rows is: that one governs P pictures).  The
    * macroblocks of an intra slice are a serial chain (left-neighbour prediction), so shorter slices = a shorter chain on the
-   * GPU (DESIGN.md §5.2).  pic_seg is the value in force for the picture being coded (0 = whole rows). */
-  int seg_cols, pic_seg;
+   * GPU (DESIGN.md §5.2).  The slices of the picture being coded are a grid of pic_rows x pic_cols macroblocks in raster order:
+   * slice_rows x mbw for P pictures, 1 x seg_cols for IDR pictures. */
+  int seg_cols, pic_rows, pic_cols;
   uint8_t* recon[2];      /* NV12, coded size; recon[cur] is being written, recon[cur^1] is the reference */
   int cur;
   mb_t* mbs;
@@ -271,11 +272,21 @@ static int count_nz(const int16_t* l, int from, int to) { int n = 0; for (int k 
 static uint8_t* plane_y(enc_t* e, int idx) { return e->recon[idx]; }
 static uint8_t* plane_uv(enc_t* e, int idx) { return e->recon[idx] + (size_t)e->cw * e->ch; }
 
-static int slice_first_row(const enc_t* e, int mby) { return (mby / e->slice_rows) * e->slice_rows; }
-static int avail_top(const enc_t* e, int mby) { return e->pic_seg ? 0 : mby > slice_first_row(e, mby); }
-static int avail_left(const enc_t* e, int mbx) { return e->pic_seg ? (mbx % e->pic_seg) != 0 : mbx > 0; }
-static int pic_segs(const enc_t* e) { return e->pic_seg ? (e->mbw + e->pic_seg - 1) / e->pic_seg : 1; }
-static int pic_n_slices(const enc_t* e) { return e->pic_seg ? e->mbh * pic_segs(e) : e->n_slices; }
+static int avail_top(const enc_t* e, int mby) { return mby % e->pic_rows != 0; }
+static int avail_left(const enc_t* e, int mbx) { return mbx % e->pic_cols != 0; }
+static int slices_per_row(const enc_t* e) { return (e->mbw + e->pic_cols - 1) / e->pic_cols; }
+static int pic_n_slices(const enc_t* e) { return (e->mbh + e->pic_rows - 1) / e->pic_rows * slices_per_row(e); }
+/* slice s of the picture being coded: macroblock rows [row0, row1) x columns [x0, x1) */
+typedef struct { int row0, row1, x0, x1; } rect_t;
+static rect_t slice_rect(const enc_t* e, int s) {
+  const int per_row = slices_per_row(e);
+  rect_t r;
+  r.row0 = s / per_row * e->pic_rows; r.row1 = r.row0 + e->pic_rows;
+  r.x0 = s % per_row * e->pic_cols; r.x1 = r.x0 + e->pic_cols;
+  if (r.row1 > e->mbh) r.row1 = e->mbh;
+  if (r.x1 > e->mbw) r.x1 = e->mbw;
+  return r;
+}
 /* default IDR slicing: about 540 slices per picture, none shorter than 30 macroblocks */
 static int auto_seg_cols(int mbw, int mbh) {
   int segs = 540 / mbh, cap = mbw / 30;
@@ -1035,15 +1046,13 @@ static void write_slice_header(const enc_t* e, bitw_t* b, int first_mb, int idr,
 /* entropy-code one slice (7.3.4, 7.3.5) into a NAL appended at out; returns bytes written */
 static size_t code_slice(enc_t* e, int s, int idr, int qp, uint8_t* skip, uint8_t* out, int64_t* bits) {
   bitw_t b; bw_init(&b);
-  int row0 = s * e->slice_rows, row1 = row0 + e->slice_rows, x0 = 0, x1 = e->mbw;
-  if (e->pic_seg) { const int segs = pic_segs(e); row0 = s / segs; row1 = row0 + 1; x0 = (s % segs) * e->pic_seg; x1 = x0 + e->pic_seg; if (x1 > e->mbw) x1 = e->mbw; }
-  if (row1 > e->mbh) row1 = e->mbh;
-  int br0, br1; band_rows(e, row0, &br0, &br1);
-  const int first_nal_of_au = row0 == br0 && x0 == 0 && !idr;     /* 4-byte start code opens each band's access unit */
-  write_slice_header(e, &b, (row0 - br0) * e->mbw + x0, idr, qp, idr ? 0 : e->stripe_rows ? e->stripe_fn[row0 / e->stripe_rows] : e->frame_num);
+  const rect_t r = slice_rect(e, s);
+  int br0, br1; band_rows(e, r.row0, &br0, &br1);
+  const int first_nal_of_au = r.row0 == br0 && r.x0 == 0 && !idr;     /* 4-byte start code opens each band's access unit */
+  write_slice_header(e, &b, (r.row0 - br0) * e->mbw + r.x0, idr, qp, idr ? 0 : e->stripe_rows ? e->stripe_fn[r.row0 / e->stripe_rows] : e->frame_num);
   int skip_run = 0;
-  for (int mby = row0; mby < row1; mby++)
-    for (int mbx = x0; mbx < x1; mbx++) {
+  for (int mby = r.row0; mby < r.row1; mby++)
+    for (int mbx = r.x0; mbx < r.x1; mbx++) {
       const mb_t* m = &e->mbs[mby * e->mbw + mbx];
       if (!idr) {
         int sp[2];
@@ -1195,7 +1204,6 @@ void* b2v_ref_enc_create(int width, int height, int slice_rows) {
    * IDR pictures have their own, finer slicing (seg_cols below) whatever slice_rows is. */
   e->auto_rows = slice_rows <= 0;
   e->slice_rows = slice_rows > 0 ? slice_rows : (e->mbh < DEFAULT_SLICE_ROWS ? e->mbh : DEFAULT_SLICE_ROWS);
-  e->n_slices = (e->mbh + e->slice_rows - 1) / e->slice_rows;
   size_t fb = (size_t)e->cw * e->ch * 3 / 2;
   e->recon[0] = (uint8_t*)calloc(fb, 1); e->recon[1] = (uint8_t*)calloc(fb, 1);
   e->mbs = (mb_t*)calloc((size_t)e->mbw * e->mbh, sizeof(mb_t));
@@ -1224,17 +1232,19 @@ int b2v_ref_enc_rc_state(void* h, int64_t* out) {
   return 0;
 }
 void b2v_ref_enc_set_paintover(void* h, int trigger_frames, int qp) { enc_t* e = (enc_t*)h; e->paint_trigger = trigger_frames; e->paint_qp = qp; }
-/* slices of IDR pictures: n > 0 macroblocks per slice inside a row, n < 0 slices of slice_rows whole rows as in P pictures, 0 = the default rule */
-void b2v_ref_enc_set_idr_slice_mbs(void* h, int n) {
+/* slices of IDR pictures: n > 0 macroblocks per slice inside a row, 0 = the default rule.  Returns 0, or -1 for n < 0 (setting unchanged). */
+int b2v_ref_enc_set_idr_slice_mbs(void* h, int n) {
   enc_t* e = (enc_t*)h;
-  e->seg_cols = n < 0 ? 0 : n == 0 ? auto_seg_cols(e->mbw, e->mbh) : n >= e->mbw ? e->mbw : n;
+  if (n < 0) return -1;
+  e->seg_cols = n == 0 ? auto_seg_cols(e->mbw, e->mbh) : n >= e->mbw ? e->mbw : n;
+  return 0;
 }
 void b2v_ref_enc_set_paintover_burst(void* h, int burst_frames) { ((enc_t*)h)->paint_burst = burst_frames > 0 ? burst_frames : 1; }
 /* striped mode: stripe_rows macroblock rows per band (a multiple of slice_rows); 0 = full frame.  Returns the band count or -1. */
 int b2v_ref_enc_set_stripes(void* h, int stripe_rows) {
   enc_t* e = (enc_t*)h;
   if (stripe_rows <= 0 || stripe_rows >= e->mbh) { e->stripe_rows = 0; e->n_stripes = 1; return 1; }
-  if (e->auto_rows) { e->slice_rows = stripe_rows; e->n_slices = (e->mbh + e->slice_rows - 1) / e->slice_rows; }   /* default: one slice per band */
+  if (e->auto_rows) e->slice_rows = stripe_rows;   /* default: one slice per band */
   if (stripe_rows % e->slice_rows) return -1;
   const int n = (e->mbh + stripe_rows - 1) / stripe_rows;
   if (n > MAX_STRIPES) return -1;
@@ -1265,7 +1275,7 @@ int64_t b2v_ref_enc_encode(void* h, const uint8_t* cur_nv12, int idr, int rc_mod
   const struct rcfb used = e->fb[k];                         /* the controller state after picture pic-2 */
   const int qp = rc_frame_qp(e, &used, idr, rc_mode, qp_fixed, target_bits);
   e->cur ^= 1;
-  e->pic_seg = idr ? e->seg_cols : 0;
+  e->pic_rows = idr ? 1 : e->slice_rows; e->pic_cols = idr ? e->seg_cols : e->mbw;
   const int nsl = pic_n_slices(e);
   if (idr) { e->frame_num = 0; }
   /* phase A: analysis + reconstruction.  Intra: macroblocks of a slice are sequential (left/top
@@ -1273,11 +1283,9 @@ int64_t b2v_ref_enc_encode(void* h, const uint8_t* cur_nv12, int idr, int rc_mod
   if (idr) {
 #pragma omp parallel for schedule(dynamic, 1)
     for (int s = 0; s < nsl; s++) {
-      int row0 = s * e->slice_rows, row1 = (s + 1) * e->slice_rows, x0 = 0, x1 = e->mbw;
-      if (e->pic_seg) { const int segs = pic_segs(e); row0 = s / segs; row1 = row0 + 1; x0 = (s % segs) * e->pic_seg; x1 = x0 + e->pic_seg; if (x1 > e->mbw) x1 = e->mbw; }
-      if (row1 > e->mbh) row1 = e->mbh;
-      for (int mby = row0; mby < row1; mby++)
-        for (int mbx = x0; mbx < x1; mbx++) encode_intra_mb(e, cur_nv12, mbx, mby, qp);
+      const rect_t r = slice_rect(e, s);
+      for (int mby = r.row0; mby < r.row1; mby++)
+        for (int mbx = r.x0; mbx < r.x1; mbx++) encode_intra_mb(e, cur_nv12, mbx, mby, qp);
     }
   } else {
     /* anchors first (their vectors are candidates for the rest of their groups), then everybody else */
@@ -1289,8 +1297,8 @@ int64_t b2v_ref_enc_encode(void* h, const uint8_t* cur_nv12, int idr, int rc_mod
   }
   /* phase B: entropy coding per slice, then concatenation */
   uint8_t* skip = (uint8_t*)calloc(mbs, 1);
-  size_t per = (size_t)e->slice_rows * e->mbw * 1024 + 256;
-  if (e->pic_seg) per = (size_t)e->pic_seg * 1024 + 256;
+  const rect_t full = slice_rect(e, 0);        /* slice 0 is a full-size slice */
+  const size_t per = (size_t)(full.row1 - full.row0) * (full.x1 - full.x0) * 1024 + 256;
   uint8_t* tmp = (uint8_t*)malloc(per * nsl);
   size_t* lens = (size_t*)calloc(nsl, sizeof(size_t));
   int64_t* sbits = (int64_t*)calloc(nsl, sizeof(int64_t));
@@ -1308,8 +1316,10 @@ int64_t b2v_ref_enc_encode(void* h, const uint8_t* cur_nv12, int idr, int rc_mod
       const int last = t == e->n_stripes - 1;
       const size_t o0 = o;
       if (idr) { memcpy(out + o, e->sps_band[last], e->sps_band_len[last]); o += e->sps_band_len[last]; memcpy(out + o, e->pps, e->pps_len); o += e->pps_len; }
-      const int s0 = e->pic_seg ? r0 * pic_segs(e) : r0 / e->slice_rows, s1 = e->pic_seg ? r1 * pic_segs(e) : (r1 + e->slice_rows - 1) / e->slice_rows;
-      for (int s = s0; s < s1; s++) { memcpy(out + o, tmp + per * s, lens[s]); o += lens[s]; bits += sbits[s]; }
+      for (int s = 0; s < nsl; s++) {
+        const int row0 = slice_rect(e, s).row0;
+        if (row0 >= r0 && row0 < r1) { memcpy(out + o, tmp + per * s, lens[s]); o += lens[s]; bits += sbits[s]; }
+      }
       int coded = idr;
       for (int i = r0 * e->mbw; i < r1 * e->mbw && !coded; i++) coded |= !skip[i];
       e->stripe_tab[t][0] = (int32_t)o0; e->stripe_tab[t][1] = (int32_t)(o - o0); e->stripe_tab[t][2] = coded;

@@ -543,6 +543,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   int dw = cfg->dst_w > 0 ? cfg->dst_w : sw, dh = cfg->dst_h > 0 ? cfg->dst_h : sh;
   if (!size_ok(sw, sh)) return fail(B2V_EINVAL, "source size %dx%d unsupported (even, 16..7680 x 16..4320)", sw, sh);
   if (!size_ok(dw, dh)) return fail(B2V_EINVAL, "encoded size %dx%d unsupported", dw, dh);
+  if (cfg->idr_slice_mbs < 0) return fail(B2V_EINVAL, "idr_slice_mbs %d out of range (0 = default, n > 0 macroblocks per slice)", cfg->idr_slice_mbs);
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(B2V_EINVAL, "device %d out of range (%d devices)", cfg->device, ndev);

@@ -54,8 +54,8 @@ __device__ const int32_t rc_qs[52] = {
 struct ChunkAgg; struct ChunkInc;
 struct FrameCtx {          // everything a kernel needs about the picture being coded
   int cw, ch, mbw, mbh, slice_rows, n_slices;   // n_slices: of THIS picture
-  int seg_cols;            // > 0 (IDR pictures): slices of seg_cols macroblocks inside a row, whatever slice_rows is — the macroblocks
-                           // of an intra slice are a serial chain, so shorter slices shorten the chain (DESIGN.md §5.2); 0 = whole rows
+  int slice_cols;          // this picture's slices are a grid of slice_rows x slice_cols macroblocks in raster order: P pictures
+                           // slice_rows x mbw, IDR pictures 1 x slice_cols, never more than one row (DESIGN.md §5.2)
   int idr, rc_mode, qp_fixed;
   int paint_trigger, paint_qp, paint_burst;   // paint-over: `paint_burst` refinement pictures after `paint_trigger` all-skipped pictures (0 = off)
   int pic;                 // picture counter of this encoder (parity selects the feedback record and the double-buffered side data)
@@ -78,8 +78,7 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   uint32_t* slice_size;    // [n_slices] final NAL bytes (start code + header + EP'd payload)
   uint32_t* slice_rbsp;    // [n_slices] RBSP bytes before emulation prevention
   long long* slice_bits;   // [n_slices]
-  int* progress;           // [mbh] intra wavefront progress counters
-  int chunks_per_slice;    // k_slice_build: blocks per slice (chunks of up to 256 macroblocks), set at launch
+  int chunks_per_slice;    // k_slice_build: blocks per slice (chunks of up to 256 macroblocks)
   struct ChunkAgg* chunk_agg; struct ChunkInc* chunk_inc;   // [chunks] look-back records of k_slice_build
   int* slice_done;         // [n_slices] chunks of the slice that have finished copying (reset by the last one)
   RcState* rc;
@@ -116,18 +115,16 @@ __device__ __forceinline__ int frame_qp(const FrameCtx& f) {
   if (paint && f.paint_qp < q) q = clip3i(0, 51, f.paint_qp);
   return q;
 }
-// slice geometry (mirrors oracle/h264_ref.c avail_top / avail_left / code_slice)
-__device__ __forceinline__ bool top_in_slice(const FrameCtx& f, int mby) { return f.seg_cols ? false : (mby % f.slice_rows) != 0; }
-__device__ __forceinline__ bool left_in_slice(const FrameCtx& f, int mbx) { return f.seg_cols ? (mbx % f.seg_cols) != 0 : mbx > 0; }
-__device__ __forceinline__ int segs_per_row(const FrameCtx& f) { return f.seg_cols ? (f.mbw + f.seg_cols - 1) / f.seg_cols : 1; }
-__device__ __forceinline__ int slice_of(const FrameCtx& f, int mbx, int mby) { return f.seg_cols ? mby * segs_per_row(f) + mbx / f.seg_cols : mby / f.slice_rows; }
+// slice geometry (mirrors oracle/h264_ref.c slice_rect / avail_top / avail_left)
+__device__ __forceinline__ bool top_in_slice(const FrameCtx& f, int mby) { return mby % f.slice_rows != 0; }
+__device__ __forceinline__ bool left_in_slice(const FrameCtx& f, int mbx) { return mbx % f.slice_cols != 0; }
+__device__ __forceinline__ int slices_per_row(const FrameCtx& f) { return (f.mbw + f.slice_cols - 1) / f.slice_cols; }
 struct SliceGeo { int row0, row1, x0, x1, mb0, n_mb; };      // macroblock rows [row0,row1) x columns [x0,x1); mb0 = first macroblock
 __device__ __forceinline__ SliceGeo slice_geo(const FrameCtx& f, int s) {
+  const int per_row = slices_per_row(f), r = s / per_row;
   SliceGeo g;
-  if (f.seg_cols) {
-    const int segs = segs_per_row(f);
-    g.row0 = s / segs; g.row1 = g.row0 + 1; g.x0 = (s - g.row0 * segs) * f.seg_cols; g.x1 = min(f.mbw, g.x0 + f.seg_cols);
-  } else { g.row0 = s * f.slice_rows; g.row1 = min(f.mbh, g.row0 + f.slice_rows); g.x0 = 0; g.x1 = f.mbw; }
+  g.row0 = r * f.slice_rows; g.row1 = min(f.mbh, g.row0 + f.slice_rows);
+  g.x0 = (s - r * per_row) * f.slice_cols; g.x1 = min(f.mbw, g.x0 + f.slice_cols);
   g.mb0 = g.row0 * f.mbw + g.x0; g.n_mb = (g.row1 - g.row0) * (g.x1 - g.x0);
   return g;
 }

@@ -18,10 +18,18 @@ namespace b2v {
 static thread_local char g_enc_err[256] = "";
 const char* encoder_last_error() { return g_enc_err; }
 
+// The slices of a picture: a grid of rows x cols macroblocks (FrameCtx::slice_rows / slice_cols)
+struct SliceGrid {
+  int rows = 0, cols = 0;
+  int n = 0;               // slices per picture
+  int words = 0;           // RBSP scratch words per slice
+  int chunks = 0;          // k_slice_build blocks per slice: chunks of up to 256 macroblocks
+};
+
 struct Encoder {
   EncoderConfig cfg{};
-  int mbw = 0, mbh = 0, n_slices = 0;
-  int seg_cols = 0, n_seg_slices = 0, seg_slice_words = 0;   // IDR pictures: sub-row slices (0 = whole rows)
+  int mbw = 0, mbh = 0;
+  SliceGrid p_grid, idr_grid;
   uint8_t* recon[2] = {nullptr, nullptr};
   int cur = 0;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
@@ -34,8 +42,6 @@ struct Encoder {
   unsigned long long* me_pub = nullptr;   // anchor macroblocks' vectors of the picture being analysed (h264_inter.cu)
   uint32_t *mb_words = nullptr, *mb_nbits = nullptr, *slice_buf = nullptr, *slice_size = nullptr, *slice_rbsp = nullptr;
   long long* slice_bits = nullptr;
-  int slice_words = 0;
-  int* progress = nullptr;
   int* overflow = nullptr;
   RcState* rc = nullptr;
   uint8_t* param_sets = nullptr; int param_len = 0, param_len_last = 0;
@@ -72,6 +78,15 @@ void append_nal(std::vector<uint8_t>& out, int ref_idc, int type, const std::vec
     out.push_back(b);
     zeros = b == 0 ? zeros + 1 : 0;
   }
+}
+
+SliceGrid slice_grid(int mbw, int mbh, int rows, int cols) {
+  SliceGrid g;
+  g.rows = rows; g.cols = cols;
+  g.n = (mbh + rows - 1) / rows * ((mbw + cols - 1) / cols);
+  g.words = rows * cols * MB_WORDS + 64;
+  g.chunks = (rows * cols + 255) / 256;
+  return g;
 }
 
 int level_idc_for(int mbs) { return mbs <= 3600 ? 31 : mbs <= 8704 ? 42 : mbs <= 22080 ? 51 : mbs <= 36864 ? 52 : 62; }
@@ -129,7 +144,7 @@ std::vector<uint8_t> make_param_sets(const EncoderConfig& c, int mbw, int mbh, i
   } while (0)
 
 int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
-  if (!cfg_in || !out || (cfg_in->coded_w & 15) || (cfg_in->coded_h & 15)) {
+  if (!cfg_in || !out || (cfg_in->coded_w & 15) || (cfg_in->coded_h & 15) || cfg_in->idr_slice_mbs < 0) {
     snprintf(g_enc_err, sizeof g_enc_err, "bad encoder config");
     return -1;
   }
@@ -138,13 +153,19 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   e->mbw = cfg_in->coded_w / 16; e->mbh = cfg_in->coded_h / 16;
   // slice_rows <= 0: the default rule (oracle/h264_ref.c b2v_ref_enc_create): P pictures in slices of 8 macroblock rows, one slice per
   // band in striped mode — inside a slice the row above predicts the motion vector and P_Skip infers a moving one, which halves the
-  // bytes of a scrolling picture against one row per slice.  IDR pictures are sliced on their own (seg_cols below).
+  // bytes of a scrolling picture against one row per slice.  IDR pictures are sliced on their own (idr_grid below).
   if (e->cfg.slice_rows <= 0) {
     const bool striped = e->cfg.stripe_rows > 0 && e->cfg.stripe_rows < e->mbh;
     e->cfg.slice_rows = striped ? e->cfg.stripe_rows : (e->mbh < 8 ? e->mbh : 8);
   }
   const EncoderConfig* cfg = &e->cfg;
-  e->n_slices = (e->mbh + cfg->slice_rows - 1) / cfg->slice_rows;
+  e->p_grid = slice_grid(e->mbw, e->mbh, cfg->slice_rows, e->mbw);
+  {   // IDR pictures: slices inside a row (same rule as oracle/h264_ref.c auto_seg_cols: about 540 slices, none under 30 macroblocks)
+    int cols = cfg->idr_slice_mbs;
+    if (cols == 0) { int segs = 540 / e->mbh; const int cap = e->mbw / 30; if (segs > cap) segs = cap; cols = segs <= 1 ? e->mbw : (e->mbw + segs - 1) / segs; }
+    if (cols >= e->mbw) cols = e->mbw;          // one slice per macroblock row
+    e->idr_grid = slice_grid(e->mbw, e->mbh, 1, cols);
+  }
   const size_t mbs = (size_t)e->mbw * e->mbh, fb = (size_t)cfg->coded_w * cfg->coded_h * 3 / 2;
   ECK(cudaMalloc((void**)&e->recon[0], fb));
   ECK(cudaMalloc((void**)&e->recon[1], fb));
@@ -164,32 +185,21 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   ECK(cudaMemset(e->me_pub, 0, mbs * sizeof(unsigned long long)));
   ECK(cudaMalloc((void**)&e->mb_words, mbs * MB_WORDS * sizeof(uint32_t)));
   ECK(cudaMalloc((void**)&e->mb_nbits, mbs * sizeof(uint32_t)));
-  e->slice_words = cfg->slice_rows * e->mbw * MB_WORDS + 64;
-  // IDR pictures: slices shorter than a row (same rule as oracle/h264_ref.c auto_seg_cols: about 540 slices, none under 30 macroblocks)
-  // (idr_slice_mbs < 0: IDR pictures in slices of slice_rows whole rows, like P pictures — rows of a slice then wait on the row above)
-  if (cfg->idr_slice_mbs >= 0) {
-    int cols = cfg->idr_slice_mbs;
-    if (cols == 0) { int segs = 540 / e->mbh; const int cap = e->mbw / 30; if (segs > cap) segs = cap; cols = segs <= 1 ? e->mbw : (e->mbw + segs - 1) / segs; }
-    if (cols >= e->mbw) cols = e->mbw;          // one slice per macroblock row
-    e->seg_cols = cols;
-  }
-  if (e->seg_cols) { e->n_seg_slices = e->mbh * ((e->mbw + e->seg_cols - 1) / e->seg_cols); e->seg_slice_words = e->seg_cols * MB_WORDS + 64; }
-  const size_t nsl_max = (size_t)(e->n_seg_slices > e->n_slices ? e->n_seg_slices : e->n_slices);
-  size_t sb_words = (size_t)e->n_slices * e->slice_words;
-  if ((size_t)e->n_seg_slices * e->seg_slice_words > sb_words) sb_words = (size_t)e->n_seg_slices * e->seg_slice_words;
+  // slice buffers serve either grid
+  const SliceGrid &gp = e->p_grid, &gi = e->idr_grid;
+  const size_t nsl_max = (size_t)std::max(gp.n, gi.n);
+  const size_t sb_words = std::max((size_t)gp.n * gp.words, (size_t)gi.n * gi.words);
   ECK(cudaMalloc((void**)&e->slice_buf, sb_words * sizeof(uint32_t)));
   ECK(cudaMemset(e->slice_buf, 0, sb_words * sizeof(uint32_t)));
   ECK(cudaMalloc((void**)&e->slice_size, nsl_max * sizeof(uint32_t)));
   ECK(cudaMalloc((void**)&e->slice_rbsp, nsl_max * sizeof(uint32_t)));
   ECK(cudaMalloc((void**)&e->slice_bits, nsl_max * sizeof(long long)));
-  {   // k_slice_build's look-back records: one per chunk of up to 256 macroblocks (32 bytes cover either record type)
-    const size_t cps_row = ((size_t)cfg->slice_rows * e->mbw + 255) / 256, cps_seg = e->seg_cols ? ((size_t)e->seg_cols + 255) / 256 : 0;
-    const size_t chunks = std::max((size_t)e->n_slices * cps_row, (size_t)e->n_seg_slices * cps_seg) + 1;
+  {   // k_slice_build's look-back records: one per chunk (32 bytes cover either record type)
+    const size_t chunks = std::max((size_t)gp.n * gp.chunks, (size_t)gi.n * gi.chunks) + 1;
     ECK(cudaMalloc((void**)&e->chunk_agg, chunks * 32)); ECK(cudaMemset(e->chunk_agg, 0, chunks * 32));
     ECK(cudaMalloc((void**)&e->chunk_inc, chunks * 32)); ECK(cudaMemset(e->chunk_inc, 0, chunks * 32));
     ECK(cudaMalloc((void**)&e->slice_done, nsl_max * sizeof(int))); ECK(cudaMemset(e->slice_done, 0, nsl_max * sizeof(int)));
   }
-  ECK(cudaMalloc((void**)&e->progress, e->mbh * sizeof(int)));
   ECK(cudaMalloc((void**)&e->overflow, sizeof(int)));
   ECK(cudaMemset(e->overflow, 0, sizeof(int)));
   ECK(cudaMalloc((void**)&e->rc, sizeof(RcState)));
@@ -227,7 +237,7 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
 void encoder_destroy(Encoder* e) {
   if (!e) return;
   void* ptrs[] = {e->recon[0], e->recon[1], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
-                  e->slice_size, e->slice_rbsp, e->slice_bits, e->progress, e->overflow, e->rc, e->param_sets, e->i4modes[0],
+                  e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->chunk_agg, e->chunk_inc, e->slice_done};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
@@ -249,21 +259,21 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   if (idr) e->frame_num = 0;
   FrameCtx f{};
   f.cw = e->cfg.coded_w; f.ch = e->cfg.coded_h; f.mbw = e->mbw; f.mbh = e->mbh;
-  const bool seg = idr && e->seg_cols > 0;
-  f.slice_rows = e->cfg.slice_rows; f.n_slices = seg ? e->n_seg_slices : e->n_slices; f.seg_cols = seg ? e->seg_cols : 0;
+  const SliceGrid& g = idr ? e->idr_grid : e->p_grid;
+  f.slice_rows = g.rows; f.slice_cols = g.cols; f.n_slices = g.n; f.slice_words = g.words; f.chunks_per_slice = g.chunks;
   f.idr = idr; f.rc_mode = p->rc_mode; f.qp_fixed = p->qp_fixed; f.target_bits = p->target_bits;
   f.frame_num = e->frame_num; f.idr_pic_id = e->idr_count; f.pic = (int)(e->pic & 0x7fffffff);
   f.cur = p->cur; f.ref = e->recon[e->cur ^ 1]; f.recon = e->recon[e->cur];
   f.mbinfo = e->mbinfo[par]; f.mbinfo_prev = e->mbinfo[par ^ 1]; f.i4modes = e->i4modes[par]; f.coef = e->coef[par]; f.nnz = e->nnz[par];
   f.me_pub = e->me_pub;
-  f.chunk_agg = (ChunkAgg*)e->chunk_agg; f.chunk_inc = (ChunkInc*)e->chunk_inc; f.slice_done = e->slice_done; f.chunks_per_slice = 1;
+  f.chunk_agg = (ChunkAgg*)e->chunk_agg; f.chunk_inc = (ChunkInc*)e->chunk_inc; f.slice_done = e->slice_done;
   {   // anchors: ceil(mbw/4) columns x (groups of 4 rows inside every band)
     const int rows_last = e->mbh - (e->n_bands - 1) * e->band_rows;
     f.n_anchor = ((e->mbw + 3) / 4) * ((e->n_bands - 1) * ((e->band_rows + 3) / 4) + (rows_last + 3) / 4);
   }
   f.mb_words = e->mb_words; f.mb_nbits = e->mb_nbits;
-  f.slice_buf = e->slice_buf; f.slice_words = seg ? e->seg_slice_words : e->slice_words; f.slice_size = e->slice_size; f.slice_rbsp = e->slice_rbsp;
-  f.slice_bits = e->slice_bits; f.paint_trigger = p->paint_trigger; f.paint_qp = p->paint_qp; f.paint_burst = p->paint_burst; f.progress = e->progress; f.rc = e->rc;
+  f.slice_buf = e->slice_buf; f.slice_size = e->slice_size; f.slice_rbsp = e->slice_rbsp;
+  f.slice_bits = e->slice_bits; f.paint_trigger = p->paint_trigger; f.paint_qp = p->paint_qp; f.paint_burst = p->paint_burst; f.rc = e->rc;
   f.band_rows = e->band_rows; f.n_bands = e->n_bands; f.striped = e->striped; f.param_len_last = e->param_len_last;
   f.band_fn = e->band_fn; f.band_coded = e->band_coded; f.au_data_off = e->au_data_off;
   f.param_sets = e->param_sets; f.param_len = e->param_len; f.csc_ts = p->csc_ts; f.au = p->au; f.overflow = e->overflow;

@@ -16,7 +16,7 @@ struct EncoderConfig {
   int coded_w, coded_h;    // multiples of 16
   int slice_rows;          // macroblock rows per slice
   int stripe_rows;         // macroblock rows per band (multiple of slice_rows); 0 = full-frame
-  int idr_slice_mbs;       // IDR pictures: macroblocks per slice inside a row (needs slice_rows == 1); 0 = default rule, < 0 = whole rows
+  int idr_slice_mbs;       // IDR pictures, whatever slice_rows is: macroblocks per slice inside a row; 0 = default rule (>= 0)
 };
 
 struct EncodeFrameParams {

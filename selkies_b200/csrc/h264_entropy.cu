@@ -325,6 +325,8 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cps = f.chunks_per_slice, s = blockIdx.x / cps, k = blockIdx.x - s * cps;
   const SliceGeo geo = slice_geo(f, s);
+  const int band = geo.row0 / f.band_rows, first_mb = geo.mb0 - band * f.band_rows * f.mbw;
+  const int fn = f.idr ? 0 : f.striped ? f.band_fn[band] : f.frame_num;
   const int n_chunks = (geo.n_mb + SLICE_THREADS - 1) / SLICE_THREADS;
   const int tag = f.pic + 1, qp = frame_qp(f);
   uint32_t* out = f.slice_buf + (size_t)s * f.slice_words;
@@ -374,8 +376,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       long long bits; int trail = 0; bool ok = true;
       {
         CountSink h;
-        const int band = geo.row0 / f.band_rows;
-        slice_header(h, f, geo.mb0 - band * f.band_rows * f.mbw, qp, f.idr ? 0 : f.striped ? f.band_fn[band] : f.frame_num);
+        slice_header(h, f, first_mb, qp, fn);
         bits = h.n;
       }
       int start = 0;
@@ -451,8 +452,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       *reinterpret_cast<volatile int*>(&c->flag) = tag;
       if (k == 0) {                              // slice header (the bits it occupies were counted above)
         GlobalSink g{out, 0};
-        const int band = geo.row0 / f.band_rows;
-        slice_header(g, f, geo.mb0 - band * f.band_rows * f.mbw, qp, f.idr ? 0 : f.striped ? f.band_fn[band] : f.frame_num);
+        slice_header(g, f, first_mb, qp, fn);
       }
       if (last_chunk) {                          // trailing mb_skip_run, rbsp_trailing_bits
         GlobalSink g{out, s_bits_out};
@@ -461,7 +461,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
         f.slice_bits[s] = g.pos;
         if (runt < geo.n_mb) {                   // the slice holds a coded macroblock (benign races: every writer stores the same value)
           f.rc->pic_coded = 1;
-          if (f.striped) f.band_coded[geo.row0 / f.band_rows] = 1;
+          if (f.striped) f.band_coded[band] = 1;
         }
         g.put(1, 1);
         f.slice_rbsp[s] = (uint32_t)((g.pos + 7) >> 3);
@@ -579,9 +579,6 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
   __shared__ int s_wsum[PACK_THREADS / 32];
   __shared__ int s_carry;
   const int s = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // the controller has already moved on to the next picture (rc_step ran in k_slice_build, before this kernel and possibly on another
-  // stream): this picture's QP is the one it recorded
-  const int qp = f.rc->last_qp;
   // byte offset of this slice's NAL inside the access unit
   long long part = 0;
   for (int j = tid; j < s; j += PACK_THREADS) part += f.slice_size[j];
@@ -665,7 +662,7 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
     if (f.striped && tid == 0) {      // band table entry; the band's frame_num advances only if it is delivered
       long long sz = f.idr ? plen : 0;
       const int band_row1 = min(f.mbh, (band + 1) * f.band_rows);
-      const int s1 = min(f.n_slices, f.seg_cols ? band_row1 * segs_per_row(f) : (band_row1 + f.slice_rows - 1) / f.slice_rows);
+      const int s1 = min(f.n_slices, (band_row1 + f.slice_rows - 1) / f.slice_rows * slices_per_row(f));
       for (int j = s; j < s1; j++) sz += f.slice_size[j];
       const int coded = f.idr ? 1 : f.band_coded[band];
       const int fn = f.idr ? 0 : f.band_fn[band];
@@ -682,7 +679,9 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
       AuHeader* h = reinterpret_cast<AuHeader*>(f.au);
       int ovf = *f.overflow;
       if (total > cap) { ovf |= 2; total = cap; }
-      h->size = (int32_t)total; h->qp = qp; h->is_idr = f.idr; h->n_slices = f.n_slices; h->total_bits = bits;
+      // the controller has already moved on to the next picture (rc_step ran in k_slice_build, before this kernel and possibly on
+      // another stream): this picture's QP is the one it recorded
+      h->size = (int32_t)total; h->qp = f.rc->last_qp; h->is_idr = f.idr; h->n_slices = f.n_slices; h->total_bits = bits;
       h->overflow = ovf;
       h->next_qp = f.rc->fb[f.pic & 1].qp;         // the controller's decision for the picture two ahead
       h->csc_t0 = f.csc_ts ? f.csc_ts[0] : 0; h->csc_t1 = f.csc_ts ? f.csc_ts[1] : 0;
@@ -696,10 +695,7 @@ int launch_cavlc(const FrameCtx& f, cudaStream_t st) {
   return 1;
 }
 int launch_slice_build(const FrameCtx& f, cudaStream_t st) {
-  FrameCtx g = f;
-  const int full = f.seg_cols ? f.seg_cols : f.slice_rows * f.mbw;       // macroblocks of a full-size slice of this picture
-  g.chunks_per_slice = (full + SLICE_THREADS - 1) / SLICE_THREADS;
-  k_slice_build<<<f.n_slices * g.chunks_per_slice, SLICE_THREADS, 0, st>>>(g);      // scan + copy + emulation-prevention count
+  k_slice_build<<<f.n_slices * f.chunks_per_slice, SLICE_THREADS, 0, st>>>(f);      // scan + copy + emulation-prevention count
   return 1;
 }
 int launch_pack_cap(const FrameCtx& f, long long au_cap, cudaStream_t st) {

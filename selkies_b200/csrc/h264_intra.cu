@@ -1,11 +1,10 @@
 // h264_intra.cu — IDR pictures: Intra4x4 / Intra16x16 macroblocks (ITU-T H.264 8.3.1, 8.3.3 luma; 8.3.4 chroma).
 //
-// One block of TWO warps per macroblock ROW: intra prediction needs the reconstructed left neighbour, so the
-// macroblocks of a row are a serial chain; rows of the same slice additionally wait for the row above
-// (wavefront, two macroblocks of lag because Intra4x4 reads the above-right samples) through a progress
-// counter in global memory.  With the default slice_rows = 1 every row is its own slice and all rows run in parallel.
-// The chain is latency-bound (one dependent shuffle / shared-memory round trip after the other), so the two ways of
-// coding a macroblock run side by side: warp 0 codes Intra16x16 + chroma while warp 1 runs the Intra4x4 pass.
+// One block of THREE warps per slice.  IDR slices never span rows (a grid of 1 x slice_cols macroblocks, DESIGN.md §5.2), so
+// no macroblock has a neighbour above and no block depends on another.  Inside a slice intra prediction needs the reconstructed
+// left neighbour, so its macroblocks are a serial chain.  The chain is latency-bound (one dependent shuffle / shared-memory round
+// trip after the other), so the two ways of coding a macroblock run side by side: warp 0 codes Intra16x16 + chroma while
+// warps 1 and 2 run the Intra4x4 pass.
 //
 // Per macroblock the luma is coded BOTH ways and the better one kept:
 //   Intra4x4   16 blocks in decoding order; per block the 32 lanes evaluate 8 modes x 4 rows (+ horizontal-up)
@@ -24,14 +23,11 @@ constexpr int I4_SKIP_SAD_PER_LAMBDA = 32;   // Intra4x4 is only tried when the 
 
 __device__ __forceinline__ uint32_t rep4(int v) { return (uint32_t)v * 0x01010101u; }
 
-struct IntraNb {
-  uint8_t top_y[20];                         // 16 samples above the macroblock + 4 above-right
+struct IntraNb {                             // what a macroblock takes from its left neighbour (it has none above)
   uint8_t left_y[16];
-  uint8_t top_uv[16]; uint8_t left_uv[16];   // interleaved Cb,Cr: [x*2+c] / [y*2+c]
-  int tl_y, tl_u, tl_v;
+  uint8_t left_uv[16];                       // interleaved Cb,Cr: [y*2+c]
   int cdc[8];                                // chroma DC prediction per (comp*4 + blk)
   uint8_t left_modes[4];                     // Intra4x4PredMode of the left macroblock's right column (2 if it is not I4x4)
-  uint8_t top_modes[4];                      // ... of the above macroblock's bottom row
 };
 
 struct I4State {
@@ -72,8 +68,8 @@ __device__ __forceinline__ bool i4_mode_ok(int mode, bool has_a, bool has_b, boo
     default: return has_a && has_b && has_d;
   }
 }
-// (above-right availability inside the macroblock and the inverse zig-zag are nibble-packed literals in the kernel:
-//  raster { 2,2,2,3, 1,0,1,0, 1,1,1,0, 1,0,1,0 } with 1 = inside, 2 = macroblock above, 3 = above-right macroblock)
+// (above-right availability and the inverse zig-zag are packed literals in the kernel: the above-right samples of a block
+//  are available when they lie inside the macroblock, raster { 0,0,0,0, 1,0,1,0, 1,1,1,0, 1,0,1,0 } = bit mask 0x5750)
 
 // one 1-D stage of the forward / inverse core transform for the element `k` of (a,b,c,d)
 __device__ __forceinline__ int fwd1(int k, int a, int b, int c, int d) {
@@ -84,38 +80,23 @@ __device__ __forceinline__ int inv1(int k, int p0, int p1, int p2, int p3) {
   return k == 0 ? e0 + e3 : k == 1 ? e1 + e2 : k == 2 ? e1 - e2 : e0 - e3;
 }
 
-// Intra16x16 luma mode decision (8.3.3): key = SAD*4 + mode over the available modes; p0/p1 = this lane's 8 predicted samples
-struct I16Dec { int key, mode; uint32_t p0, p1; };
-__device__ __forceinline__ I16Dec i16_decide(const IntraNb& nb, const MbTile& t, int lane, bool has_top, bool has_left) {
+// Intra16x16 luma mode decision (8.3.3) without a neighbour above: horizontal (needs the left one) or DC, key = SAD*4 + mode;
+// p = the value of this lane's 8 predicted samples, 4 to a word (both modes repeat one value along a row)
+struct I16Dec { int key, mode; uint32_t p; };
+__device__ __forceinline__ I16Dec i16_decide(const IntraNb& nb, const MbTile& t, int lane, bool has_left) {
   const int r8 = lane >> 1, c8 = (lane & 1) * 8;
   const uint32_t cy0 = *reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8]);
   const uint32_t cy1 = *reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8 + 4]);
-  int sum_t = 0, sum_l = 0, H = 0, V = 0;
+  int sum_l = 0;
 #pragma unroll
-  for (int i = 0; i < 16; i++) { sum_t += nb.top_y[i]; sum_l += nb.left_y[i]; }
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    H += (i + 1) * ((int)nb.top_y[8 + i] - (i == 7 ? nb.tl_y : (int)nb.top_y[6 - i]));
-    V += (i + 1) * ((int)nb.left_y[8 + i] - (i == 7 ? nb.tl_y : (int)nb.left_y[6 - i]));
-  }
-  const int dc_y = has_top && has_left ? (sum_t + sum_l + 16) >> 5 : has_top ? (sum_t + 8) >> 4 : has_left ? (sum_l + 8) >> 4 : 128;
-  const int pa = 16 * ((int)nb.left_y[15] + (int)nb.top_y[15]), pb = (5 * H + 32) >> 6, pc = (5 * V + 32) >> 6;
-  uint32_t pv0 = *reinterpret_cast<const uint32_t*>(&nb.top_y[c8]), pv1 = *reinterpret_cast<const uint32_t*>(&nb.top_y[c8 + 4]);
-  uint32_t ph = rep4(nb.left_y[r8]), pd = rep4(dc_y), pp0 = 0, pp1 = 0;
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    pp0 |= (uint32_t)clip255((pa + pb * (c8 + j - 7) + pc * (r8 - 7) + 16) >> 5) << (8 * j);
-    pp1 |= (uint32_t)clip255((pa + pb * (c8 + 4 + j - 7) + pc * (r8 - 7) + 16) >> 5) << (8 * j);
-  }
+  for (int i = 0; i < 16; i++) sum_l += nb.left_y[i];
+  const uint32_t ph = rep4(nb.left_y[r8]), pd = rep4(has_left ? (sum_l + 8) >> 4 : 128);
   int best_key = 0x7fffffff, best_mode = 2, s;
-  if (has_top) { s = __reduce_add_sync(FULL, __vsadu4(cy0, pv0) + __vsadu4(cy1, pv1)); if (s * 4 + 0 < best_key) { best_key = s * 4 + 0; best_mode = 0; } }
   if (has_left) { s = __reduce_add_sync(FULL, __vsadu4(cy0, ph) + __vsadu4(cy1, ph)); if (s * 4 + 1 < best_key) { best_key = s * 4 + 1; best_mode = 1; } }
   s = __reduce_add_sync(FULL, __vsadu4(cy0, pd) + __vsadu4(cy1, pd)); if (s * 4 + 2 < best_key) { best_key = s * 4 + 2; best_mode = 2; }
-  if (has_top && has_left) { s = __reduce_add_sync(FULL, __vsadu4(cy0, pp0) + __vsadu4(cy1, pp1)); if (s * 4 + 3 < best_key) { best_key = s * 4 + 3; best_mode = 3; } }
   I16Dec d;
   d.key = best_key; d.mode = best_mode;
-  d.p0 = best_mode == 0 ? pv0 : best_mode == 1 ? ph : best_mode == 2 ? pd : pp0;
-  d.p1 = best_mode == 0 ? pv1 : best_mode == 1 ? ph : best_mode == 2 ? pd : pp1;
+  d.p = best_mode == 1 ? ph : pd;
   return d;
 }
 
@@ -130,12 +111,10 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
   __shared__ __align__(16) I4State i4;
   __shared__ I4Result r4;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const SliceGeo geo = slice_geo(f, f.seg_cols ? (int)blockIdx.x : (int)blockIdx.x / f.slice_rows);   // sub-row slices: one block per slice
-  const int mby = f.seg_cols ? geo.row0 : (int)blockIdx.x, mbx0 = f.seg_cols ? geo.x0 : 0, mbx1 = f.seg_cols ? geo.x1 : f.mbw;
+  const SliceGeo geo = slice_geo(f, blockIdx.x);        // columns [x0, x1) of row row0
+  const int mby = geo.row0;
   const int qp = frame_qp(f);
   const int lambda = me_lambda[qp];
-  const bool has_top = top_in_slice(f, mby);
-  const bool signal_progress = !f.seg_cols && f.slice_rows > 1 && mby + 1 < f.mbh && top_in_slice(f, mby + 1);
   const size_t ysz = (size_t)f.cw * f.ch;
   const uint8_t* cur_y = f.cur; const uint8_t* cur_uv = f.cur + ysz;
   uint8_t* rec_y = f.recon; uint8_t* rec_uv = f.recon + ysz;
@@ -154,37 +133,16 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
   const uint32_t cm = *reinterpret_cast<const uint32_t*>(&i4.code[lm][ly * 4]);   // V-indices of this lane's four predicted samples
   const uint32_t ch = *reinterpret_cast<const uint32_t*>(&i4.code[8][ly * 4]);    // ... for horizontal-up
 
-  for (int mbx = mbx0; mbx < mbx1; mbx++) {
+  for (int mbx = geo.x0; mbx < geo.x1; mbx++) {
     const int mb = mby * f.mbw + mbx;
-    const bool has_left = mbx > mbx0;
-    const bool has_tr = has_top && mbx + 1 < f.mbw;
-    if (has_top) {       // wavefront: the row above must have finished macroblock mbx+1 (above-right samples)
-      if (threadIdx.x == 0) { const int need = min(mbx + 2, f.mbw); while (*((volatile int*)&f.progress[mby - 1]) < need) { } __threadfence(); }
-      __syncthreads();
-    }
-    // ---- load current macroblock and neighbours (warp 0) ------------------------------------------
+    const bool has_left = mbx > geo.x0;
+    // ---- load current macroblock (warp 0) ------------------------------------------------------------
     if (warp == 0) {
       const uint2 v = *reinterpret_cast<const uint2*>(cur_y + (size_t)(mby * 16 + r8) * f.cw + mbx * 16 + c8);
       *reinterpret_cast<uint2*>(&t.cur_y[r8][c8]) = v;
       if (lane < 16) {
         const uint2 w = *reinterpret_cast<const uint2*>(cur_uv + (size_t)(mby * 8 + r8) * f.cw + mbx * 16 + c8);
         *reinterpret_cast<uint2*>(&t.cur_uv[r8][c8]) = w;
-      }
-      if (has_top) {
-        if (lane < 16) nb.top_y[lane] = __ldcg(rec_y + (size_t)(mby * 16 - 1) * f.cw + mbx * 16 + lane);
-        else nb.top_uv[lane - 16] = __ldcg(rec_uv + (size_t)(mby * 8 - 1) * f.cw + mbx * 16 + (lane - 16));
-        if (lane < 4) {
-          nb.top_y[16 + lane] = has_tr ? __ldcg(rec_y + (size_t)(mby * 16 - 1) * f.cw + mbx * 16 + 16 + lane) : (uint8_t)128;
-          // written by the block of the row above during this launch: read through L2, not the (incoherent) L1
-          const uint2 tm = __ldcg(reinterpret_cast<const uint2*>(&f.mbinfo[mb - f.mbw]));
-          const int ttype = tm.y & 255;
-          nb.top_modes[lane] = ttype == MB_I4 ? __ldcg(&f.i4modes[(size_t)(mb - f.mbw) * 16 + 12 + lane]) : (uint8_t)2;
-        }
-        if (has_left && lane == 0) {
-          nb.tl_y = __ldcg(rec_y + (size_t)(mby * 16 - 1) * f.cw + mbx * 16 - 1);
-          nb.tl_u = __ldcg(rec_uv + (size_t)(mby * 8 - 1) * f.cw + mbx * 16 - 2);
-          nb.tl_v = __ldcg(rec_uv + (size_t)(mby * 8 - 1) * f.cw + mbx * 16 - 1);
-        }
       }
     }
     __syncthreads();
@@ -196,57 +154,36 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
     // ================= warp 0: Intra16x16 luma + chroma ==================================================
     // chroma DC predictors (8.3.4.1-3), one (component, block) per lane 0..7
     if (lane < 8) {
-      const int c = lane >> 2, b = lane & 3, bx = (b & 1) * 4, by = (b >> 1) * 4;
-      int st = 0, sl = 0;
+      const int c = lane >> 2, by = ((lane & 3) >> 1) * 4;
+      int sl = 0;
 #pragma unroll
-      for (int i = 0; i < 4; i++) { st += nb.top_uv[(bx + i) * 2 + c]; sl += nb.left_uv[(by + i) * 2 + c]; }
-      int dc;
-      if (b == 0 || b == 3) dc = has_top && has_left ? (st + sl + 4) >> 3 : has_top ? (st + 2) >> 2 : has_left ? (sl + 2) >> 2 : 128;
-      else if (b == 1) dc = has_top ? (st + 2) >> 2 : has_left ? (sl + 2) >> 2 : 128;
-      else dc = has_left ? (sl + 2) >> 2 : has_top ? (st + 2) >> 2 : 128;
-      nb.cdc[lane] = dc;
+      for (int i = 0; i < 4; i++) sl += nb.left_uv[(by + i) * 2 + c];
+      nb.cdc[lane] = has_left ? (sl + 2) >> 2 : 128;
     }
     {
-      const I16Dec d = i16_decide(nb, t, lane, has_top, has_left);
+      const I16Dec d = i16_decide(nb, t, lane, has_left);
       best_mode = d.mode;
-      *reinterpret_cast<uint32_t*>(&t.pred_y[r8][c8]) = d.p0;
-      *reinterpret_cast<uint32_t*>(&t.pred_y[r8][c8 + 4]) = d.p1;
+      *reinterpret_cast<uint32_t*>(&t.pred_y[r8][c8]) = d.p;
+      *reinterpret_cast<uint32_t*>(&t.pred_y[r8][c8 + 4]) = d.p;
     }
     __syncwarp();   // nb.cdc visible
-    // ---- chroma mode decision: key = (SAD Cb + SAD Cr)*4 + mode ------------------------------------
+    // ---- chroma mode decision: DC or (with a left neighbour) horizontal, key = (SAD Cb + SAD Cr)*4 + mode -----
     const uint32_t cc = *reinterpret_cast<const uint32_t*>(&t.cur_uv[rc4][cc4]);   // Cb0 Cr0 Cb1 Cr1 at x = (lane&3)*2, +1
-    const int x0 = (lane & 3) * 2;
-    uint32_t qd, qh, qv, qp_ = 0;
+    uint32_t qd, qh;
     {
-      const int blk = (rc4 >> 2) * 2 + (x0 >> 2);
+      const int blk = (rc4 >> 2) * 2 + ((lane & 3) >> 1);
       qd = (uint32_t)nb.cdc[blk] | ((uint32_t)nb.cdc[4 + blk] << 8);
       qd |= qd << 16;
       qh = (uint32_t)nb.left_uv[rc4 * 2] | ((uint32_t)nb.left_uv[rc4 * 2 + 1] << 8);
       qh |= qh << 16;
-      qv = *reinterpret_cast<const uint32_t*>(&nb.top_uv[cc4]);
-      int Hc[2] = {0, 0}, Vc[2] = {0, 0};
-#pragma unroll
-      for (int c = 0; c < 2; c++) {
-        const int tlc = c ? nb.tl_v : nb.tl_u;
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          Hc[c] += (i + 1) * ((int)nb.top_uv[(4 + i) * 2 + c] - (i == 3 ? tlc : (int)nb.top_uv[(2 - i) * 2 + c]));
-          Vc[c] += (i + 1) * ((int)nb.left_uv[(4 + i) * 2 + c] - (i == 3 ? tlc : (int)nb.left_uv[(2 - i) * 2 + c]));
-        }
-        const int a = 16 * ((int)nb.left_uv[14 + c] + (int)nb.top_uv[14 + c]), b = (34 * Hc[c] + 32) >> 6, cq = (34 * Vc[c] + 32) >> 6;
-        qp_ |= (uint32_t)clip255((a + b * (x0 - 3) + cq * (rc4 - 3) + 16) >> 5) << (8 * c);
-        qp_ |= (uint32_t)clip255((a + b * (x0 + 1 - 3) + cq * (rc4 - 3) + 16) >> 5) << (16 + 8 * c);
-      }
     }
     int cbest_key = 0x7fffffff;
     cbest = 0;
     {
       int s = __reduce_add_sync(FULL, __vsadu4(cc, qd)); if (s * 4 + 0 < cbest_key) { cbest_key = s * 4 + 0; cbest = 0; }
       if (has_left) { s = __reduce_add_sync(FULL, __vsadu4(cc, qh)); if (s * 4 + 1 < cbest_key) { cbest_key = s * 4 + 1; cbest = 1; } }
-      if (has_top) { s = __reduce_add_sync(FULL, __vsadu4(cc, qv)); if (s * 4 + 2 < cbest_key) { cbest_key = s * 4 + 2; cbest = 2; } }
-      if (has_top && has_left) { s = __reduce_add_sync(FULL, __vsadu4(cc, qp_)); if (s * 4 + 3 < cbest_key) { cbest_key = s * 4 + 3; cbest = 3; } }
     }
-    *reinterpret_cast<uint32_t*>(&t.pred_uv[rc4][cc4]) = cbest == 0 ? qd : cbest == 1 ? qh : cbest == 2 ? qv : qp_;
+    *reinterpret_cast<uint32_t*>(&t.pred_uv[rc4][cc4]) = cbest == 0 ? qd : qh;
     __syncwarp();
 
     // ---- Intra16x16 coding (also codes the chroma, which is identical either way) --------------------------
@@ -264,19 +201,15 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
     // T = bx + 2*by at most two blocks are ready, so the pair of warps finishes the macroblock in 10 steps instead of 16.
     const int u = warp - 1;
     uint8_t* const V = i4.v[u];
-    const int best_key = i16_decide(nb, t, lane, has_top, has_left).key;      // same decision as warp 0 (reads only)
+    const int best_key = i16_decide(nb, t, lane, has_left).key;      // same decision as warp 0 (reads only)
     // ---- Intra4x4 candidate: 16 blocks in decoding order ----------------------------------------------
-    // rt = reconstruction with a one-sample frame: rt[y+1][x+1] is macroblock sample (x,y), row 0 / column 0 hold the
-    // neighbours above (16 + 4 above-right) and to the left, rt[0][0] the above-left sample.
+    // rt = reconstruction with a one-sample frame: rt[y+1][x+1] is macroblock sample (x,y), column 0 holds the neighbours to the
+    // left.  Row 0 stands for the samples above the macroblock, which are not available: no mode that reads them is selected.
     const bool try_i4 = (best_key >> 2) > I4_SKIP_SAD_PER_LAMBDA * lambda;      // nearly flat macroblocks go straight to Intra16x16
     int mode_bits4 = 0, cbp4 = 0, bits4_cavlc = 0;
     long long d4 = 0;
     if (try_i4) {
-      if (u == 0) {
-        if (lane < 20) i4.rt[0][1 + lane] = nb.top_y[lane];
-        if (lane < 16) i4.rt[1 + lane][0] = nb.left_y[lane];
-        if (lane == 31) i4.rt[0][0] = (uint8_t)nb.tl_y;
-      }
+      if (u == 0 && lane < 16) i4.rt[1 + lane][0] = nb.left_y[lane];
       i4_pair_barrier();
       for (int T = 0; T < 10; T++) {
         // raster position of this warp's block at step T (nibble-packed): warp u=0 takes row 0 and columns 2,3; u=1 columns 0,1 of rows 1..3
@@ -284,10 +217,8 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
         if (rp >= 0) {
         const int bx = rp & 3, by = rp >> 2;
         const int blk = (by >> 1) * 8 + (bx >> 1) * 4 + (by & 1) * 2 + (bx & 1);          // blkIdx in decoding order
-        const bool has_a = bx > 0 || has_left, has_b = by > 0 || has_top;
-        const bool has_d = (bx > 0 && by > 0) ? true : bx > 0 ? has_top : by > 0 ? has_left : (has_left && has_top);
-        const int trc = (int)((0x111511eau >> (2 * (by * 4 + bx))) & 3u);      // 2-bit codes of i4_tr_inside, raster order
-        const bool has_c = trc == 1 ? true : trc == 2 ? has_top : trc == 3 ? has_tr : false;
+        const bool has_a = bx > 0 || has_left, has_b = by > 0, has_d = by > 0 && (bx > 0 || has_left);
+        const bool has_c = (0x5750u >> rp) & 1u;       // above-right samples inside the macroblock
         if (lane < 15) {        // X[lane]: neighbouring samples of this block (values of unavailable ones are never selected)
           int row = by * 4, col = bx * 4;
           if (lane < 5) row += (lane == 0 ? 3 : 4 - lane) + 1;
@@ -302,12 +233,11 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
           V[48] = (uint8_t)(has_a && has_b ? (st + sl + 4) >> 3 : has_b ? (st + 2) >> 2 : has_a ? (sl + 2) >> 2 : 128);
         }
         __syncwarp();
-        // predicted mode (8.3.1.1)
-        int pm;
-        {
+        // predicted mode (8.3.1.1): 2 when the block to the left or above is not available, which is always so in the top row
+        int pm = 2;
+        if (by > 0) {
           const int ma = bx > 0 ? (int)i4.modes[by * 4 + bx - 1] : has_left ? (int)nb.left_modes[by] : -1;
-          const int mb_ = by > 0 ? (int)i4.modes[(by - 1) * 4 + bx] : has_top ? (int)nb.top_modes[bx] : -1;
-          pm = (ma < 0 || mb_ < 0) ? 2 : min(ma, mb_);
+          if (ma >= 0) pm = min(ma, (int)i4.modes[(by - 1) * 4 + bx]);
         }
         // modes 0..7: lane = mode*4 + row; mode 8: every group of four lanes evaluates it as well
         const uint32_t crow = *reinterpret_cast<const uint32_t*>(&t.cur_y[by * 4 + ly][bx * 4]);
@@ -404,19 +334,12 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
       }
     }
     }
-    if (signal_progress) {
-      __threadfence();
-      __syncthreads();
-      if (threadIdx.x == 0) *((volatile int*)&f.progress[mby]) = mbx + 1;
-    } else {
-      __syncthreads();
-    }
+    __syncthreads();
   }
 }
 
 int launch_intra(const FrameCtx& f, cudaStream_t st) {
-  cudaMemsetAsync(f.progress, 0, sizeof(int) * f.mbh, st);
-  k_intra_rows<<<f.seg_cols ? f.n_slices : f.mbh, 96, 0, st>>>(f);
+  k_intra_rows<<<f.n_slices, 96, 0, st>>>(f);
   return 1;
 }
 

@@ -3,7 +3,7 @@
 #include <cuda_runtime.h>
 namespace b2v {
 struct FrameCtx;
-int launch_intra(const FrameCtx& f, cudaStream_t st);    // IDR: Intra16x16 rows (h264_intra.cu)
+int launch_intra(const FrameCtx& f, cudaStream_t st);    // IDR: one block per slice (h264_intra.cu)
 int launch_inter(const FrameCtx& f, cudaStream_t st);    // P: motion search + residual (h264_inter.cu)
 int launch_cavlc(const FrameCtx& f, cudaStream_t st);    // per-macroblock CAVLC bit strings (h264_entropy.cu)
 int launch_slice_build(const FrameCtx& f, cudaStream_t st);     // k_slice_build: scan + copy + emulation-prevention count; its last block runs the rate-control step (h264_entropy.cu)

@@ -197,6 +197,9 @@ def test_c_abi_argument_errors_without_a_gpu():
     assert b"unsupported" in lib.b2v_last_error()
     s.src_w, s.src_h = 8192, 4320                                    # beyond 7680x4320 (selkies.py:281)
     assert lib.b2v_create(C.byref(s), N.FRAME_CB(lambda f, u: None), None, C.byref(h)) == N.B2V_EINVAL
+    s.src_w, s.src_h, s.idr_slice_mbs = 1920, 1080, -1               # negative IDR slice length
+    assert lib.b2v_create(C.byref(s), N.FRAME_CB(lambda f, u: None), None, C.byref(h)) == N.B2V_EINVAL
+    assert b"idr_slice_mbs" in lib.b2v_last_error()
     assert lib.b2v_create(None, N.FRAME_CB(lambda f, u: None), None, C.byref(h)) == N.B2V_EINVAL
     for fn, args in ((lib.b2v_flush, (None,)), (lib.b2v_request_idr, (None,)), (lib.b2v_set_framerate, (None, 30.0)),
                      (lib.b2v_set_bitrate_kbps, (None, 1000)), (lib.b2v_get_stats, (None, None))):

@@ -65,6 +65,17 @@ def test_default_slicing_decodes_and_saves_bits():
     run(1280, 720, [synth.desktop(1280, 720, t) for t in range(3)], 33, 0)   # 45 rows, IDR in two segments per row
 
 
+def test_negative_idr_slice_mbs_is_rejected():
+    """IDR slices never span rows: a negative idr_slice_mbs raises and leaves the slicing as it was."""
+    w, h = 320, 192
+    f = synth.desktop(w, h, 0)
+    enc, ref = oracle.RefEncoder(w, h), oracle.RefEncoder(w, h)
+    enc.set_idr_slice_mbs(7); ref.set_idr_slice_mbs(7)
+    with pytest.raises(ValueError):
+        enc.set_idr_slice_mbs(-1)
+    assert enc.encode_bgra(f, True, qp=28) == ref.encode_bgra(f, True, qp=28)
+
+
 def test_cropped_sizes():
     run(130, 70, [synth.gradient(130, 70, t) for t in range(3)], 24)     # coded 144x80, crop both ways
     run(16, 16, [synth.noise(16, 16, 4), synth.noise(16, 16, 5)], 20)     # one macroblock
