@@ -7,7 +7,7 @@
 //
 // Per-frame flow (four streams, events in between; nothing on the host blocks except ring back-pressure):
 //   st_copy : cudaMemcpyAsync  pinned slot -> device BGRA slot                      (a) ingest
-//   st_enc  : fused CSC(+scale) -> NV12 cur ; analysis (k_intra_rows / k_inter_mb), or the whole JPEG encode   (b),(c)
+//   st_enc  : fused CSC(+scale) -> NV12 cur ; analysis (k_intra_rows / k_inter_lean + k_inter_search), or the whole JPEG encode   (b),(c)
 //   st_pack : entropy coding of the same picture (k_cavlc_mb -> k_slice_build, which runs the rate-control step -> k_pack_au)
 //             -> AU in HBM, overlapping the analysis of the next picture on st_enc (h264_encoder.cu)
 //   st_out  : cudaMemcpyAsync  AU head (size + first chunk) -> pinned output slot

@@ -67,7 +67,8 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   MbInfo* mbinfo;          // this picture's records (double-buffered: the entropy kernels of picture k read them while picture k+1 is analysed)
   const MbInfo* mbinfo_prev;   // the previous picture's records (temporal motion predictor)
   unsigned long long* me_pub;  // [mbs] anchor macroblocks publish (pic+1) << 32 | new-content flag << 16 | (mvx & 0xff) << 8 | mvy & 0xff as soon as motion estimation is done
-  int n_anchor;                // anchors of a P picture (one per 4x4 group of macroblocks, groups counted inside each band)
+  int* me_queue;               // [2 + 2 * mbs] macroblocks k_inter_lean left to k_inter_search: anchor count, rest count, anchors [mbs], rest [mbs]
+  int search_blocks;           // k_inter_search grid: its resident capacity on this device
   uint8_t* i4modes;        // [mbs][16] Intra4x4PredMode per block (raster), valid for MB_I4
   int16_t* coef;           // [mbs][27][16]
   uint8_t* nnz;            // [mbs][32]: 0..15 luma raster, 16..19 Cb, 20..23 Cr

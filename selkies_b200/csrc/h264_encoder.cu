@@ -1,6 +1,6 @@
 // h264_encoder.cu — host side of the H.264 Constrained-Baseline encoder: parameter sets (7.3.2.1/2),
 // HBM buffers, per-picture sequencing (frame_num, idr_pic_id, reference swap) and the kernel pipeline
-//   [k_intra_rows | k_inter_mb] -> k_cavlc_mb -> k_slice_build -> k_pack_au
+//   [k_intra_rows | k_inter_lean -> k_inter_search x2] -> k_cavlc_mb -> k_slice_build -> k_pack_au
 // The output format is what the reference's consumers require (SURVEY.md §8 a13): Annex-B, CAVLC,
 // no B-frames, 4:2:0, in-band SPS/PPS on every IDR (src/selkies/rtc.py:394-401,
 // src/selkies/webrtc/codecs/h264.py:281-321).
@@ -40,6 +40,8 @@ struct Encoder {
   uint8_t* nnz[2] = {nullptr, nullptr};
   void *chunk_agg = nullptr, *chunk_inc = nullptr; int* slice_done = nullptr;   // k_slice_build look-back records (h264_entropy.cu)
   unsigned long long* me_pub = nullptr;   // anchor macroblocks' vectors of the picture being analysed (h264_inter.cu)
+  int* me_queue = nullptr;                // macroblocks left to the search passes (h264_inter.cu)
+  int search_blocks = 0;
   uint32_t *mb_words = nullptr, *mb_nbits = nullptr, *slice_buf = nullptr, *slice_size = nullptr, *slice_rbsp = nullptr;
   long long* slice_bits = nullptr;
   int* overflow = nullptr;
@@ -183,6 +185,8 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   }
   ECK(cudaMalloc((void**)&e->me_pub, mbs * sizeof(unsigned long long)));
   ECK(cudaMemset(e->me_pub, 0, mbs * sizeof(unsigned long long)));
+  ECK(cudaMalloc((void**)&e->me_queue, (2 + 2 * mbs) * sizeof(int)));
+  ECK(inter_search_grid(&e->search_blocks));
   ECK(cudaMalloc((void**)&e->mb_words, mbs * MB_WORDS * sizeof(uint32_t)));
   ECK(cudaMalloc((void**)&e->mb_nbits, mbs * sizeof(uint32_t)));
   // slice buffers serve either grid
@@ -238,7 +242,7 @@ void encoder_destroy(Encoder* e) {
   if (!e) return;
   void* ptrs[] = {e->recon[0], e->recon[1], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
-                  e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->chunk_agg, e->chunk_inc, e->slice_done};
+                  e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -265,12 +269,8 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.frame_num = e->frame_num; f.idr_pic_id = e->idr_count; f.pic = (int)(e->pic & 0x7fffffff);
   f.cur = p->cur; f.ref = e->recon[e->cur ^ 1]; f.recon = e->recon[e->cur];
   f.mbinfo = e->mbinfo[par]; f.mbinfo_prev = e->mbinfo[par ^ 1]; f.i4modes = e->i4modes[par]; f.coef = e->coef[par]; f.nnz = e->nnz[par];
-  f.me_pub = e->me_pub;
+  f.me_pub = e->me_pub; f.me_queue = e->me_queue; f.search_blocks = e->search_blocks;
   f.chunk_agg = (ChunkAgg*)e->chunk_agg; f.chunk_inc = (ChunkInc*)e->chunk_inc; f.slice_done = e->slice_done;
-  {   // anchors: ceil(mbw/4) columns x (groups of 4 rows inside every band)
-    const int rows_last = e->mbh - (e->n_bands - 1) * e->band_rows;
-    f.n_anchor = ((e->mbw + 3) / 4) * ((e->n_bands - 1) * ((e->band_rows + 3) / 4) + (rows_last + 3) / 4);
-  }
   f.mb_words = e->mb_words; f.mb_nbits = e->mb_nbits;
   f.slice_buf = e->slice_buf; f.slice_size = e->slice_size; f.slice_rbsp = e->slice_rbsp;
   f.slice_bits = e->slice_bits; f.paint_trigger = p->paint_trigger; f.paint_qp = p->paint_qp; f.paint_burst = p->paint_burst; f.rc = e->rc;
