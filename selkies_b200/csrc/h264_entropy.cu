@@ -9,10 +9,9 @@
 //   k_slice_build one block per chunk of up to 256 macroblocks of a slice: local scans + a decoupled look-back over the chunks of
 //                 the slice give every macroblock its bit offset and its mb_skip_run; 8 threads per macroblock shift the bit
 //                 strings into the slice RBSP (atomicOr); the chunk that finishes last counts the slice's emulation-prevention
-//                 bytes; the last block of the picture runs the rate-control step
-//   k_pack_au     one block per slice: prefix over slice sizes, emulation prevention (parallel rule: a 03 is
-//                 inserted before byte i iff byte<=3 and the run of zero bytes before it is even and >=2),
-//                 start codes + NAL headers, AuHeader, band table.
+//                 bytes (count_escapes); the last block of the picture runs the rate-control step
+//   k_pack_au     one block per slice: offset of the slice (segment_offset), the RBSP copied with emulation prevention
+//                 (copy_escaped; the rule is H264Escape in bitstream.cuh), start codes + NAL headers, AuHeader, band table.
 // CPU restatement: oracle/h264_ref.c cavlc_block(), code_slice(), nal_write(), rc_update().
 #include "h264_common.cuh"
 #include "h264_cavlc.cuh"
@@ -72,6 +71,20 @@ __device__ __forceinline__ void mb_header_i4(S& h, const FrameCtx& f, const MbIn
   put_ue(h, mi.chroma_mode);
   put_ue(h, cbp_to_codenum_intra[mi.cbp]);
   if (mi.cbp) put_se(h, 0);
+}
+
+// macroblock header of a coded (not I_PCM) macroblock: I_NxN above; I_16x16 (mb_type with prediction mode and cbp, intra_chroma_pred_mode,
+// mb_qp_delta); P_L0_16x16 (mb_type, mvd_l0, coded_block_pattern (inter me(v) mapping), mb_qp_delta)
+template <class S>
+__device__ __forceinline__ void mb_header(S& h, const FrameCtx& f, const MbInfo& mi, int mb, int mbx, int mby, int mvdx, int mvdy) {
+  if (mi.type == MB_I4) mb_header_i4(h, f, mi, mb, mbx, mby);
+  else if (mi.type == MB_I16) {
+    const int tcode = 1 + mi.i16_mode + 4 * (mi.cbp >> 4) + ((mi.cbp & 15) ? 12 : 0);
+    put_ue(h, (uint32_t)(f.idr ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
+  } else {
+    put_ue(h, 0); put_se(h, mvdx); put_se(h, mvdy); put_ue(h, cbp_to_codenum_inter[mi.cbp]);
+    if (mi.cbp) put_se(h, 0);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ k_cavlc_mb
@@ -155,19 +168,9 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   // ---- pass 1: sizes ---------------------------------------------------------------------------------
   CountSink cs;
   if (coded) cavlc_block(cs, lv, maxc, nC);
-  int hdr_bits;
-  {
-    CountSink h;
-    if (mi.type == MB_I4) mb_header_i4(h, f, mi, mb, mbx, mby);
-    else if (mi.type == MB_I16) {
-      const int tcode = 1 + mi.i16_mode + 4 * cbp_c + (cbp_l ? 12 : 0);
-      put_ue(h, (uint32_t)(f.idr ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
-    } else {
-      put_ue(h, 0); put_se(h, mvdx); put_se(h, mvdy); put_ue(h, cbp_to_codenum_inter[mi.cbp]);
-      if (mi.cbp) put_se(h, 0);
-    }
-    hdr_bits = h.n;
-  }
+  CountSink hs;
+  mb_header(hs, f, mi, mb, mbx, mby, mvdx, mvdy);
+  const int hdr_bits = hs.n;
   int incl = cs.n;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) { const int o = __shfl_up_sync(FULL, incl, d); if (lane >= d) incl += o; }
@@ -175,18 +178,8 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   const int my_off = hdr_bits + incl - cs.n;
 
   // ---- pass 2: write -----------------------------------------------------------------------------------
-  if (lane == 0) {
-    SmemSink h{words, 0, MB_WORDS * 32};
-    if (mi.type == MB_I4) mb_header_i4(h, f, mi, mb, mbx, mby);
-    else if (mi.type == MB_I16) {
-      const int tcode = 1 + mi.i16_mode + 4 * cbp_c + (cbp_l ? 12 : 0);
-      put_ue(h, (uint32_t)(f.idr ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
-    } else {
-      put_ue(h, 0); put_se(h, mvdx); put_se(h, mvdy); put_ue(h, cbp_to_codenum_inter[mi.cbp]);
-      if (mi.cbp) put_se(h, 0);
-    }
-  }
-  if (coded) { SmemSink ws{words, my_off, MB_WORDS * 32}; cavlc_block(ws, lv, maxc, nC); }
+  if (lane == 0) { BitWriter h{words, 0, MB_WORDS * 32}; mb_header(h, f, mi, mb, mbx, mby, mvdx, mvdy); }
+  if (coded) { BitWriter ws{words, my_off, MB_WORDS * 32}; cavlc_block(ws, lv, maxc, nC); }
   __syncwarp();
   int nb = total_bits;
   if (nb > MB_WORDS * 32) { nb = MB_WORDS * 32; if (lane == 0) atomicExch(f.overflow, 1); }
@@ -209,20 +202,7 @@ __device__ __forceinline__ void slice_header(S& s, const FrameCtx& f, int first_
   put_ue(s, 1);
 }
 
-struct GlobalSink {         // same layout as SmemSink, on the slice's RBSP words in HBM
-  uint32_t* w; long long pos;
-  __device__ __forceinline__ void put(int len, uint32_t v) {
-    if (len == 0) return;
-    const long long wi = pos >> 5; const int o = (int)(pos & 31), space = 32 - o;
-    if (len <= space) atomicOr(&w[wi], v << (space - len));
-    else { atomicOr(&w[wi], v >> (len - space)); atomicOr(&w[wi + 1], v << (32 - (len - space))); }
-    pos += len;
-  }
-};
-
-constexpr int SLICE_THREADS = 256;
-
-__device__ __forceinline__ uint32_t rbsp_byte(const uint32_t* w, long long i) { return (__ldcg(&w[i >> 2]) >> (24 - 8 * (int)(i & 3))) & 255u; }
+constexpr int SLICE_THREADS = ESC_THREADS;
 
 __device__ __forceinline__ void or_word(uint32_t* out, long long bitpos, uint32_t v) {
   if (!v) return;
@@ -287,10 +267,6 @@ __device__ __forceinline__ void rc_step(const FrameCtx& f, int qp_used, long lon
   rc->fb[f.pic & 1] = n;
 }
 
-// Defined after k_slice_build, its only caller: the compiler then lays s_red out behind the kernel's own shared variables.
-// Defining it above the kernel changes that layout and the kernel's generated code.
-__device__ __forceinline__ void slice_ep_body(const FrameCtx& f, int s);
-
 // ---- k_slice_build (chunked): one block per CHUNK of up to 256 consecutive macroblocks of a slice, so a slice of many rows is built
 // by many blocks instead of one long loop.  What a chunk needs from the chunks in front of it is (a) the bit position where it starts
 // and (b) the mb_skip_run still open at that point — the first coded macroblock of a chunk codes ue(open run + its own leading skips),
@@ -301,7 +277,8 @@ __device__ __forceinline__ void slice_ep_body(const FrameCtx& f, int s);
 // state.  A chunk that holds an I_PCM macroblock (byte alignment: its length depends on its position) publishes no usable aggregate;
 // its successors wait for its inclusive state instead.  Then every chunk shifts its macroblocks' bit strings into the slice RBSP
 // (8 threads per macroblock, offsets from shared memory), the chunk that holds the slice's last macroblock appends the trailing
-// skip run + rbsp_trailing_bits, and the last chunk of a slice to FINISH counts the slice's emulation-prevention bytes.
+// skip run + rbsp_trailing_bits, and the last chunk of a slice to FINISH counts the slice's emulation-prevention bytes (it reads
+// words other blocks wrote: count_escapes reads through L2).
 struct ChunkAgg { int flag; int has; int first_run; int trailing; long long rest_bits; };   // has: bit 0 coded macroblock present, bit 1 I_PCM inside (no aggregate)
 struct ChunkInc { int flag; int trailing; long long bits; };
 constexpr int CHUNK_MAX_POLLS = 1 << 22;
@@ -451,11 +428,11 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       __threadfence();
       *reinterpret_cast<volatile int*>(&c->flag) = tag;
       if (k == 0) {                              // slice header (the bits it occupies were counted above)
-        GlobalSink g{out, 0};
+        BitWriter g{out, 0};
         slice_header(g, f, first_mb, qp, fn);
       }
       if (last_chunk) {                          // trailing mb_skip_run, rbsp_trailing_bits
-        GlobalSink g{out, s_bits_out};
+        BitWriter g{out, s_bits_out};
         const int runt = s_trail_out;
         if (!f.idr && runt > 0) put_ue(g, (uint32_t)runt);
         f.slice_bits[s] = g.pos;
@@ -503,7 +480,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       long long pos = s_off[i];
       if (!f.idr) {
         const uint32_t run = (uint32_t)s_run[i];
-        if (sub == 0) { GlobalSink g{out, pos}; put_ue(g, run); }
+        if (sub == 0) { BitWriter g{out, pos}; put_ue(g, run); }
         pos += ue_len(run);
       }
       const uint32_t* src = f.mb_words + (size_t)mb * MB_WORDS;
@@ -534,73 +511,32 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
     s_flag = lastf;
   }
   __syncthreads();
-  if (s_flag) { __threadfence(); slice_ep_body(f, s); }
-}
-
-// ---- emulation-prevention bytes one slice needs (7.4.1), counted by one block: a 03 goes in front of byte i iff byte <= 3
-// and the run of zero bytes before it is even and >= 2.
-__device__ __forceinline__ void slice_ep_body(const FrameCtx& f, int s) {
-  __shared__ int s_red[SLICE_THREADS / 32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t* out = f.slice_buf + (size_t)s * f.slice_words;
-  const long long rbsp_bytes = __ldcg(&f.slice_rbsp[s]);
-  int ep = 0;
-  for (long long w0 = (long long)tid * 4; w0 < rbsp_bytes; w0 += SLICE_THREADS * 4) {
-    const uint32_t word = __ldcg(&out[w0 >> 2]);
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      const long long i = w0 + k;
-      const uint32_t b = (word >> (24 - 8 * k)) & 255u;
-      if (i < rbsp_bytes && b <= 3u) {
-        int z = 0;
-        while (i - 1 - z >= 0 && rbsp_byte(out, i - 1 - z) == 0u) z++;
-        if (z >= 2 && (z & 1) == 0) ep++;
-      }
+  if (s_flag) {
+    __threadfence();
+    const long long rbsp_bytes = __ldcg(&f.slice_rbsp[s]);
+    const int ep = count_escapes<H264Escape>(out, rbsp_bytes, s_warp_max);
+    if (tid == 0) {
+      const SliceGeo g = slice_geo(f, s);
+      const int start_len = (g.row0 % f.band_rows == 0 && g.x0 == 0 && !f.idr) ? 4 : 3;     // 4-byte start code on the first NAL of (each band's) access unit
+      f.slice_size[s] = (uint32_t)(start_len + 1 + rbsp_bytes + ep);
     }
-  }
-  ep = __reduce_add_sync(FULL, ep);
-  if (lane == 0) s_red[warp] = ep;
-  __syncthreads();
-  if (tid == 0) {
-    int t = 0;
-    for (int w = 0; w < SLICE_THREADS / 32; w++) t += s_red[w];
-    const SliceGeo geo = slice_geo(f, s);
-    const int start_len = (geo.row0 % f.band_rows == 0 && geo.x0 == 0 && !f.idr) ? 4 : 3;     // 4-byte start code on the first NAL of (each band's) access unit
-    f.slice_size[s] = (uint32_t)(start_len + 1 + rbsp_bytes + t);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ k_pack_au
-constexpr int PACK_THREADS = 256;
-constexpr int PACK_CH = 16;      // bytes per thread per round
+constexpr int PACK_THREADS = ESC_THREADS;
 
 __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long au_cap) {
-  __shared__ long long s_base;
   __shared__ int s_wsum[PACK_THREADS / 32];
-  __shared__ int s_carry;
-  const int s = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // byte offset of this slice's NAL inside the access unit
-  long long part = 0;
-  for (int j = tid; j < s; j += PACK_THREADS) part += f.slice_size[j];
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) part += __shfl_xor_sync(FULL, part, d);
-  __shared__ long long s_part[PACK_THREADS / 32];
-  if (lane == 0) s_part[warp] = part;
-  __syncthreads();
+  const int s = blockIdx.x, tid = threadIdx.x;
   const SliceGeo geo = slice_geo(f, s);
   const int row0 = geo.row0, band = row0 / f.band_rows;
   const bool band_first = row0 == band * f.band_rows && geo.x0 == 0;      // this slice opens its band's access unit
   const int plen = (f.striped && band == f.n_bands - 1) ? f.param_len_last : f.param_len;
-  if (tid == 0) {
-    long long t = f.idr ? (long long)band * f.param_len + plen : 0;       // parameter sets of bands 0..band precede this NAL
-    for (int w = 0; w < PACK_THREADS / 32; w++) t += s_part[w];
-    s_base = t; s_carry = 0;
-  }
-  __syncthreads();
+  // byte offset of this slice's NAL inside the access unit: the parameter sets of bands 0..band and the slices in front of it
+  const long long base = (f.idr ? (long long)band * f.param_len + plen : 0) + segment_offset(f.slice_size, s);
   uint8_t* au = f.au + f.au_data_off;
   const long long cap = au_cap - (long long)f.au_data_off;
-  const long long base = s_base;
-  const uint32_t* in = f.slice_buf + (size_t)s * f.slice_words;
   const long long n = f.slice_rbsp[s];
   const int start_len = (band_first && !f.idr) ? 4 : 3;
   if (tid == 0 && base + start_len + 1 <= cap) {
@@ -609,51 +545,7 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
     au[o++] = 0; au[o++] = 0; au[o++] = 1;
     au[o++] = (uint8_t)(((f.idr ? 3 : 2) << 5) | (f.idr ? 5 : 1));
   }
-  const long long out0 = base + start_len + 1;
-  for (long long cb = 0; cb < n; cb += (long long)PACK_THREADS * PACK_CH) {
-    const long long i0 = cb + (long long)tid * PACK_CH;
-    uint32_t bytes[PACK_CH]; uint32_t epmask = 0; int cnt = 0;
-    if (i0 < n) {
-      int z = 0;                                   // zero run in front of the chunk
-      while (i0 - 1 - z >= 0 && rbsp_byte(in, i0 - 1 - z) == 0u) z++;
-#pragma unroll
-      for (int k = 0; k < PACK_CH; k++) {
-        const long long i = i0 + k;
-        const uint32_t b = i < n ? rbsp_byte(in, i) : 0xffu;
-        bytes[k] = b;
-        if (i < n && b <= 3u && z >= 2 && (z & 1) == 0) { epmask |= 1u << k; cnt++; }
-        z = b == 0u ? z + 1 : 0;
-      }
-    }
-    int incl = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const int o = __shfl_up_sync(FULL, incl, d); if (lane >= d) incl += o; }
-    if (lane == 31) s_wsum[warp] = incl;
-    __syncthreads();
-    int before = s_carry;
-    for (int w = 0; w < warp; w++) before += s_wsum[w];
-    before += incl - cnt;
-    if (i0 < n) {
-      long long o = out0 + i0 + before;
-#pragma unroll
-      for (int k = 0; k < PACK_CH; k++) {
-        if (i0 + k < n) {
-          if ((epmask >> k) & 1u) { if (o < cap) au[o] = 3; o++; }
-          if (o < cap) au[o] = (uint8_t)bytes[k];
-          o++;
-        }
-      }
-    }
-    __syncthreads();
-    if (tid == 0) { int t = s_carry; for (int w = 0; w < PACK_THREADS / 32; w++) t += s_wsum[w]; s_carry = t; }
-    __syncthreads();
-  }
-  // self-clean the slice scratch for the next picture (k_slice_build builds the RBSP with atomicOr)
-  {
-    uint32_t* w = f.slice_buf + (size_t)s * f.slice_words;
-    const long long nw = min((long long)f.slice_words, (n >> 2) + 2);
-    for (long long i = tid; i < nw; i += PACK_THREADS) w[i] = 0;
-  }
+  copy_escaped<H264Escape>(f.slice_buf + (size_t)s * f.slice_words, n, f.slice_words, au, base + start_len + 1, cap, s_wsum);
   if (band_first) {
     if (f.idr && base <= cap) {
       const uint8_t* ps = f.param_sets + ((f.striped && band == f.n_bands - 1) ? f.param_len : 0);

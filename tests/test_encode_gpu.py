@@ -33,6 +33,15 @@ def test_p_frames_bit_exact(w, h, slice_rows):
     assert [x.is_key for x in xs] == [True, False, False, False, False]
 
 
+def test_escape_boundaries_bit_exact():
+    """Emulation-prevention bytes where the byte-stream copy splits its work: zero runs that start in the previous thread's
+    16-byte chunk, and escapes in the second 4096-byte round of a slice (test_escape_cases_oracle.py checks that this
+    content reaches both)."""
+    w, h = 1280, 720
+    xs = encode(w, h, [synth.desktop(w, h, t) for t in range(3)], qp=10)
+    assert [x.is_key for x in xs] == [True, False, False]
+
+
 def test_motion_and_noise_bit_exact():
     base = synth.noise(256, 128, 9)
     encode(256, 128, [np.roll(base, (3 * t, -5 * t), axis=(0, 1)) for t in range(4)], qp=26, slice_rows=1)
