@@ -122,7 +122,7 @@ typedef struct {
   int stripe_fn[MAX_STRIPES];
   int32_t stripe_tab[MAX_STRIPES][3];   /* last picture: byte offset, size, coded flag */
   uint8_t sps_band[2][64]; int sps_band_len[2];   /* [0] regular band, [1] last band (may be shorter / cropped) */
-  int no_i4, no_tpred, no_refine_cap, no_anchor, no_newcontent, no_zcand;    /* A/B switches for experiments (environment B2V_REF_NO_I4 / B2V_REF_NO_TPRED / B2V_REF_NO_REFINE_CAP, read once at create) */
+  int no_anchor, no_newcontent, no_zcand;    /* A/B switches for experiments (environment B2V_REF_NO_ANCHOR / B2V_REF_NO_NEWCONTENT / B2V_REF_NO_ZCAND, read once at create) */
 } enc_t;
 
 static int clip3(int lo, int hi, int v) { return v < lo ? lo : (v > hi ? hi : v); }
@@ -611,7 +611,7 @@ static void encode_intra_mb(enc_t* e, const uint8_t* cur_nv12, int mbx, int mby,
       for (int blk = 0; blk < 16; blk++) bits4 += m4.i4_modes[blk_y[blk] * 4 + blk_x[blk]] == i4_pred_mode(e, mbx, mby, blk_x[blk], blk_y[blk]) ? 1 : 4;
       *m = keep; }
     const int64_t l2 = rd_lambda[qp];
-    if (d4 + l2 * bits4 < d16 + l2 * bits16 && !e->no_i4) {
+    if (d4 + l2 * bits4 < d16 + l2 * bits16) {
       int8_t cm = m->chroma_mode;
       *m = m4; m->type = 3; m->chroma_mode = cm;
       for (int r = 0; r < 16; r++) memcpy(ry + (size_t)(mby * 16 + r) * e->cw + mbx * 16, rec4 + 16 * r, 16);
@@ -738,13 +738,13 @@ static void encode_inter_mb(enc_t* e, const uint8_t* cur_nv12, int mbx, int mby,
    * AND it costs less than the zero vector (otherwise a stale vector could survive on a scene that has become static);
    * quarter-sample refinement then runs as after a search. */
   int pred_hit = 0, src_mvx = 0, src_mvy = 0, dyr = 16, tried_zero = 0;      /* src_mv: the vector the accepted candidate was derived from */
-  if (search && prev_type == 1 && !e->no_tpred) {
+  if (search && prev_type == 1) {
     const int cdx = asr(prev_mvx + 2, 2), cdy = asr(prev_mvy + 2, 2);
     tried_zero = !(cdx | cdy);
     if ((!tried_zero || !e->no_zcand) && try_candidate(cy, win, cdx, cdy, lambda, sad0, &best)) { search = 0; pred_hit = 1; bdx = cdx; bdy = cdy; src_mvx = prev_mvx; src_mvy = prev_mvy; }
   }
   /* anchor predictor: the vector the anchor of this macroblock's 4x4 group found in THIS picture (anchors run first) */
-  if (search && !e->no_tpred && !e->no_anchor && !is_anchor(e, mbx, mby)) {
+  if (search && !e->no_anchor && !is_anchor(e, mbx, mby)) {
     int ax, ay; anchor_of(e, mbx, mby, &ax, &ay);
     const mb_t* a = &e->mbs[ay * e->mbw + ax];
     const int cdx = asr(a->me_mv[0] + 2, 2), cdy = asr(a->me_mv[1] + 2, 2);
@@ -782,7 +782,7 @@ static void encode_inter_mb(enc_t* e, const uint8_t* cur_nv12, int mbx, int mby,
   /* a predictor hit whose previous vector was full-sample is not refined again: the previous refinement already preferred it */
   const int pred_frac = pred_hit && ((src_mvx | src_mvy) & 3);
   /* ... nor when it is hopeless (mean absolute difference of 32 per sample and more: new content, nothing to polish) */
-  if ((search || pred_frac) && iabs(bdx) <= 13 && iabs(bdy) <= 13 && sad_int > ME_EARLY_SAD_PER_LAMBDA * lambda && (e->no_refine_cap || sad_int < ME_REFINE_MAX_SAD)) {
+  if ((search || pred_frac) && iabs(bdx) <= 13 && iabs(bdy) <= 13 && sad_int > ME_EARLY_SAD_PER_LAMBDA * lambda && sad_int < ME_REFINE_MAX_SAD) {
     int16_t b1[22][17];
     const int ox = 16 + bdx, oy = 16 + bdy;
     for (int v = -3; v <= 18; v++) for (int u = -3; u <= 18; u++) Gp[v + 3][u + 3] = win[oy + v][ox + u];
@@ -1218,7 +1218,7 @@ void* b2v_ref_enc_create(int width, int height, int slice_rows) {
   e->mbs = (mb_t*)calloc((size_t)e->mbw * e->mbh, sizeof(mb_t));
   e->fb[0].qp = e->fb[1].qp = -1; e->paint_burst = 1;
   e->seg_cols = auto_seg_cols(e->mbw, e->mbh);
-  e->no_i4 = getenv("B2V_REF_NO_I4") != NULL; e->no_tpred = getenv("B2V_REF_NO_TPRED") != NULL; e->no_refine_cap = getenv("B2V_REF_NO_REFINE_CAP") != NULL; e->no_anchor = getenv("B2V_REF_NO_ANCHOR") != NULL; e->no_newcontent = getenv("B2V_REF_NO_NEWCONTENT") != NULL; e->no_zcand = getenv("B2V_REF_NO_ZCAND") != NULL;
+  e->no_anchor = getenv("B2V_REF_NO_ANCHOR") != NULL; e->no_newcontent = getenv("B2V_REF_NO_NEWCONTENT") != NULL; e->no_zcand = getenv("B2V_REF_NO_ZCAND") != NULL;
   write_param_sets(e);
   return e;
 }

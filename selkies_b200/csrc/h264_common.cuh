@@ -484,4 +484,20 @@ __device__ __forceinline__ void apply_pcm(MbTile& t, int lane, uint8_t* nnz_mb) 
   if (lane < 24) nnz_mb[lane] = 16;
 }
 
+// The macroblock at luma column x0 of macroblock row mby in and out of the tile, 8 luma samples per lane (row lane >> 1, columns
+// (lane & 1) * 8 ..) and 8 interleaved chroma bytes per lane 0..15.  stage_source returns this lane's luma samples.  ysz = f.cw * f.ch,
+// where the chroma plane starts, comes from the caller: recomputed here, it costs k_inter_lean and k_intra_rows two registers each.
+__device__ __forceinline__ uint2 stage_source(const FrameCtx& f, MbTile& t, int lane, int x0, int mby, size_t ysz) {
+  const int r8 = lane >> 1, c8 = (lane & 1) * 8;
+  const uint2 v = *reinterpret_cast<const uint2*>(f.cur + (size_t)(mby * 16 + r8) * f.cw + x0 + c8);
+  *reinterpret_cast<uint2*>(&t.cur_y[r8][c8]) = v;
+  if (lane < 16) *reinterpret_cast<uint2*>(&t.cur_uv[r8][c8]) = *reinterpret_cast<const uint2*>(f.cur + ysz + (size_t)(mby * 8 + r8) * f.cw + x0 + c8);
+  return v;
+}
+__device__ __forceinline__ void store_recon(const FrameCtx& f, const MbTile& t, int lane, int x0, int mby, size_t ysz) {
+  const int r8 = lane >> 1, c8 = (lane & 1) * 8;
+  *reinterpret_cast<uint2*>(f.recon + (size_t)(mby * 16 + r8) * f.cw + x0 + c8) = *reinterpret_cast<const uint2*>(&t.rec_y[r8][c8]);
+  if (lane < 16) *reinterpret_cast<uint2*>(f.recon + ysz + (size_t)(mby * 8 + r8) * f.cw + x0 + c8) = *reinterpret_cast<const uint2*>(&t.rec_uv[r8][c8]);
+}
+
 }  // namespace b2v

@@ -15,8 +15,11 @@
 // Three passes per picture (DESIGN.md §5.3).  k_inter_lean takes every macroblock in raster order and finishes the ones that leave
 // through the zero vector or an unrefined temporal-predictor hit — most of a desktop picture — without the search's registers and
 // shared memory; it queues the rest.  k_inter_search then runs twice: over the queued anchors, then over everything else queued,
-// which reads the anchors' vectors.  Apart from that, there is no dependency between macroblocks of a P picture: motion-vector
-// prediction and the P_Skip decision only matter for entropy coding and are resolved in h264_entropy.cu.
+// which reads the anchors' vectors.  Both kernels take a macroblock's early exits through the same functions (start_mb,
+// temporal_predictor, stage_pred_window, test_candidate) on inputs that nothing writes during the analysis of a picture, so a queued
+// macroblock's tests decide in k_inter_search as they did in k_inter_lean.  Apart from the anchors' vectors, there is no dependency
+// between macroblocks of a P picture: motion-vector prediction and the P_Skip decision only matter for entropy coding and are
+// resolved in h264_entropy.cu.
 // Encoder decisions: DESIGN.md §5.3; CPU restatement: oracle/h264_ref.c encode_inter_mb().
 #include "h264_common.cuh"
 #include "h264_kernels.h"
@@ -43,9 +46,9 @@ struct alignas(16) LeanSm {       // one per warp of k_inter_lean
 };
 // rows [r0, ...) x words [w0, w0 + stride) of the 48 x 12-word window, stored densely: the whole window or the k_inter_lean part
 struct WinView {
-  const uint32_t* p;
+  uint32_t* p;
   int stride, r0, w0;
-  __device__ __forceinline__ const uint32_t* at(int r, int w) const { return p + (r - r0) * stride + (w - w0); }
+  __device__ __forceinline__ uint32_t* at(int r, int w) const { return p + (r - r0) * stride + (w - w0); }
 };
 
 constexpr int ME_PRED_SAD_FACTOR = 4;      // temporal predictor accepted up to 4x the early-termination threshold (and only as a strict local minimum)
@@ -145,10 +148,10 @@ __device__ __forceinline__ uint32_t search_rows(const InterSm& sm, int lane, int
 
 // A macroblock's place: its band's first row and the anchor of its 4x4 group — one per group, at offset (1,1), groups counted inside
 // each band (oracle/h264_ref.c anchor_of()).  An anchor's vector is the first candidate of the other macroblocks of its group whose
-// temporal predictor failed.
+// temporal predictor failed.  `inside`: the window's 48 columns lie inside the picture, so it needs no per-sample clamping.
 struct MbPos {
   int mb, mbx, mby, band_r0, ax, ay;
-  bool anchor;
+  bool anchor, inside;
 };
 __device__ __forceinline__ MbPos mb_pos(const FrameCtx& f, int mb) {
   MbPos p;
@@ -157,22 +160,66 @@ __device__ __forceinline__ MbPos mb_pos(const FrameCtx& f, int mb) {
   p.ax = min(4 * (p.mbx >> 2) + 1, f.mbw - 1);
   p.ay = p.band_r0 + min(4 * ((p.mby - p.band_r0) >> 2) + 1, min(f.mbh - p.band_r0, f.band_rows) - 1);
   p.anchor = p.ax == p.mbx && p.ay == p.mby;
+  p.inside = p.mbx >= 1 && p.mbx * 16 + 32 <= f.cw;
   return p;
 }
 
-// the 16x16 source block and its chroma into the tile; returns this lane's 8 luma samples (row lane >> 1, columns (lane & 1) * 8 ..)
-__device__ __forceinline__ uint2 stage_source(const FrameCtx& f, MbTile& t, int lane, int x0, int mby) {
-  const int r8 = lane >> 1, c8 = (lane & 1) * 8;
-  const uint2 v = *reinterpret_cast<const uint2*>(f.cur + (size_t)(mby * 16 + r8) * f.cw + x0 + c8);
-  *reinterpret_cast<uint2*>(&t.cur_y[r8][c8]) = v;
-  if (lane < 16) {
-    const uint2 w = *reinterpret_cast<const uint2*>(f.cur + (size_t)f.cw * f.ch + (size_t)(mby * 8 + r8) * f.cw + x0 + c8);
-    *reinterpret_cast<uint2*>(&t.cur_uv[r8][c8]) = w;
-  }
-  return v;
+// The start of a macroblock in both passes: one batch of independent global loads — the source block, staged into the tile, the
+// co-located luma block z and, speculatively (otherwise they cost a dependent-load latency later), the co-located chroma reference
+// (the chroma prediction of a zero vector) and the previous picture's record (temporal predictor) — and SAD(0,0) from the source and
+// z as loaded.  The tile is read by other lanes after a __syncwarp.
+struct MbStart { uint32_t uv_coloc; uint2 z; MbInfo prev; int sad0; };
+__device__ __forceinline__ MbStart start_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p) {
+  const size_t ysz = (size_t)f.cw * f.ch;
+  const int x0 = p.mbx * 16, r8 = lane >> 1, c8 = (lane & 1) * 8;
+  MbStart s;
+  s.uv_coloc = __ldg(reinterpret_cast<const uint32_t*>(f.ref + ysz + (size_t)(p.mby * 8 + (lane >> 2)) * f.cw + x0 + (lane & 3) * 4));
+  s.z = __ldg(reinterpret_cast<const uint2*>(f.ref + (size_t)(p.mby * 16 + r8) * f.cw + x0 + c8));
+  s.prev = f.mbinfo_prev[p.mb];
+  const uint2 c = stage_source(f, t, lane, x0, p.mby, ysz);
+  s.sad0 = __reduce_add_sync(FULL, (int)sad4acc(c.x, s.z.x, sad4acc(c.y, s.z.y, 0u)));
+  return s;
 }
 
 // ---- temporal-predictor early termination (DESIGN.md §5.3; oracle/h264_ref.c encode_inter_mb / try_candidate) ----
+// A vector (quarter samples) as a full-sample candidate (kx,ky); true when the candidate's 3x3 test lies inside the window.
+__device__ __forceinline__ bool full_sample_candidate(int mvx, int mvy, int& kx, int& ky) {
+  kx = (mvx + 2) >> 2; ky = (mvy + 2) >> 2;
+  return kx >= -15 && kx <= 14 && ky >= -15 && ky <= 15;
+}
+// The temporal predictor: the vector this macroblock had in the previous picture, rounded to full samples (scrolling and panning
+// content repeats it; the zero vector counts: static content whose co-located SAD sits just above the early-termination threshold
+// would otherwise search only to find (0,0) again), and the 24 rows x 8 words of the window from (ra, wa) on that its test, a refinement
+// around it and its prediction touch: rows [13+cdy, 36+cdy] and bytes [13+cdx, 34+cdx] cover the 3x3 test (rows 15+cdy..32+cdy), the
+// 6-tap support (-3..+18) and the prediction, clamped so that they stay inside the window.
+struct TemporalPred { int cdx, cdy, ra, wa; bool try_pred; };
+__device__ __forceinline__ TemporalPred temporal_predictor(const MbInfo& prev) {
+  TemporalPred tp;
+  tp.try_pred = full_sample_candidate(prev.mvx, prev.mvy, tp.cdx, tp.cdy) && prev.type == MB_P16;
+  tp.ra = min(max(13 + tp.cdy, 0), WIN_ROWS - PW_ROWS); tp.wa = min(max((13 + tp.cdx) >> 2, 0), WIN_WORDS - PW_WORDS);
+  return tp;
+}
+// Those 24 rows x 8 words (a macroblock whose window lies inside the picture) into `dst`: the whole window or k_inter_lean's dense
+// copy of that part, so that both passes test the predictor on the same words at the same window coordinates.
+__device__ __forceinline__ void stage_pred_window(const FrameCtx& f, const WinView& dst, int lane, const MbPos& p, int ylo, int yhi, const TemporalPred& tp) {
+  const uint32_t* base = reinterpret_cast<const uint32_t*>(f.ref + p.mbx * 16 - 16);
+  uint32_t v[6];
+#pragma unroll
+  for (int k = 0; k < 6; k++) {
+    const int idx = lane + 32 * k;
+    v[k] = __ldg(base + (size_t)clip3i(ylo, yhi, p.mby * 16 - 16 + tp.ra + (idx >> 3)) * (f.cw >> 2) + tp.wa + (idx & 7));
+  }
+#pragma unroll
+  for (int k = 0; k < 6; k++) {
+    const int idx = lane + 32 * k;
+    *dst.at(tp.ra + (idx >> 3), tp.wa + (idx & 7)) = v[k];
+  }
+  __syncwarp();
+}
+
+// the SAD of a candidate key (cost << 11 | candidate index) whose vector is (mvx, mvy), quarter samples
+__device__ __forceinline__ int key_sad(uint32_t key, int lambda, int mvx, int mvy) { return (int)(key >> 11) - lambda * (se_bits_dev(mvx) + se_bits_dev(mvy)); }
+
 // Candidate (kx,ky), full samples, window staged around it: true (and `best` = its key) when its SAD is within 4x the noise
 // threshold AND it is a strict local minimum of the cost over its 8 full-sample neighbours AND it costs no more than the zero vector.
 __device__ __forceinline__ bool test_candidate(const WinView& w, const MbTile& t, int lane, int kx, int ky, int lambda, int sad0, uint32_t& best) {
@@ -193,9 +240,8 @@ __device__ __forceinline__ bool test_candidate(const WinView& w, const MbTile& t
       if (i == 0 && j == 0) kc = key; else kmin = min(kmin, key);
     }
   }
-  const int sadc = (int)(kc >> 11) - lambda * (se_bits_dev(4 * kx) + se_bits_dev(4 * ky));
   const uint32_t key0 = ((uint32_t)(sad0 + 2 * lambda) << 11) | (uint32_t)(16 * 32 + 16);   // ... and it must not cost more than the zero vector
-  if (sadc <= ME_PRED_SAD_FACTOR * ME_EARLY_SAD_PER_LAMBDA * lambda && kc < kmin && kc <= key0) { best = kc; return true; }
+  if (key_sad(kc, lambda, 4 * kx, 4 * ky) <= ME_PRED_SAD_FACTOR * ME_EARLY_SAD_PER_LAMBDA * lambda && kc < kmin && kc <= key0) { best = kc; return true; }
   return false;
 }
 
@@ -219,7 +265,7 @@ __device__ __forceinline__ void publish_anchor(const FrameCtx& f, int mb, int sa
 __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc) {
   const size_t ysz = (size_t)f.cw * f.ch;
   const uint8_t* __restrict__ ref_uv = f.ref + ysz;
-  const int r8 = lane >> 1, c8 = (lane & 1) * 8, rc4 = lane >> 2, cc4 = (lane & 3) * 4;
+  const int rc4 = lane >> 2, cc4 = (lane & 3) * 4;
   const int mb = p.mb, mbx = p.mbx, mby = p.mby;
   {
     // chroma: mvC = luma mv, in 1/8 chroma samples (8.4.1.4, 8.4.2.2.2)
@@ -260,13 +306,8 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
   if (48 + luma_bits + chroma_bits > MB_BITS_LIMIT) { apply_pcm(t, lane, f.nnz + (size_t)mb * 32); cbp = -1; }   // A.3.1: send raw
   __syncwarp();
   {
-    const int ry = mb / f.mbw, rx0 = (mb - ry * f.mbw) * 16;
-    const uint2 v = *reinterpret_cast<const uint2*>(&t.rec_y[r8][c8]);
-    *reinterpret_cast<uint2*>(f.recon + (size_t)(ry * 16 + r8) * f.cw + rx0 + c8) = v;
-    if (lane < 16) {
-      const uint2 w = *reinterpret_cast<const uint2*>(&t.rec_uv[r8][c8]);
-      *reinterpret_cast<uint2*>(f.recon + ysz + (size_t)(ry * 8 + r8) * f.cw + rx0 + c8) = w;
-    }
+    const int ry = mb / f.mbw;
+    store_recon(f, t, lane, (mb - ry * f.mbw) * 16, ry, ysz);
     if (lane == 0) {
       MbInfo mi; mi.mvx = (int16_t)(mv & 0xffff); mi.mvy = (int16_t)(mv >> 16); mi.type = MB_P16; mi.i16_mode = 0; mi.chroma_mode = 0; mi.cbp = (uint8_t)cbp;
       if (cbp < 0) { mi.mvx = 0; mi.mvy = 0; mi.type = MB_PCM; mi.cbp = 0; }   // too big for CAVLC: I_PCM (transform_mb)
@@ -290,46 +331,28 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
   MbTile& t = sm.t;
   const int qp = frame_qp(f), lambda = me_lambda[qp];
   const int ylo = p.band_r0 * 16, yhi = min(f.mbh, p.band_r0 + f.band_rows) * 16 - 1;
-  const uint8_t* __restrict__ ref_y = f.ref;
-  const int x0 = p.mbx * 16, y0 = p.mby * 16, r8 = lane >> 1, c8 = (lane & 1) * 8;
-  // one batch of independent global loads: co-located chroma and luma reference, the previous picture's record, the source block
-  const uint32_t uv_coloc = __ldg(reinterpret_cast<const uint32_t*>(f.ref + (size_t)f.cw * f.ch + (size_t)(p.mby * 8 + (lane >> 2)) * f.cw + x0 + (lane & 3) * 4));
-  const uint2 z = __ldg(reinterpret_cast<const uint2*>(ref_y + (size_t)(y0 + r8) * f.cw + x0 + c8));
-  const MbInfo prev = f.mbinfo_prev[m];
-  const uint2 c = stage_source(f, t, lane, x0, p.mby);
+  const MbStart s = start_mb(f, t, lane, p);
   __syncwarp();
 
   // zero-motion early termination: co-located block within the quantisation noise of this QP
-  const int sad0 = __reduce_add_sync(FULL, (int)sad4acc(c.x, z.x, sad4acc(c.y, z.y, 0u)));
   int mvx = 0, mvy = 0, sad_int = 0;
-  if (sad0 <= ME_EARLY_SAD_PER_LAMBDA * lambda) {
-    *reinterpret_cast<uint2*>(&t.pred_y[r8][c8]) = z;
+  if (s.sad0 <= ME_EARLY_SAD_PER_LAMBDA * lambda) {
+    *reinterpret_cast<uint2*>(&t.pred_y[lane >> 1][(lane & 1) * 8]) = s.z;
   } else {
-    // the temporal predictor, with the 24 rows x 8 words around it that its test and its prediction touch (k_inter_search stages
-    // the same words at the same window coordinates).  A picture-edge macroblock, which needs per-sample clamping, is deferred.
-    const int cdx = (prev.mvx + 2) >> 2, cdy = (prev.mvy + 2) >> 2;
-    const bool try_pred = prev.type == MB_P16 && cdx >= -15 && cdx <= 14 && cdy >= -15 && cdy <= 15;
+    // the temporal predictor on the part of the window around it.  A picture-edge macroblock, which needs per-sample clamping, is
+    // deferred.
+    const TemporalPred tp = temporal_predictor(s.prev);
     bool hit = false;
-    if (try_pred && x0 >= 16 && x0 + 32 <= f.cw) {
-      const int ra = min(max(13 + cdy, 0), WIN_ROWS - PW_ROWS), wa = min(max((13 + cdx) >> 2, 0), WIN_WORDS - PW_WORDS);
-      const uint32_t* base = reinterpret_cast<const uint32_t*>(ref_y + x0 - 16);
-      uint32_t v[6];
-#pragma unroll
-      for (int k = 0; k < 6; k++) {
-        const int idx = lane + 32 * k;
-        v[k] = __ldg(base + (size_t)clip3i(ylo, yhi, y0 - 16 + ra + (idx >> 3)) * (f.cw >> 2) + wa + (idx & 7));
-      }
-#pragma unroll
-      for (int k = 0; k < 6; k++) sm.pw[(lane + 32 * k) >> 3][lane & 7] = v[k];
-      __syncwarp();
-      const WinView w{&sm.pw[0][0], PW_WORDS, ra, wa};
+    if (tp.try_pred && p.inside) {
+      const WinView w{&sm.pw[0][0], PW_WORDS, tp.ra, tp.wa};
+      stage_pred_window(f, w, lane, p, ylo, yhi, tp);
       uint32_t best;
       // a hit whose previous vector was fractional is refined: k_inter_search does that
-      hit = test_candidate(w, t, lane, cdx, cdy, lambda, sad0, best) && ((prev.mvx | prev.mvy) & 3) == 0;
+      hit = test_candidate(w, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best) && ((s.prev.mvx | s.prev.mvy) & 3) == 0;
       if (hit) {
-        full_sample_pred(w, t, lane, 16 + cdx, 16 + cdy);
-        mvx = 4 * cdx; mvy = 4 * cdy;
-        sad_int = (int)(best >> 11) - lambda * (se_bits_dev(mvx) + se_bits_dev(mvy));
+        full_sample_pred(w, t, lane, 16 + tp.cdx, 16 + tp.cdy);
+        mvx = 4 * tp.cdx; mvy = 4 * tp.cdy;
+        sad_int = key_sad(best, lambda, mvx, mvy);
       }
     }
     if (!hit) {
@@ -341,61 +364,32 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
     }
   }
   if (p.anchor && lane == 0) publish_anchor(f, m, sad_int, mvx, mvy);
-  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, uv_coloc);
+  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
-// One macroblock that k_inter_lean queued, from the start: its zero-motion and temporal-predictor tests are repeated on the same
-// inputs (source, reference and the previous picture's records are not written during the analysis of a picture) and so fail, or
-// hit, exactly as they did there.
+// One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
+// previous picture's records are not written during the analysis of a picture).  Its co-located block failed the zero-motion test
+// there and fails it again here, so that test is not repeated; its temporal predictor fails, or hits, as it did there.
 __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int lane, const MbPos& p) {
-  const int mb = p.mb, mbx = p.mbx, mby = p.mby, x0 = mbx * 16, y0 = mby * 16;
+  const int mb = p.mb, x0 = p.mbx * 16, y0 = p.mby * 16;
   const bool anchor = p.anchor;
   MbTile& t = sm.t;
   const WinView win{&sm.win[0][0], WIN_WORDS, 0, 0};
-  const int qp = frame_qp(f);
+  const int qp = frame_qp(f), lambda = me_lambda[qp];
   // reference rows this macroblock may touch: its own band (the band's decoder pads at the band's edges, 8.4.2.2.1)
   const int ylo = p.band_r0 * 16, yhi = min(f.mbh, p.band_r0 + f.band_rows) * 16 - 1;
-  const size_t ysz = (size_t)f.cw * f.ch;
-  const uint8_t* __restrict__ ref_y = f.ref; const uint8_t* __restrict__ ref_uv = f.ref + ysz;
-  const int r8 = lane >> 1, c8 = (lane & 1) * 8, rc4 = lane >> 2, cc4 = (lane & 3) * 4;
-
-  // ---- stage the source block and the search window ------------------------------------------------
-  // one batch of independent global loads: source block, co-located reference block, and — speculatively, they are needed again a
-  // dependent-load latency later otherwise — the co-located chroma reference (the chroma prediction of a zero vector) and this
-  // macroblock's record of the previous picture (temporal predictor)
-  const uint32_t uv_coloc = __ldg(reinterpret_cast<const uint32_t*>(ref_uv + (size_t)(mby * 8 + rc4) * f.cw + x0 + cc4));
-  const MbInfo prev = f.mbinfo_prev[mb];                    // the previous picture's record (other half of the double buffer)
-  {
-    stage_source(f, t, lane, x0, mby);
-    // the co-located 16x16 block first (window rows 16..31, words 4..7)
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      const int i = lane + 32 * k;
-      sm.win[16 + (i >> 2)][4 + (i & 3)] = __ldg(reinterpret_cast<const uint32_t*>(ref_y + (size_t)(y0 + (i >> 2)) * f.cw + x0) + (i & 3));
-    }
-  }
+  const uint8_t* __restrict__ ref_y = f.ref;
+  const MbStart s = start_mb(f, t, lane, p);
+  *reinterpret_cast<uint2*>(&sm.win[16 + (lane >> 1)][4 + (lane & 1) * 2]) = s.z;     // the co-located block: window rows 16..31, words 4..7
   __syncwarp();
 
-  // ---- zero-motion early termination (DESIGN.md §5.3): co-located block within the quantisation noise of this QP ----
-  const int lambda = me_lambda[qp];
-  uint32_t best = (uint32_t)(16 * 32 + 16);      // candidate (0,0)
-  int sad0;
-  {
-    const uint32_t* w0p = &sm.win[16 + r8][4 + (c8 >> 2)];
-    const uint32_t s0 = sad4acc(*reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8]), w0p[0],
-                                sad4acc(*reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8 + 4]), w0p[1], 0u));
-    sad0 = __reduce_add_sync(FULL, (int)s0);
-    if (sad0 > ME_EARLY_SAD_PER_LAMBDA * lambda) best = 0xffffffffu;
-  }
-  // ---- not static: stage the reference.  A macroblock that carries a vector from the previous picture first gets only what the
-  // temporal-predictor test, the refinement around it and the final prediction can touch — 24 rows x 8 words around the predicted
-  // position instead of the 48 x 12 window; the rest follows only if the predictor is rejected and the search has to run.
-  const int cdx = (prev.mvx + 2) >> 2, cdy = (prev.mvy + 2) >> 2;
-  const bool try_pred = prev.type == MB_P16 && cdx >= -15 && cdx <= 14 && cdy >= -15 && cdy <= 15;     // the zero vector included
-  const bool x_inside = x0 >= 16 && x0 + 32 <= f.cw;
+  // ---- the reference.  A macroblock that carries a vector from the previous picture first gets only what the temporal-predictor
+  // test, the refinement around it and the final prediction can touch — 24 rows x 8 words around the predicted position instead of
+  // the 48 x 12 window; the rest follows only if the predictor is rejected and the search has to run.
+  const TemporalPred tp = temporal_predictor(s.prev);
   bool window_complete = false;
   auto stage_window = [&]() {
-    if (x_inside) {   // 512 more words: lanes 0..23 take (row pair j, word) = two rows of 12 words per step — no index arithmetic
+    if (p.inside) {   // 512 more words: lanes 0..23 take (row pair j, word) = two rows of 12 words per step — no index arithmetic
       // beyond an add per step —, every load issued before the first shared-memory store
       uint32_t v[24];
       const int half = lane >= 12 ? 1 : 0, w = lane - 12 * half;
@@ -428,31 +422,12 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
     window_complete = true;
     __syncwarp();
   };
-  if (best == 0xffffffffu) {
-    if (x_inside && try_pred) {
-      // rows [13+cdy, 36+cdy] and bytes [13+cdx, 34+cdx] of the window cover the 3x3 predictor test (rows 15+cdy..32+cdy), the 6-tap
-      // support of a refinement around it (-3..+18) and the prediction; clamped so that 24 rows x 8 words stay inside the window
-      const int ra = min(max(13 + cdy, 0), WIN_ROWS - PW_ROWS), wa = min(max((13 + cdx) >> 2, 0), WIN_WORDS - PW_WORDS);
-      const uint32_t* base = reinterpret_cast<const uint32_t*>(ref_y + x0 - 16);
-      uint32_t v[6];
-#pragma unroll
-      for (int k = 0; k < 6; k++) {
-        const int idx = lane + 32 * k, row = ra + (idx >> 3), w = wa + (idx & 7);
-        v[k] = __ldg(base + (size_t)clip3i(ylo, yhi, y0 - 16 + row) * (f.cw >> 2) + w);
-      }
-#pragma unroll
-      for (int k = 0; k < 6; k++) {
-        const int idx = lane + 32 * k;
-        sm.win[ra + (idx >> 3)][wa + (idx & 7)] = v[k];
-      }
-      __syncwarp();
-    } else stage_window();
-  }
-  // ---- temporal predictor: the vector this macroblock had in the previous picture, rounded to full samples (scrolling / panning
-  // content repeats it; the zero vector counts: static content whose co-located SAD sits just above the early-termination threshold
-  // would otherwise search only to find (0,0) again); quarter-sample refinement then runs as after a search. ----
-  bool pred_hit = false, pred_frac = false, reduced = false;
-  if (best == 0xffffffffu && try_pred && test_candidate(win, t, lane, cdx, cdy, lambda, sad0, best)) { pred_hit = true; pred_frac = ((prev.mvx | prev.mvy) & 3) != 0; }
+  // k_inter_lean did not test the predictor of a picture-edge macroblock: it is tested here, on the full clamped window
+  if (p.inside && tp.try_pred) stage_pred_window(f, win, lane, p, ylo, yhi, tp); else stage_window();
+  // ---- temporal predictor; quarter-sample refinement then runs as after a search ----
+  uint32_t best = 0xffffffffu;
+  bool pred_frac = false, reduced = false;
+  if (tp.try_pred && test_candidate(win, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best)) pred_frac = ((s.prev.mvx | s.prev.mvy) & 3) != 0;
   // ---- anchor predictor (oracle/h264_ref.c encode_inter_mb): the temporal predictor failed (or there was none) — motion that
   // STARTS in this picture.  Instead of one exhaustive search per macroblock, try what this group's anchor has found. ----
   if (best == 0xffffffffu && !anchor) {
@@ -462,12 +437,13 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
     const unsigned long long v = f.me_pub[(size_t)p.ay * f.mbw + p.ax];
     const bool have = (uint32_t)(v >> 32) == (uint32_t)f.pic + 1u;
     const int amvx = (int)(int8_t)(v >> 8), amvy = (int)(int8_t)v;
-    const int kx = (amvx + 2) >> 2, ky = (amvy + 2) >> 2;
-    const bool zero_again = (kx | ky) == 0 && try_pred && (cdx | cdy) == 0;      // the zero vector is not tested twice
-    if (have && !zero_again && kx >= -15 && kx <= 14 && ky >= -15 && ky <= 15 && test_candidate(win, t, lane, kx, ky, lambda, sad0, best)) { pred_hit = true; pred_frac = ((amvx | amvy) & 3) != 0; }
+    int kx, ky;
+    const bool in_window = full_sample_candidate(amvx, amvy, kx, ky);
+    const bool zero_again = (kx | ky) == 0 && tp.try_pred && (tp.cdx | tp.cdy) == 0;      // the zero vector is not tested twice
+    if (have && !zero_again && in_window && test_candidate(win, t, lane, kx, ky, lambda, s.sad0, best)) pred_frac = ((amvx | amvy) & 3) != 0;
     // new content: the anchor's exhaustive search found nothing (bit 16) and the co-located block is as far off — the search
     // shrinks to the rows around dy = 0: picking the least bad of 1089 noise candidates buys hardly more than picking it of 160
-    else reduced = have && ((v >> 16) & 1) != 0 && sad0 >= ME_REFINE_MAX_SAD;
+    else reduced = have && ((v >> 16) & 1) != 0 && s.sad0 >= ME_REFINE_MAX_SAD;
   }
   const bool searched = best == 0xffffffffu;
   if (searched && !window_complete) stage_window();          // predictor rejected: the search needs the whole window
@@ -478,7 +454,7 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   int mvx = 4 * dx, mvy = 4 * dy;
   // refine only inside the window (6-tap support [-3,+18]) and when the full-sample match is not already within the
   // quantisation noise of this QP (same threshold as the zero-motion early termination)
-  const int sad_int = (searched || pred_hit) ? (int)(best >> 11) - lambda * (se_bits_dev(4 * dx) + se_bits_dev(4 * dy)) : 0;
+  const int sad_int = key_sad(best, lambda, 4 * dx, 4 * dy);
   // a predictor hit whose previous vector was full-sample is not refined again: the previous refinement already preferred it
   // ... and not when the full-sample match is hopeless (mean absolute difference >= 32 per sample: new content, nothing to polish —
   // the refinement is a third of the work of a searched macroblock and bought 0 % bits on such pictures)
@@ -550,7 +526,7 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   }
   if (anchor && lane == 0) publish_anchor(f, mb, sad_int, mvx, mvy);
   if (!refine) full_sample_pred(win, t, lane, dxi, dyi);
-  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, uv_coloc);
+  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
 // Passes B and C: the queue k_inter_lean filled (0: anchors, 1: the rest), walked by a grid of the kernel's resident capacity.  No

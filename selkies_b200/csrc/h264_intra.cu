@@ -116,8 +116,6 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
   const int qp = frame_qp(f);
   const int lambda = me_lambda[qp];
   const size_t ysz = (size_t)f.cw * f.ch;
-  const uint8_t* cur_y = f.cur; const uint8_t* cur_uv = f.cur + ysz;
-  uint8_t* rec_y = f.recon; uint8_t* rec_uv = f.recon + ysz;
   const int r8 = lane >> 1, c8 = (lane & 1) * 8;            // this lane's 8 luma pixels
   const int rc4 = lane >> 2, cc4 = (lane & 3) * 4;          // this lane's 4 interleaved chroma bytes
   const QuantParams q4 = make_quant(qp, true);
@@ -136,15 +134,7 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
   for (int mbx = geo.x0; mbx < geo.x1; mbx++) {
     const int mb = mby * f.mbw + mbx;
     const bool has_left = mbx > geo.x0;
-    // ---- load current macroblock (warp 0) ------------------------------------------------------------
-    if (warp == 0) {
-      const uint2 v = *reinterpret_cast<const uint2*>(cur_y + (size_t)(mby * 16 + r8) * f.cw + mbx * 16 + c8);
-      *reinterpret_cast<uint2*>(&t.cur_y[r8][c8]) = v;
-      if (lane < 16) {
-        const uint2 w = *reinterpret_cast<const uint2*>(cur_uv + (size_t)(mby * 8 + r8) * f.cw + mbx * 16 + c8);
-        *reinterpret_cast<uint2*>(&t.cur_uv[r8][c8]) = w;
-      }
-    }
+    if (warp == 0) stage_source(f, t, lane, mbx * 16, mby, ysz);     // load the current macroblock
     __syncthreads();
     int best_mode = 2, cbest = 0, cbp = 0, luma_bits16 = 0, chroma_bits = 0;
     long long d16 = 0;
@@ -318,12 +308,7 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
     __syncwarp();
     if (est > MB_BITS_LIMIT) { apply_pcm(t, lane, nnz_mb); type = MB_PCM; cbp = 0; __syncwarp(); }   // A.3.1: send raw
     {
-      const uint2 v = *reinterpret_cast<const uint2*>(&t.rec_y[r8][c8]);
-      *reinterpret_cast<uint2*>(rec_y + (size_t)(mby * 16 + r8) * f.cw + mbx * 16 + c8) = v;
-      if (lane < 16) {
-        const uint2 w = *reinterpret_cast<const uint2*>(&t.rec_uv[r8][c8]);
-        *reinterpret_cast<uint2*>(rec_uv + (size_t)(mby * 8 + r8) * f.cw + mbx * 16 + c8) = w;
-      }
+      store_recon(f, t, lane, mbx * 16, mby, ysz);
       // right column becomes the next macroblock's left neighbour
       if (lane < 16) nb.left_y[lane] = t.rec_y[lane][15];
       else nb.left_uv[lane - 16] = t.rec_uv[(lane - 16) >> 1][14 + ((lane - 16) & 1)];
