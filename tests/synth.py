@@ -57,6 +57,25 @@ def desktop(w, h, t=0, seed=1):
     return f
 
 
+def tiles(w, h, noise_at=(), light_at=(), seed=0, grey=130, base=None):
+    """A flat grey field (or a copy of `base`) with 16x16 tiles at macroblock addresses (raster order, ceil(w / 16) macroblocks per
+    row).  Grey 130 converts to Y = Cb = Cr = 128, which intra DC prediction reproduces exactly at any QP.  At the addresses of
+    `noise_at`: uniform noise, I_PCM at QP 0 and 4 in IDR slices and in P pictures whose reference holds something else there; at
+    those of `light_at`: a flat tile a few levels off grey, which costs a few bits.  Fresh noise per seed, so that a motion
+    search never finds a tile of an earlier picture."""
+    f = np.array(base) if base is not None else np.full((h, w, 4), grey, np.uint8)
+    f[..., 3] = 255
+    mbw = (w + 15) // 16
+    rng = np.random.default_rng(seed)
+    for a in noise_at:
+        y, x = a // mbw * 16, a % mbw * 16
+        f[y:y + 16, x:x + 16, :3] = rng.integers(0, 256, (16, 16, 3), dtype=np.uint8)[: h - y, : w - x]
+    for k, a in enumerate(light_at):
+        y, x = a // mbw * 16, a % mbw * 16
+        f[y:y + 16, x:x + 16, :3] = grey + 6 + 2 * (seed % 5) + k % 3
+    return f
+
+
 def predictor_paths(w, h):
     """Eleven pictures that walk every exit of the P-picture motion search (DESIGN.md §5.3): a still (zero-motion exit), the same with
     +-2 LSB noise (zero-vector candidate), the onset of a scroll (anchors search, their groups take the anchor's vector), the scroll
