@@ -157,9 +157,30 @@ int   b2v_ring_submit(void* h, int32_t slot, int32_t stride_bytes, int64_t captu
 /* Give an acquired slot back WITHOUT encoding it (the producer had no frame after all: end of a canned source, a grab that
  * failed).  Only the most recently acquired slot can be returned; the next b2v_ring_acquire hands out the same slot. */
 int   b2v_ring_release(void* h, int32_t slot);
-/* device-resident frames (bench `value`: inputs already in HBM) */
+/* device-resident frames (bench `value`: inputs already in HBM); b2v_submit_resident is b2v_submit_device of the library's own
+ * copy (BGRA, no producer stream) */
 int   b2v_resident_upload(void* h, int32_t index, const void* bgra_host, int32_t stride_bytes);
 int   b2v_submit_resident(void* h, int32_t index, int64_t capture_ns);
+
+/* ---- frame ingest from device memory (a producer whose frames are already on the session's GPU: a renderer through CUDA/GL
+ *      interop, a compositor's exported buffers, a PyTorch model).  No copy: the colour conversion reads the frame in place. */
+enum { B2V_PIX_BGRA = 0, B2V_PIX_RGBA = 1, B2V_PIX_BGR = 2, B2V_PIX_RGB = 3 };   /* byte order in memory; alpha ignored */
+/* Encodes `frame`: src_h rows of src_w pixels (the session's source size; scaling, striped mode, JPEG mode and
+ * B2V_FLAG_NO_ENCODE apply as for b2v_ring_submit) at `pitch_bytes`, in device (or managed) memory of the session's GPU.
+ *
+ * Stream order, both ways.  `cuda_stream` is the producer's stream on the session's device (NULL = the legacy default stream;
+ * cudaStreamPerThread is accepted).  The picture's colour conversion runs after everything enqueued on `cuda_stream` before this
+ * call (an event recorded there, waited on by the library's stream: the host never blocks on the producer), and work enqueued
+ * on `cuda_stream` after this call runs after that conversion (an event recorded behind it, waited on by `cuda_stream`).  So
+ * when the call returns, the producer may overwrite or free the buffer in stream order on `cuda_stream`; from another stream it
+ * must order itself after `cuda_stream` first.  Settings apply as for any submit (see "When a call takes effect" below).
+ *
+ * Rejections (B2V_EINVAL + message, nothing enqueued, the session keeps running): an unknown pixel_format; a null handle or
+ * frame; pitch_bytes < src_w * bytes per pixel; frame or pitch not a multiple of 4 for BGRA / RGBA; memory that is not device
+ * or managed memory of the session's device (host memory, pinned and mapped host memory included: the kernel would read it
+ * over PCIe); a frame whose last byte, frame + pitch_bytes * (src_h - 1) + src_w * bytes per pixel - 1, lies outside the
+ * allocation that holds `frame`.  A stream of another device fails the session like any CUDA error during a submit. */
+int   b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, void* cuda_stream, int64_t capture_ns);
 int   b2v_flush(void* h);                                /* wait until every submitted frame was delivered */
 
 /* ---- live control: ScreenCapture.update_framerate (media_pipeline.py:236),

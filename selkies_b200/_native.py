@@ -17,6 +17,7 @@ B2V_OK, B2V_EINVAL, B2V_ECUDA, B2V_ENOMEM, B2V_ESTATE, B2V_ETIMEOUT = 0, -1, -2,
 B2V_RC_CBR, B2V_RC_CQP = 0, 1
 B2V_HDR_NONE, B2V_HDR_PIXELFLUX = 0, 1
 B2V_FLAG_SPS_EVERY_IDR, B2V_FLAG_NO_ENCODE, B2V_FLAG_TIMING, B2V_FLAG_DEVICE_TIMER, B2V_FLAG_TIMING_CSC, B2V_FLAG_JPEG = 1, 2, 4, 8, 16, 32
+B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
 
 
 class B2VSettings(C.Structure):
@@ -70,6 +71,7 @@ SYMBOLS = [
     ("b2v_ring_release", C.c_int, [C.c_void_p, C.c_int32]),
     ("b2v_resident_upload", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
     ("b2v_submit_resident", C.c_int, [C.c_void_p, C.c_int32, C.c_int64]),
+    ("b2v_submit_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64]),
     ("b2v_flush", C.c_int, [C.c_void_p]),
     ("b2v_set_framerate", C.c_int, [C.c_void_p, C.c_double]),
     ("b2v_set_bitrate_kbps", C.c_int, [C.c_void_p, C.c_int32]),

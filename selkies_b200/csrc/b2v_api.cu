@@ -1,5 +1,5 @@
 // b2v_api.cu — the C-ABI of libb2video.so (include/b2video.h): session lifecycle, the pinned BGRA
-// ingest ring, stream/event plumbing and the output thread that fires the frame callback.
+// ingest ring, device-memory ingest, stream/event plumbing and the output thread that fires the frame callback.
 //
 // Replaces pixelflux.ScreenCapture as the reference drives it (media_pipeline.py:275-332,
 // selkies.py:3091-3189): start_capture -> b2v_create, stop_capture -> b2v_destroy,
@@ -7,6 +7,8 @@
 //
 // Per-frame flow (four streams, events in between; nothing on the host blocks except ring back-pressure):
 //   st_copy : cudaMemcpyAsync  pinned slot -> device BGRA slot                      (a) ingest
+//             (b2v_submit_device: no copy; st_enc waits for an event on the producer's stream, and the producer's stream
+//             waits for an event behind the CSC)
 //   st_enc  : fused CSC(+scale) -> NV12 cur ; analysis (k_intra_rows / k_inter_lean + k_inter_search), or the whole JPEG encode   (b),(c)
 //   st_pack : entropy coding of the same picture (k_cavlc_mb -> k_slice_build, which runs the rate-control step -> k_pack_au)
 //             -> AU in HBM, overlapping the analysis of the next picture on st_enc (h264_encoder.cu)
@@ -24,6 +26,8 @@
 
 #include <sys/prctl.h>
 #include <time.h>
+
+#include <cuda.h>                         // CUresult / CUdeviceptr only: driver entry points are reached through the runtime
 
 #include "../../include/b2video.h"
 #include "b2v_internal.h"
@@ -118,6 +122,7 @@ struct Session {
   int out_next = 0;
   int ring_next = 0;
   cudaEvent_t ev_timer[2] = {};
+  cudaEvent_t ev_dev_in = nullptr, ev_dev_done = nullptr;   // b2v_submit_device: producer -> st_enc, CSC -> producer
   unsigned long long* d_csc_ts = nullptr;     // [kMaxSlots][2] device stamps of the CSC launches (timing mode)
 
   // frame sequencing
@@ -216,9 +221,9 @@ void free_geometry(Session* s) {
   if (s->jenc) { jpeg_destroy(s->jenc); s->jenc = nullptr; }
 }
 
-CscParams csc_params(Session* s, const uint8_t* d_bgra, int stride, uint8_t* d_nv12) {
+CscParams csc_params(Session* s, const uint8_t* d_src, int stride, int fmt, uint8_t* d_nv12) {
   CscParams p{};
-  p.src = d_bgra; p.src_w = s->src_w; p.src_h = s->src_h; p.src_stride = stride;
+  p.src = d_src; p.src_w = s->src_w; p.src_h = s->src_h; p.src_stride = stride; p.fmt = fmt;
   p.dst_w = s->dst_w; p.dst_h = s->dst_h; p.coded_w = s->coded_w; p.coded_h = s->coded_h;
   p.out_y = d_nv12; p.out_uv = d_nv12 + (size_t)s->coded_w * s->coded_h;
   p.tx = s->d_tx; p.ty = s->d_ty;
@@ -387,8 +392,9 @@ int submit_failed(Session* s, int out_idx, int in_slot, cudaError_t e, const cha
 #define CKS(call)                                                                              \
   do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return submit_failed(s, out_idx, in_slot, e_, #call); } while (0)
 
-// common tail of b2v_ring_submit / b2v_submit_resident: CSC + encode + D2H + job
-int submit_common(Session* s, const uint8_t* d_bgra, int stride, int in_slot, int64_t capture_ns) {
+// common tail of b2v_ring_submit / b2v_submit_device / b2v_submit_resident: CSC + encode + D2H + job.  `producer` (device
+// frames of the caller) is the stream the CSC is ordered after, and that is ordered after the CSC in turn; null: no such stream.
+int submit_common(Session* s, const uint8_t* d_src, int stride, int fmt, int in_slot, const cudaStream_t* producer, int64_t capture_ns) {
   int out_idx = 0;
   Job j{};
   EncodeFrameParams fp{};
@@ -430,8 +436,12 @@ int submit_common(Session* s, const uint8_t* d_bgra, int stride, int in_slot, in
     s->submitted++;
     s->stats.frames_submitted++;
   }
-  CscParams cp = csc_params(s, d_bgra, stride, s->d_cur);
+  CscParams cp = csc_params(s, d_src, stride, fmt, s->d_cur);
   cudaEvent_t* ev = j.timing ? s->ev_t[out_idx] : nullptr;
+  if (producer) {
+    CKS(cudaEventRecord(s->ev_dev_in, *producer));
+    CKS(cudaStreamWaitEvent(s->st_enc, s->ev_dev_in, 0));
+  }
   if (ev && s->d_csc_ts && s->encode) {
     cp.ts = s->d_csc_ts + 2 * out_idx;
     cudaMemsetAsync(cp.ts, 0xFF, sizeof(unsigned long long), s->st_enc);
@@ -440,6 +450,10 @@ int submit_common(Session* s, const uint8_t* d_bgra, int stride, int in_slot, in
   if (ev) cudaEventRecord(ev[0], s->st_enc);
   int nl = launch_csc(cp, s->st_enc);
   if (ev) cudaEventRecord(ev[1], s->st_enc);
+  if (producer) {                       // the caller may reuse the frame in stream order once the CSC has read it
+    CKS(cudaEventRecord(s->ev_dev_done, s->st_enc));
+    CKS(cudaStreamWaitEvent(*producer, s->ev_dev_done, 0));
+  }
   cudaStream_t st_done = s->st_enc;     // where the access unit (without encoding: the NV12 picture) is complete
   if (s->encode && s->jpeg) {
     nl += jpeg_encode(s->jenc, s->d_cur, s->d_au[out_idx], j.is_key, s->st_enc);
@@ -482,12 +496,56 @@ void release_session(Session* s) {
   }
   if (s->ev_timer[0]) cudaEventDestroy(s->ev_timer[0]);
   if (s->ev_timer[1]) cudaEventDestroy(s->ev_timer[1]);
+  if (s->ev_dev_in) cudaEventDestroy(s->ev_dev_in);
+  if (s->ev_dev_done) cudaEventDestroy(s->ev_dev_done);
   if (s->d_csc_ts) cudaFree(s->d_csc_ts);
   if (s->st_copy) cudaStreamDestroy(s->st_copy);
   if (s->st_enc) cudaStreamDestroy(s->st_enc);
   if (s->st_out) cudaStreamDestroy(s->st_out);
   if (s->st_pack) cudaStreamDestroy(s->st_pack);
   delete s;
+}
+
+// Checks of b2v_submit_device on the caller's frame (include/b2video.h), before anything is enqueued: the arguments first, with
+// no CUDA call; then what the driver knows of the memory.  Caller holds submit_mu.
+typedef CUresult (*AddressRangeFn)(CUdeviceptr* base, size_t* size, CUdeviceptr p);
+AddressRangeFn address_range_fn() {
+  static const AddressRangeFn fn = [] {         // the runtime's driver entry point: libb2video does not link libcuda itself
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q{};
+    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+      cudaGetLastError();
+      f = nullptr;
+    }
+    return (AddressRangeFn)f;
+  }();
+  return fn;
+}
+
+int check_device_frame(Session* s, const uint8_t* frame, int pitch, int fmt) {
+  const int bpp = fmt < B2V_PIX_BGR ? 4 : 3;
+  const int64_t row = (int64_t)s->src_w * bpp;
+  if (pitch < row) return fail(B2V_EINVAL, "pitch %d is below one row of the frame (%d pixels x %d bytes)", pitch, s->src_w, bpp);
+  if (bpp == 4 && (((uintptr_t)frame & 3) || (pitch & 3)))
+    return fail(B2V_EINVAL, "4-byte pixels need a frame address and a pitch that are multiples of 4 (frame %p, pitch %d)", (const void*)frame, pitch);
+  CK(cudaSetDevice(s->device));
+  cudaPointerAttributes a{};
+  cudaError_t e = cudaPointerGetAttributes(&a, frame);
+  if (e != cudaSuccess) { cudaGetLastError(); return fail(B2V_EINVAL, "frame %p: %s", (const void*)frame, cudaGetErrorString(e)); }
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+    return fail(B2V_EINVAL, "frame %p is not device memory (%s memory): the colour conversion would read it over PCIe", (const void*)frame,
+                a.type == cudaMemoryTypeHost ? "page-locked host" : "unregistered host");
+  if (a.device != s->device) return fail(B2V_EINVAL, "frame %p is memory of device %d, the session runs on device %d", (const void*)frame, a.device, s->device);
+  const AddressRangeFn range = address_range_fn();
+  if (!range) return fail(B2V_ECUDA, "cuMemGetAddressRange is not available from the CUDA driver");
+  CUdeviceptr base = 0;
+  size_t size = 0;
+  if (range(&base, &size, (CUdeviceptr)(uintptr_t)frame) != CUDA_SUCCESS) return fail(B2V_EINVAL, "frame %p: no device allocation holds it", (const void*)frame);
+  const unsigned long long end = (unsigned long long)(uintptr_t)frame + (unsigned long long)pitch * (s->src_h - 1) + (unsigned long long)row;
+  if (end > (unsigned long long)base + size)
+    return fail(B2V_EINVAL, "frame %p: %d rows at pitch %d end %llu bytes past the end of its allocation (%zu bytes at 0x%llx)", (const void*)frame,
+                s->src_h, pitch, end - ((unsigned long long)base + size), size, (unsigned long long)base);
+  return 0;
 }
 
 // b2v_bench_csc (burst = false: each launch bracketed by its own event pair, the sum excludes host launch gaps) and
@@ -502,7 +560,7 @@ int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launc
   std::vector<uint8_t*> outs(n_resident, nullptr);
   size_t ob = (size_t)s->coded_w * s->coded_h * 3 / 2;
   for (auto& o : outs) CK(cudaMalloc((void**)&o, ob));
-  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, s->resident[i], s->src_w * 4, outs[i]), s->st_enc);   // warm-up
+  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, s->resident[i], s->src_w * 4, B2V_PIX_BGRA, outs[i]), s->st_enc);   // warm-up
   CK(cudaStreamSynchronize(s->st_enc));
   const int pairs = burst ? 1 : iters;
   std::vector<cudaEvent_t> e0(pairs), e1(pairs);
@@ -511,7 +569,7 @@ int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launc
   for (int i = 0; i < iters; i++) {
     int k = i % n_resident;
     if (!burst) cudaEventRecord(e0[i], s->st_enc);
-    launch_csc(csc_params(s, s->resident[k], s->src_w * 4, outs[k]), s->st_enc);
+    launch_csc(csc_params(s, s->resident[k], s->src_w * 4, B2V_PIX_BGRA, outs[k]), s->st_enc);
     if (!burst) cudaEventRecord(e1[i], s->st_enc);
   }
   if (burst) cudaEventRecord(e1[0], s->st_enc);
@@ -576,6 +634,8 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   }
   for (auto& evs : s->ev_t) for (cudaEvent_t& e : evs) cudaEventCreate(&e);
   cudaEventCreate(&s->ev_timer[0]); cudaEventCreate(&s->ev_timer[1]);
+  cudaEventCreateWithFlags(&s->ev_dev_in, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&s->ev_dev_done, cudaEventDisableTiming);
   if (s->timing && (cfg->flags & B2V_FLAG_DEVICE_TIMER)) cudaMalloc((void**)&s->d_csc_ts, sizeof(unsigned long long) * 2 * kMaxSlots);
   int rc = alloc_geometry(s);
   if (rc) { release_session(s); return rc; }
@@ -651,7 +711,7 @@ int b2v_ring_submit(void* h, int32_t slot, int32_t stride, int64_t capture_ns) {
     s->stats.h2d_bytes += (int64_t)stride * s->src_h;
     s->stats.ns_submit += now_ns() - t0;
   }
-  return submit_common(s, s->dev_slot[slot], stride, slot, capture_ns);
+  return submit_common(s, s->dev_slot[slot], stride, B2V_PIX_BGRA, slot, nullptr, capture_ns);
 }
 
 int b2v_resident_upload(void* h, int32_t index, const void* bgra, int32_t stride) {
@@ -671,7 +731,18 @@ int b2v_submit_resident(void* h, int32_t index, int64_t capture_ns) {
   if (!s || index < 0 || index >= (int)s->resident.size() || !s->resident[index]) return fail(B2V_EINVAL, "resident frame %d not uploaded", index);
   std::lock_guard<std::mutex> sub(s->submit_mu);
   CK(cudaSetDevice(s->device));
-  return submit_common(s, s->resident[index], s->src_w * 4, -1, capture_ns);
+  return submit_common(s, s->resident[index], s->src_w * 4, B2V_PIX_BGRA, -1, nullptr, capture_ns);
+}
+
+int b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, void* cuda_stream, int64_t capture_ns) {
+  Session* s = (Session*)h;
+  if (pixel_format < B2V_PIX_BGRA || pixel_format > B2V_PIX_RGB) return fail(B2V_EINVAL, "unknown pixel format %d", pixel_format);
+  if (!s || !frame) return fail(B2V_EINVAL, "null argument");
+  std::lock_guard<std::mutex> sub(s->submit_mu);         // the source size is stable from here on (b2v_set_resolution takes it too)
+  int rc = check_device_frame(s, (const uint8_t*)frame, pitch_bytes, pixel_format);
+  if (rc) return rc;
+  const cudaStream_t producer = (cudaStream_t)cuda_stream;
+  return submit_common(s, (const uint8_t*)frame, pitch_bytes, pixel_format, -1, &producer, capture_ns);
 }
 
 int b2v_flush(void* h) {
@@ -788,7 +859,7 @@ int b2v_csc_nv12(void* h, const void* bgra, int32_t stride, void* nv12) {
   CK(cudaMalloc((void**)&d_in, (size_t)s->src_w * 4 * s->src_h));
   CK(cudaMalloc((void**)&d_out, out_bytes));
   CK(cudaMemcpy2DAsync(d_in, (size_t)s->src_w * 4, bgra, stride, (size_t)s->src_w * 4, s->src_h, cudaMemcpyHostToDevice, s->st_enc));
-  CscParams p = csc_params(s, d_in, s->src_w * 4, d_out);
+  CscParams p = csc_params(s, d_in, s->src_w * 4, B2V_PIX_BGRA, d_out);
   p.coded_w = s->dst_w; p.coded_h = s->dst_h;          // visible region only
   p.out_uv = d_out + (size_t)s->dst_w * s->dst_h;
   launch_csc(p, s->st_enc);

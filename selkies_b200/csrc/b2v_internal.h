@@ -4,6 +4,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "../../include/b2video.h"
+
 namespace b2v {
 
 // ---- access-unit container: both encoders write it into HBM, the session's output thread reads it ----
@@ -42,7 +44,7 @@ constexpr int KVR = 7196, KVG = -6536, KVB = -660;
 struct Tap { int32_t i0; int32_t i1; int32_t f; int32_t pad; };
 
 struct CscParams {
-  const uint8_t* src;   // BGRA, device
+  const uint8_t* src;   // device; pixels in the byte order `fmt` names
   int src_w, src_h, src_stride;
   int dst_w, dst_h;     // visible (scaled) size
   int coded_w, coded_h; // output plane size (multiples of 16 for the encoder; == dst for csc-only)
@@ -52,6 +54,8 @@ struct CscParams {
   const Tap* ty;        // dst_h taps
   unsigned long long* ts; // null, or {min block-start, max block-end} %globaltimer stamps of this launch (B2V_FLAG_TIMING)
   int matrix;             // 0 = BT.709 limited range (H.264 path), 1 = JFIF full-range BT.601 (JPEG stripe path)
+  int fmt;                // B2V_PIX_*: 4 bytes per pixel (BGRA, RGBA) or 3 (BGR, RGB); src and src_stride are multiples of 4 for the
+                          // 4-byte orders
 };
 
 // returns number of kernel launches issued (1)

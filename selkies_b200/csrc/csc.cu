@@ -1,4 +1,4 @@
-// csc.cu — fused BGRA -> BT.709 limited-range NV12 colour conversion (+ bilinear scale), sm_90a.
+// csc.cu — fused BGRA / RGBA / BGR / RGB -> BT.709 limited-range NV12 colour conversion (+ bilinear scale), sm_90a.
 //
 // Replaces the colour-conversion stage of the reference's native capture module
 // (pixelflux, call site src/selkies/media_pipeline.py:299-300; legacy GStreamer
@@ -12,6 +12,12 @@
 //              issued back to back so four 16-byte loads are in flight per thread.
 //   arithmetic: dp2a (two 16-bit coefficient x 8-bit pixel MACs per instruction); rounding
 //              constant and the +16 / +128 offsets are folded into the accumulator seed.
+//   packed 3-byte path (BGR / RGB, 1:1, width % 16 == 0): one thread = 16 px x 2 rows: 4.5 B/px algorithmic.  A warp reads
+//              its 1536 B of a row as three warp-contiguous 16-byte loads, trades them through shared memory so that each
+//              thread holds its own 48 B, expands them to pixel words with byte permutes and stores 16 B of Y per row and
+//              16 B of CbCr.
+//   channel order: RGBA and RGB swap the coefficients of bytes 0 and 2 (at compile time in the 1:1 kernels, by matrix row in
+//              the others); the pixels are never reordered.
 //   general path (scaled or ragged widths): one thread per 2x2 output block, taps from tables.
 #include <mutex>
 
@@ -35,7 +41,7 @@ __device__ __forceinline__ void st_stream(uint8_t* p, unsigned v) {
   asm volatile("st.global.cs.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// pixel word: byte0 = B, byte1 = G, byte2 = R, byte3 = A (ignored: coefficient 0)
+// pixel word: byte0 = B, byte1 = G, byte2 = R, byte3 = A (ignored: coefficient 0).  With S (RGBA, RGB) byte0 = R, byte2 = B.
 __host__ __device__ constexpr int pack16(int lo, int hi) { return (int)(((unsigned)lo & 0xffffu) | ((unsigned)hi << 16)); }
 // Colour matrices (14-bit coefficients).  0: BT.709 limited range, the H.264 path (DESIGN.md §3).  1: JFIF full-range BT.601, the
 // JPEG stripe path (0.5 is coded as 8191 so that a saturated red / blue stays at 255; greys still give exactly 128) — the same
@@ -43,7 +49,18 @@ __host__ __device__ constexpr int pack16(int lo, int hi) { return (int)(((unsign
 template <int M> struct Mx;
 template <> struct Mx<0> { static constexpr int YR = KYR, YG = KYG, YB = KYB, UR = KUR, UG = KUG, UB = KUB, VR = KVR, VG = KVG, VB = KVB, YOFF = 16; };
 template <> struct Mx<1> { static constexpr int YR = 4899, YG = 9617, YB = 1868, UR = -2765, UG = -5427, UB = 8191, VR = 8191, VG = -6860, VB = -1332, YOFF = 0; };
-__device__ const int c_mx[2][10] = {{KYR, KYG, KYB, KUR, KUG, KUB, KVR, KVG, KVB, 16}, {4899, 9617, 1868, -2765, -5427, 8191, 8191, -6860, -1332, 0}};
+// Coefficients of bytes 0 and 2 of a pixel word, by channel order (S: byte 0 is R).
+template <int M, bool S> struct Ord {
+  using X = Mx<M>;
+  static constexpr int Y0 = S ? X::YR : X::YB, Y2 = S ? X::YB : X::YR, U0 = S ? X::UR : X::UB, U2 = S ? X::UB : X::UR,
+                       V0 = S ? X::VR : X::VB, V2 = S ? X::VB : X::VR;
+};
+// Rows of the general and scaled kernels, indexed by 2 * matrix + (pixel_format & 1): {Y, Cb, Cr coefficients of the channels
+// read as (R, G, B)} and the luma offset.  The odd rows swap R and B: those kernels call byte 2 "R" and byte 0 "B" whatever
+// the order, and the swapped row weighs each byte by its true channel, so the sums are the same integers.
+__device__ const int c_mx[4][10] = {{KYR, KYG, KYB, KUR, KUG, KUB, KVR, KVG, KVB, 16}, {KYB, KYG, KYR, KUB, KUG, KUR, KVB, KVG, KVR, 16},
+                                    {4899, 9617, 1868, -2765, -5427, 8191, 8191, -6860, -1332, 0},
+                                    {1868, 9617, 4899, 8191, -5427, -2765, -1332, -6860, 8191, 0}};
 constexpr int C_SEED = (128 << 16) + (1 << 15);
 
 __device__ __forceinline__ unsigned dp2a_lo_u(unsigned coef, unsigned px, unsigned acc) {
@@ -55,11 +72,12 @@ __device__ __forceinline__ unsigned dp2a_hi_u(unsigned coef, unsigned px, unsign
 // Luma with the coefficients scaled by 4 (all three are positive and 4*KYG still fits an UNSIGNED 16-bit dp2a lane):
 // 4*(k.px) + 4*seed puts (k.px + seed) >> 14 into byte 2 of the accumulator, exactly (the factor 4 is exact), so the result is
 // picked up by the same byte permute that packs four pixels — no shift instruction per pixel.  Chroma (>> 16) sits in byte 2 already.
-template <int M>
+template <int M, bool S>
 __device__ __forceinline__ unsigned luma_b2(unsigned px) {      // Y in byte 2
   using X = Mx<M>;
+  using O = Ord<M, S>;
   static_assert(4 * X::YG < 65536 && 4 * (X::YR + X::YG + X::YB) * 255 + 4 * ((X::YOFF << 14) + (1 << 13)) < (1 << 24), "luma accumulator must stay below byte 3");
-  constexpr unsigned lo = (unsigned)pack16(4 * X::YB, 4 * X::YG), hi = (unsigned)pack16(4 * X::YR, 0), seed = 4u * (unsigned)((X::YOFF << 14) + (1 << 13));
+  constexpr unsigned lo = (unsigned)pack16(4 * O::Y0, 4 * X::YG), hi = (unsigned)pack16(4 * O::Y2, 0), seed = 4u * (unsigned)((X::YOFF << 14) + (1 << 13));
   return dp2a_hi_u(hi, px, dp2a_lo_u(lo, px, seed));
 }
 __device__ __forceinline__ int chroma_acc(int clo, int chi, unsigned px, int acc) {
@@ -71,12 +89,13 @@ __device__ __forceinline__ unsigned pack4_b2(unsigned a, unsigned b, unsigned c,
 }
 
 // 4 px x 2 rows -> Y (two u32) + CbCr (one u32 = Cb0 Cr0 Cb1 Cr1)
-template <int M = 0>
+template <int M, bool S>
 __device__ __forceinline__ void convert_quad(const uint4& a, const uint4& b, unsigned& y0, unsigned& y1, unsigned& uv) {
   using X = Mx<M>;
-  constexpr int CU_LO = pack16(X::UB, X::UG), CU_HI = pack16(X::UR, 0), CV_LO = pack16(X::VB, X::VG), CV_HI = pack16(X::VR, 0);
-  y0 = pack4_b2(luma_b2<M>(a.x), luma_b2<M>(a.y), luma_b2<M>(a.z), luma_b2<M>(a.w));
-  y1 = pack4_b2(luma_b2<M>(b.x), luma_b2<M>(b.y), luma_b2<M>(b.z), luma_b2<M>(b.w));
+  using O = Ord<M, S>;
+  constexpr int CU_LO = pack16(O::U0, X::UG), CU_HI = pack16(O::U2, 0), CV_LO = pack16(O::V0, X::VG), CV_HI = pack16(O::V2, 0);
+  y0 = pack4_b2(luma_b2<M, S>(a.x), luma_b2<M, S>(a.y), luma_b2<M, S>(a.z), luma_b2<M, S>(a.w));
+  y1 = pack4_b2(luma_b2<M, S>(b.x), luma_b2<M, S>(b.y), luma_b2<M, S>(b.z), luma_b2<M, S>(b.w));
   int u0 = chroma_acc(CU_LO, CU_HI, b.y, chroma_acc(CU_LO, CU_HI, b.x, chroma_acc(CU_LO, CU_HI, a.y, chroma_acc(CU_LO, CU_HI, a.x, C_SEED))));
   int v0 = chroma_acc(CV_LO, CV_HI, b.y, chroma_acc(CV_LO, CV_HI, b.x, chroma_acc(CV_LO, CV_HI, a.y, chroma_acc(CV_LO, CV_HI, a.x, C_SEED))));
   int u1 = chroma_acc(CU_LO, CU_HI, b.w, chroma_acc(CU_LO, CU_HI, b.z, chroma_acc(CU_LO, CU_HI, a.w, chroma_acc(CU_LO, CU_HI, a.z, C_SEED))));
@@ -88,7 +107,7 @@ __device__ __forceinline__ void convert_quad(const uint4& a, const uint4& b, uns
 // grid.x covers 4-px quads of a row, grid.y strides over groups of CSC_UNITS row pairs.
 constexpr int CSC_UNITS = 2;     // units per thread (DESIGN.md §3)
 constexpr int CSC_BLOCK = 160;   // threads per block, shrunk to a divisor of the row where one exists
-template <int M>
+template <int M, bool S>
 __global__ void __launch_bounds__(256) csc_bgra_nv12_fast(CscParams p, int quads, int pairs) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (p.ts && threadIdx.x == 0) {   // device-side stopwatch of this launch: first block start .. last block end
@@ -112,7 +131,7 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_fast(CscParams p, int quads
       int pr = pr0 + u;
       if (pr < pairs) {
         unsigned y0, y1, uv;
-        convert_quad<M>(a[u], b[u], y0, y1, uv);
+        convert_quad<M, S>(a[u], b[u], y0, y1, uv);
         st_stream(p.out_y + (size_t)(2 * pr) * p.coded_w + q * 4, y0);
         st_stream(p.out_y + (size_t)(2 * pr + 1) * p.coded_w + q * 4, y1);
         st_stream(p.out_uv + (size_t)pr * p.coded_w + q * 4, uv);
@@ -125,16 +144,82 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_fast(CscParams p, int quads
   }
 }
 
+// ---- packed 3-byte fast path (BGR / RGB, 1:1, width % 16 == 0, src and stride 16-byte aligned) --------------------------
+// grid.x covers 16-px units of a row (C3_WARPS warps per block at most), grid.y strides over row pairs.  A warp's 32 units are
+// 1536 B of a row: load k of lane l is the 16-byte chunk 32k + l (one contiguous 512 B per warp instruction); lane l then reads
+// its chunks 3l .. 3l+2 back from shared memory (a 48-byte stride: the eight lanes of a quarter-warp cover 32 banks once).
+constexpr int C3_WARPS = 8;
+__device__ __forceinline__ void st_stream4(uint8_t* p, unsigned a, unsigned b, unsigned c, unsigned d) {
+  asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+// 12 bytes = 4 packed pixels -> 4 pixel words (bytes 0..2 = the pixel in memory order; byte 3 is left over and weighs 0)
+__device__ __forceinline__ uint4 expand3(unsigned a, unsigned b, unsigned c) {
+  return make_uint4(a, __byte_perm(a, b, 0x0543), __byte_perm(b, c, 0x0432), __byte_perm(c, c, 0x0321));
+}
+template <int M, bool S>
+__global__ void __launch_bounds__(C3_WARPS * 32) csc_rgb24_nv12_fast(CscParams p, int units, int pairs) {
+  __shared__ __align__(16) uint4 stage[C3_WARPS][2][96];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int u = blockIdx.x * blockDim.x + threadIdx.x, wu0 = u - lane;      // this thread's unit, the warp's first unit
+  if (p.ts && threadIdx.x == 0) {
+    unsigned long long t0; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0)); atomicMin(p.ts, t0);
+  }
+  if (wu0 < units) {                                                         // warp-uniform
+    const int chunks = min(96, 3 * (units - wu0));
+    for (int pr = blockIdx.y; pr < pairs; pr += gridDim.y) {
+      const int r0 = min(2 * pr, p.src_h - 1), r1 = min(2 * pr + 1, p.src_h - 1);   // bottom padding rows replicate
+      const uint8_t* g0 = p.src + (size_t)r0 * p.src_stride + (size_t)wu0 * 48;
+      const uint8_t* g1 = p.src + (size_t)r1 * p.src_stride + (size_t)wu0 * 48;
+      uint4 a[3], b[3];
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const int c = 32 * k + lane;
+        if (c < chunks) { a[k] = ld_stream(g0 + 16 * c); b[k] = ld_stream(g1 + 16 * c); }
+      }
+      __syncwarp();                                   // the previous pair's reads of `stage` are done
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const int c = 32 * k + lane;
+        if (c < chunks) { stage[w][0][c] = a[k]; stage[w][1][c] = b[k]; }
+      }
+      __syncwarp();
+      if (u < units) {
+        const uint4 x0 = stage[w][0][3 * lane], x1 = stage[w][0][3 * lane + 1], x2 = stage[w][0][3 * lane + 2];
+        const uint4 z0 = stage[w][1][3 * lane], z1 = stage[w][1][3 * lane + 1], z2 = stage[w][1][3 * lane + 2];
+        unsigned y0[4], y1[4], uv[4];
+        convert_quad<M, S>(expand3(x0.x, x0.y, x0.z), expand3(z0.x, z0.y, z0.z), y0[0], y1[0], uv[0]);
+        convert_quad<M, S>(expand3(x0.w, x1.x, x1.y), expand3(z0.w, z1.x, z1.y), y0[1], y1[1], uv[1]);
+        convert_quad<M, S>(expand3(x1.z, x1.w, x2.x), expand3(z1.z, z1.w, z2.x), y0[2], y1[2], uv[2]);
+        convert_quad<M, S>(expand3(x2.y, x2.z, x2.w), expand3(z2.y, z2.z, z2.w), y0[3], y1[3], uv[3]);
+        st_stream4(p.out_y + (size_t)(2 * pr) * p.coded_w + u * 16, y0[0], y0[1], y0[2], y0[3]);
+        st_stream4(p.out_y + (size_t)(2 * pr + 1) * p.coded_w + u * 16, y1[0], y1[1], y1[2], y1[3]);
+        st_stream4(p.out_uv + (size_t)pr * p.coded_w + u * 16, uv[0], uv[1], uv[2], uv[3]);
+      }
+    }
+  }
+  if (p.ts) {
+    __syncthreads();
+    if (threadIdx.x == 0) { unsigned long long t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); atomicMax(p.ts + 1, t1); }
+  }
+}
+
 // ---- general path: bilinear scale and/or ragged width, one thread per 2x2 output block -----
+// pixel word of pixel x of a row: bytes 0..2 are its colour bytes in memory order (3-byte formats: any alignment)
+__device__ __forceinline__ unsigned load_px(const uint8_t* row, int x, int fmt) {
+  if (fmt < B2V_PIX_BGR) return *(const unsigned*)(row + x * 4);
+  const uint8_t* q = row + x * 3;
+  return (unsigned)q[0] | ((unsigned)q[1] << 8) | ((unsigned)q[2] << 16);
+}
+// B = byte 0, R = byte 2 of the pixel word: swapped for RGBA / RGB, which the matrix row c_mx[2 * matrix + 1] accounts for
 __device__ __forceinline__ void fetch_bgr(const CscParams& p, int x, int y, int& B, int& G, int& R) {
   int x0, x1, fx, y0, y1, fy;
   if (p.tx) { Tap t = p.tx[x]; x0 = t.i0; x1 = t.i1; fx = t.f; } else { x0 = x1 = x; fx = 0; }
   if (p.ty) { Tap t = p.ty[y]; y0 = t.i0; y1 = t.i1; fy = t.f; } else { y0 = y1 = y; fy = 0; }
   const uint8_t* r0 = p.src + (size_t)y0 * p.src_stride;
   const uint8_t* r1 = p.src + (size_t)y1 * p.src_stride;
-  unsigned p00 = *(const unsigned*)(r0 + x0 * 4);
+  unsigned p00 = load_px(r0, x0, p.fmt);
   if (fx == 0 && fy == 0) { B = p00 & 255; G = (p00 >> 8) & 255; R = (p00 >> 16) & 255; return; }
-  unsigned p01 = *(const unsigned*)(r0 + x1 * 4), p10 = *(const unsigned*)(r1 + x0 * 4), p11 = *(const unsigned*)(r1 + x1 * 4);
+  unsigned p01 = load_px(r0, x1, p.fmt), p10 = load_px(r1, x0, p.fmt), p11 = load_px(r1, x1, p.fmt);
   int out[3];
 #pragma unroll
   for (int c = 0; c < 3; c++) {
@@ -150,7 +235,7 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscParams p) {
   int bx = blockIdx.x * blockDim.x + threadIdx.x;   // 2x2 block column
   int by = blockIdx.y * blockDim.y + threadIdx.y;
   if (bx * 2 >= p.coded_w || by * 2 >= p.coded_h) return;
-  const int* mx = c_mx[p.matrix];
+  const int* mx = c_mx[2 * p.matrix + (p.fmt & 1)];
   int sb = 0, sg = 0, sr = 0;
   unsigned yy[4];
 #pragma unroll
@@ -174,6 +259,7 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscParams p) {
 // staged in shared memory with 16-byte loads; every tap is then a shared-memory read.  The arithmetic is the spec's (oracle/
 // csc_ref.c fetch_bgr): per channel top/bottom horizontal blends at full precision (B and R ride in the two 16-bit halves of one
 // word: 255*256 fits), one vertical blend, one rounding.  Roofline: 4 B per source pixel read + 1.5 B per output pixel written.
+// Packed 3-byte sources are staged as the same pixel words (any alignment), so everything after the staging is shared.
 constexpr int SC_TW = 64, SC_TH = 8, SC_THREADS = (SC_TW / 2) * (SC_TH / 2);
 
 __device__ __forceinline__ void blend_px(const uint32_t* r0, const uint32_t* r1, int x0, int x1, int fx, int fy, int& B, int& G, int& R) {
@@ -199,14 +285,14 @@ __global__ void __launch_bounds__(SC_THREADS) csc_bgra_nv12_scaled(CscParams p, 
   const int fw4 = (xs1 - xs0 + 4) >> 2, fh = ys1 - ys0 + 1;      // quads per row, rows
   for (int i = tid; i < fh * fw4; i += SC_THREADS) {
     const int r = i / fw4, c = i - r * fw4, sx = xs0 + 4 * c;
-    const uint8_t* g = p.src + (size_t)(ys0 + r) * p.src_stride + (size_t)sx * 4;
+    const uint8_t* row = p.src + (size_t)(ys0 + r) * p.src_stride;
     uint4 v;
-    if (sx + 3 < p.src_w) v = ld_stream(g);
-    else {                                                      // last quad of a row whose width is not a multiple of 4
-      v.x = *reinterpret_cast<const uint32_t*>(g);
-      v.y = sx + 1 < p.src_w ? *reinterpret_cast<const uint32_t*>(g + 4) : 0u;
-      v.z = sx + 2 < p.src_w ? *reinterpret_cast<const uint32_t*>(g + 8) : 0u;
-      v.w = 0u;
+    if (sx + 3 < p.src_w && p.fmt < B2V_PIX_BGR) v = ld_stream(row + (size_t)sx * 4);
+    else {                          // packed 3-byte pixels, or the last quad of a row whose width is not a multiple of 4
+      v.x = load_px(row, sx, p.fmt);
+      v.y = sx + 1 < p.src_w ? load_px(row, sx + 1, p.fmt) : 0u;
+      v.z = sx + 2 < p.src_w ? load_px(row, sx + 2, p.fmt) : 0u;
+      v.w = sx + 3 < p.src_w ? load_px(row, sx + 3, p.fmt) : 0u;
     }
     *reinterpret_cast<uint4*>(&sc_tile[r * fw_cap + 4 * c]) = v;
   }
@@ -215,7 +301,7 @@ __global__ void __launch_bounds__(SC_THREADS) csc_bgra_nv12_scaled(CscParams p, 
   const int bx = tid % (SC_TW / 2), by = tid / (SC_TW / 2);
   const int ox = ox0 + 2 * bx, oy = oy0 + 2 * by;
   if (ox >= p.coded_w || oy >= p.coded_h) return;
-  const int* mx = c_mx[p.matrix];
+  const int* mx = c_mx[2 * p.matrix + (p.fmt & 1)];
   int sb = 0, sg = 0, sr = 0;
   unsigned yy[4];
 #pragma unroll
@@ -262,9 +348,11 @@ static void opt_in_smem(const void* fn, int* granted, int smem) {
 }
 
 int launch_csc(const CscParams& p, cudaStream_t st) {
-  const bool fast = p.tx == nullptr && p.ty == nullptr && p.dst_w == p.src_w && p.dst_h == p.src_h && p.coded_w == p.dst_w &&
-                    (p.coded_w % 4) == 0 && (p.src_stride % 16) == 0 && ((uintptr_t)p.src % 16) == 0 &&
-                    ((uintptr_t)p.out_y % 4) == 0 && ((uintptr_t)p.out_uv % 4) == 0;
+  const bool swap = (p.fmt & 1) != 0, packed3 = p.fmt >= B2V_PIX_BGR;
+  const bool one_to_one = p.tx == nullptr && p.ty == nullptr && p.dst_w == p.src_w && p.dst_h == p.src_h && p.coded_w == p.dst_w;
+  const bool aligned16 = (p.src_stride % 16) == 0 && ((uintptr_t)p.src % 16) == 0;
+  const bool fast = one_to_one && !packed3 && (p.coded_w % 4) == 0 && aligned16 && ((uintptr_t)p.out_y % 4) == 0 && ((uintptr_t)p.out_uv % 4) == 0;
+  const bool fast3 = one_to_one && packed3 && (p.coded_w % 16) == 0 && aligned16 && ((uintptr_t)p.out_y % 16) == 0 && ((uintptr_t)p.out_uv % 16) == 0;
   if (fast) {
     const int quads = p.coded_w / 4, pairs = p.coded_h / 2;
     int block = CSC_BLOCK;
@@ -273,11 +361,29 @@ int launch_csc(const CscParams& p, cudaStream_t st) {
     int gy = (pairs + CSC_UNITS - 1) / CSC_UNITS;            // one group of CSC_UNITS row pairs per block
     if (gy > 65535) gy = 65535;
     const dim3 grid((quads + block - 1) / block, gy);
-    if (p.matrix == 1) csc_bgra_nv12_fast<1><<<grid, block, 0, st>>>(p, quads, pairs);
-    else csc_bgra_nv12_fast<0><<<grid, block, 0, st>>>(p, quads, pairs);
+    if (p.matrix == 1) {
+      if (swap) csc_bgra_nv12_fast<1, true><<<grid, block, 0, st>>>(p, quads, pairs);
+      else csc_bgra_nv12_fast<1, false><<<grid, block, 0, st>>>(p, quads, pairs);
+    } else {
+      if (swap) csc_bgra_nv12_fast<0, true><<<grid, block, 0, st>>>(p, quads, pairs);
+      else csc_bgra_nv12_fast<0, false><<<grid, block, 0, st>>>(p, quads, pairs);
+    }
+  } else if (fast3) {
+    // whole warps of 16-px units, spread evenly over as few blocks of at most C3_WARPS warps as the row needs
+    const int units = p.coded_w / 16, pairs = p.coded_h / 2;
+    const int warps = (units + 31) / 32, bx = (warps + C3_WARPS - 1) / C3_WARPS, block = 32 * ((warps + bx - 1) / bx);
+    const dim3 grid(bx, pairs < 65535 ? pairs : 65535);
+    if (p.matrix == 1) {
+      if (swap) csc_rgb24_nv12_fast<1, true><<<grid, block, 0, st>>>(p, units, pairs);
+      else csc_rgb24_nv12_fast<1, false><<<grid, block, 0, st>>>(p, units, pairs);
+    } else {
+      if (swap) csc_rgb24_nv12_fast<0, true><<<grid, block, 0, st>>>(p, units, pairs);
+      else csc_rgb24_nv12_fast<0, false><<<grid, block, 0, st>>>(p, units, pairs);
+    }
   } else {
-    // scaled: the tiled kernel when the tile's source footprint fits shared memory (any sane scale factor), else the general one
-    if (p.tx && p.ty && (p.src_stride % 16) == 0 && ((uintptr_t)p.src % 16) == 0) {
+    // scaled: the tiled kernel when the tile's source footprint fits shared memory (any sane scale factor), else the general one.
+    // 4-byte pixels are staged with 16-byte loads, so they need a 16-byte aligned source; 3-byte pixels are read bytewise.
+    if (p.tx && p.ty && (packed3 || aligned16)) {
       const long long fw = ((long long)SC_TW * p.src_w + p.dst_w - 1) / p.dst_w + 8, fh = ((long long)SC_TH * p.src_h + p.dst_h - 1) / p.dst_h + 3;
       const int fw_cap = (int)((fw + 3) & ~3LL), fh_cap = (int)fh;
       const long long smem = (long long)fw_cap * fh_cap * 4;

@@ -18,7 +18,9 @@ library's native output thread.
 
 What differs, by construction: the reference's module also grabs the X11 framebuffer.  Screen capture is
 outside this tier (SURVEY.md §8b), so frames come from a pluggable `FrameSource` (default: a synthetic
-desktop generator); a real grabber only has to fill the pinned ring slot it is handed.
+desktop generator); a real grabber only has to fill the pinned ring slot it is handed.  A producer whose
+frames are already on the GPU (a renderer, a compositor, a torch model) is a `DeviceFrameSource`: each
+display reads its capture_x / capture_y window of the device surface in place.
 """
 from __future__ import annotations
 
@@ -113,6 +115,23 @@ class FrameSource:
         raise NotImplementedError
 
 
+class DeviceFrameSource:
+    """Producer of frames in device memory.  `frame(index)` returns a device array (any object with `__cuda_array_interface__`,
+    uint8 (H, W, 4) or (H, W, 3) as `pixel_format` says) covering the whole surface, or None to end the stream.  ScreenCapture
+    encodes its capture_width x capture_height window at (capture_x, capture_y) without a copy, in stream order with the
+    producer (Session.submit_device): the surface may be redrawn on the producer's stream as soon as `frame` returns the next
+    time.  `stream`: the producer's stream, when the array does not name it (None: the array's own, or torch's current)."""
+
+    pixel_format = "BGRA"
+    stream = None
+
+    def configure(self, width: int, height: int) -> None:
+        self.width, self.height = width, height
+
+    def frame(self, index: int):   # pragma: no cover - interface
+        raise NotImplementedError
+
+
 class SyntheticDesktopSource(FrameSource):
     """Flat regions, text-like 1-px patterns and a region scrolling 8 px/frame (SURVEY.md §8d S3)."""
 
@@ -185,6 +204,7 @@ class ScreenCapture:
         self._kf_seconds = -1.0
         self._fps = 60.0
         self._cursor_cb = None
+        self._origin = (0, 0)
         self.frames_emitted = 0
 
     # -- lifecycle ----------------------------------------------------------------------------------
@@ -203,6 +223,7 @@ class ScreenCapture:
                 warnings.warn("h264_fullcolor: this pipeline encodes 4:2:0 (Constrained Baseline); the stream decodes under the 4:4:4 decoder "
                               "configuration the client selects, with chroma at half resolution", RuntimeWarning, stacklevel=2)
             w, h = int(settings.capture_width), int(settings.capture_height)
+            self._origin = (int(getattr(settings, "capture_x", 0) or 0), int(getattr(settings, "capture_y", 0) or 0))   # device sources only
             w -= w & 1
             h -= h & 1                                # the reference forces even sizes (webrtc_mode.py:397-402)
             s = SimpleNamespace(paintover_trigger_frames=0, paintover_crf=0, paintover_burst_frames=0)      # Session keyword arguments; paint-over off
@@ -321,14 +342,8 @@ class ScreenCapture:
             if session is None:
                 break
             with self._resize_lock:
-                try:
-                    slot, view = session.acquire()
-                except N.B2VError:
-                    break                         # the session is stopping
-                if not self._source.fill(view, index):
-                    session.release_slot(slot)    # end of the source: nothing to encode
+                if not self._encode_next(session, index):
                     break
-                session.submit_slot(slot, time.monotonic_ns())
             index += 1
             next_t += 1.0 / max(1e-3, fps)
             delay = next_t - time.perf_counter()
@@ -336,6 +351,30 @@ class ScreenCapture:
                 self._stop.wait(delay)
             else:
                 next_t = time.perf_counter()      # fell behind: do not burst
+
+    def _encode_next(self, session: Session, index: int) -> bool:
+        """Submits frame `index` of the source; False at the end of the source or when the session is stopping."""
+        if isinstance(self._source, DeviceFrameSource):
+            f = self._source.frame(index)
+            if f is None:
+                return False
+            try:
+                session.submit_device(f, pixel_format=self._source.pixel_format, stream=self._source.stream, origin=self._origin,
+                                      capture_ns=time.monotonic_ns())
+            except N.B2VError as e:
+                if e.code == N.B2V_EINVAL:        # the source handed over something the library cannot read: say so
+                    raise
+                return False                      # the session is stopping
+            return True
+        try:
+            slot, view = session.acquire()
+        except N.B2VError:
+            return False                          # the session is stopping
+        if not self._source.fill(view, index):
+            session.release_slot(slot)            # end of the source: nothing to encode
+            return False
+        session.submit_slot(slot, time.monotonic_ns())
+        return True
 
     def _on_frame(self, fptr):
         f = fptr.contents

@@ -7,6 +7,7 @@ pixelflux_compat.ScreenCapture, bench.py and the tests.
 from __future__ import annotations
 
 import ctypes as C
+import sys
 import threading
 from typing import Callable, Optional
 
@@ -28,6 +29,59 @@ class EncodedFrame:
         self.y_start, self.height = y_start, height
 
 
+# pixel formats of device frames: name -> (B2V_PIX_* code, bytes per pixel); the name is the byte order in memory
+PIXEL_FORMATS = {"BGRA": (N.B2V_PIX_BGRA, 4), "RGBA": (N.B2V_PIX_RGBA, 4), "BGR": (N.B2V_PIX_BGR, 3), "RGB": (N.B2V_PIX_RGB, 3)}
+
+
+def device_frame_args(frame, width: int, height: int, device: int, pixel_format: str = "BGRA", origin=(0, 0), stream=None):
+    """Reads the `__cuda_array_interface__` of `frame` and returns the arguments of b2v_submit_device for its `width` x `height`
+    window at `origin` = (x, y): (pointer, pitch in bytes, B2V_PIX_* code, producer stream handle).  The array must be uint8,
+    (H, W, 4) or (H, W, 3) as the format says, with packed pixels and any row stride.  Raises TypeError / ValueError for
+    anything else; the library checks the memory itself (device, allocation bounds).
+
+    Producer stream: `stream` when given (a handle, or an object with `.cuda_stream` such as torch.cuda.Stream); else the
+    array's own `stream` entry (version 3 of the interface: None = nothing to wait for, 1 = the legacy default stream, 2 = the
+    per-thread default stream, otherwise a handle); else, for a torch tensor, torch's current stream on its device; else the
+    legacy default stream."""
+    if pixel_format not in PIXEL_FORMATS:
+        raise ValueError(f"unknown pixel format {pixel_format!r} (one of {', '.join(PIXEL_FORMATS)})")
+    fmt, bpp = PIXEL_FORMATS[pixel_format]
+    cai = getattr(frame, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{type(frame).__name__} has no __cuda_array_interface__: submit_device takes device arrays (host frames go "
+                        "through submit())")
+    torch = sys.modules.get("torch")                   # a torch tensor means torch is imported already; never import it here
+    is_torch = torch is not None and isinstance(frame, torch.Tensor)
+    if is_torch and (frame.device.type != "cuda" or frame.device.index != device):
+        raise ValueError(f"frame is on {frame.device}, the session runs on cuda:{device}")
+    if cai.get("mask") is not None:
+        raise ValueError("masked arrays are not supported")
+    if str(cai["typestr"])[1:] != "u1":
+        raise TypeError(f"frame dtype {cai['typestr']!r}: uint8 pixels are needed")
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 3 or shape[2] != bpp:
+        raise ValueError(f"frame shape {shape}: {pixel_format} needs (H, W, {bpp})")
+    strides = cai.get("strides")
+    pitch, px, ch = (shape[1] * bpp, bpp, 1) if strides is None else (int(v) for v in strides)
+    if px != bpp or ch != 1:
+        raise ValueError(f"frame strides {tuple(strides)}: pixels must be packed ({bpp}, 1); only the row stride is free")
+    if pitch < shape[1] * bpp or pitch >= 1 << 31:
+        raise ValueError(f"row stride {pitch} does not hold a row of {shape[1]} pixels")
+    x, y = (int(v) for v in origin)
+    if x < 0 or y < 0 or x + width > shape[1] or y + height > shape[0]:
+        raise ValueError(f"window {width}x{height} at ({x}, {y}) lies outside the {shape[1]}x{shape[0]} frame")
+    ptr = int(cai["data"][0]) + y * pitch + x * bpp
+    if stream is not None:
+        handle = int(getattr(stream, "cuda_stream", stream))
+    elif "stream" in cai:
+        handle = 0 if cai["stream"] is None else int(cai["stream"])
+    elif is_torch:
+        handle = torch.cuda.current_stream(frame.device).cuda_stream
+    else:
+        handle = 0
+    return ptr, pitch, fmt, handle
+
+
 class Session:
     def __init__(self, width: int, height: int, *, dst_width: int = 0, dst_height: int = 0, fps: float = 60.0,
                  device: int = 0, rc_mode: int = N.B2V_RC_CBR, bitrate_kbps: int = 8000, crf: int = 26,
@@ -35,6 +89,7 @@ class Session:
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
                  collect: bool = True):
         self._lib = N.lib()
+        self.device = device
         self.width, self.height = width, height
         self.dst_width, self.dst_height = dst_width or width, dst_height or height
         self.frames: list[EncodedFrame] = []
@@ -97,6 +152,14 @@ class Session:
 
     def submit_resident(self, index: int, capture_ns: int = 0) -> None:
         N.check(self._lib.b2v_submit_resident(self._h, index, capture_ns))
+
+    def submit_device(self, frame, *, pixel_format: str = "BGRA", stream=None, origin=(0, 0), capture_ns: int = 0) -> None:
+        """Encode the `width` x `height` window at `origin` = (x, y) of a frame in device memory of the session's GPU, without a
+        copy: `frame` is any object with `__cuda_array_interface__` (torch, CuPy, Numba), uint8 (H, W, 4) for BGRA / RGBA or
+        (H, W, 3) for BGR / RGB.  The conversion runs in stream order after the producer's stream (see device_frame_args), and
+        that stream waits for it in turn: the frame may be overwritten in stream order as soon as this returns."""
+        ptr, pitch, fmt, handle = device_frame_args(frame, self.width, self.height, self.device, pixel_format, origin, stream)
+        N.check(self._lib.b2v_submit_device(self._h, ptr, pitch, fmt, handle, capture_ns))
 
     def flush(self) -> None:
         N.check(self._lib.b2v_flush(self._h))
