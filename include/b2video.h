@@ -163,7 +163,8 @@ int   b2v_resident_upload(void* h, int32_t index, const void* bgra_host, int32_t
 int   b2v_submit_resident(void* h, int32_t index, int64_t capture_ns);
 
 /* ---- frame ingest from device memory (a producer whose frames are already on the session's GPU: a renderer through CUDA/GL
- *      interop, a compositor's exported buffers, a PyTorch model).  No copy: the colour conversion reads the frame in place. */
+ *      interop, a compositor's exported buffers; for a PyTorch model's tensors see b2v_submit_tensor).  No copy: the colour
+ *      conversion reads the frame in place. */
 enum { B2V_PIX_BGRA = 0, B2V_PIX_RGBA = 1, B2V_PIX_BGR = 2, B2V_PIX_RGB = 3 };   /* byte order in memory; alpha ignored */
 /* Encodes `frame`: src_h rows of src_w pixels (the session's source size; scaling, striped mode, JPEG mode and
  * B2V_FLAG_NO_ENCODE apply as for b2v_ring_submit) at `pitch_bytes`, in device (or managed) memory of the session's GPU.
@@ -181,7 +182,34 @@ enum { B2V_PIX_BGRA = 0, B2V_PIX_RGBA = 1, B2V_PIX_BGR = 2, B2V_PIX_RGB = 3 };  
  * over PCIe); a frame whose last byte, frame + pitch_bytes * (src_h - 1) + src_w * bytes per pixel - 1, lies outside the
  * allocation that holds `frame`.  A stream of another device fails the session like any CUDA error during a submit. */
 int   b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, void* cuda_stream, int64_t capture_ns);
-int   b2v_flush(void* h);                                /* wait until every submitted frame was delivered */
+
+/* ---- frame ingest of a device tensor as a model leaves it: planar or interleaved, uint8 or floating point in [0, 1], any strides.
+ *      No preparation pass: the colour conversion reads the elements where they are and quantises them in registers. */
+enum { B2V_DT_U8 = 0, B2V_DT_F16 = 1, B2V_DT_BF16 = 2, B2V_DT_F32 = 3 };
+typedef struct b2v_tensor {
+  const void* data;                       /* element (channel 0, row 0, column 0) of the src_w x src_h picture */
+  int32_t dtype;                          /* B2V_DT_*                                                         */
+  int32_t pixel_format;                   /* B2V_PIX_*: how many channels (BGRA / RGBA 4, BGR / RGB 3; a fourth is never read) and
+                                             whether channel 0 is blue or red                                 */
+  int64_t stride_c, stride_y, stride_x;   /* bytes; each positive and a multiple of the element size: the element of channel c,
+                                             row y, column x is at data + c * stride_c + y * stride_y + x * stride_x.  One
+                                             description for (C, H, W), (H, W, C), channels_last, a slice of a batch, a window
+                                             of a larger surface and a padded pitch */
+} b2v_tensor;
+/* b2v_submit_device with this richer description of the frame: the same stream order both ways (the producer may overwrite the
+ * tensor in stream order on `cuda_stream` when the call returns), the same settings, scaling and modes.
+ *
+ * Element -> 8-bit sample: uint8 is the value; fp16 / bf16 / fp32 widen to fp32 and give
+ * q = round_half_even(255 * min(max(x, 0), 1)), one fp32 multiplication; NaN -> 0, -0 -> 0, +inf -> 255 (DESIGN.md §3).  The three
+ * samples of a pixel then take the integer colour conversion of every other entry.  Other value ranges are the caller's to map.
+ *
+ * Rejections (B2V_EINVAL + message, nothing enqueued, the session keeps running): a null handle, descriptor or data; an unknown
+ * dtype or pixel_format; a stride that is <= 0, not a multiple of the element size, or too large (stride_y, stride_x: 2^31 and up;
+ * stride_c: 2^48 and up); data not
+ * aligned to the element size; memory that is not device or managed memory of the session's device; a last byte read,
+ * data + 2 * stride_c + (src_h - 1) * stride_y + (src_w - 1) * stride_x + element size - 1, outside the allocation holding `data`. */
+int   b2v_submit_tensor(void* h, const b2v_tensor* t, void* cuda_stream, int64_t capture_ns);
+int   b2v_flush(void* h);                               /* wait until every submitted frame was delivered */
 
 /* ---- live control: ScreenCapture.update_framerate (media_pipeline.py:236),
  *      update_video_bitrate (:195), request_idr_frame (:244); set_resolution is
@@ -207,6 +235,8 @@ int  b2v_reset_stats(void* h);
 int  b2v_coded_size(void* h, int32_t* coded_w, int32_t* coded_h);
 /* synchronous fused CSC(+scale) of one host BGRA frame to host NV12 (dst_w*dst_h*3/2 bytes) */
 int  b2v_csc_nv12(void* h, const void* bgra_host, int32_t stride_bytes, void* nv12_host);
+/* the same of one device tensor, read in place after the work enqueued on `cuda_stream` (checked as b2v_submit_tensor checks it) */
+int  b2v_csc_nv12_tensor(void* h, const b2v_tensor* t, void* cuda_stream, void* nv12_host);
 /* reconstruction of the last encoded frame: NV12, coded_w*coded_h*3/2 bytes */
 int  b2v_get_recon(void* h, void* nv12_host);
 /* repeat the CSC kernel `iters` times over resident frames and return mean ms per launch

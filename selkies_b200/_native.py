@@ -18,6 +18,7 @@ B2V_RC_CBR, B2V_RC_CQP = 0, 1
 B2V_HDR_NONE, B2V_HDR_PIXELFLUX = 0, 1
 B2V_FLAG_SPS_EVERY_IDR, B2V_FLAG_NO_ENCODE, B2V_FLAG_TIMING, B2V_FLAG_DEVICE_TIMER, B2V_FLAG_TIMING_CSC, B2V_FLAG_JPEG = 1, 2, 4, 8, 16, 32
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
+B2V_DT_U8, B2V_DT_F16, B2V_DT_BF16, B2V_DT_F32 = 0, 1, 2, 3
 
 
 class B2VSettings(C.Structure):
@@ -58,6 +59,13 @@ class B2VStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class B2VTensor(C.Structure):
+    _fields_ = [
+        ("data", C.c_void_p), ("dtype", C.c_int32), ("pixel_format", C.c_int32),
+        ("stride_c", C.c_int64), ("stride_y", C.c_int64), ("stride_x", C.c_int64),
+    ]
+
+
 FRAME_CB = C.CFUNCTYPE(None, C.POINTER(B2VFrame), C.c_void_p)
 
 # every symbol include/b2video.h declares: (name, restype, argtypes)
@@ -72,6 +80,7 @@ SYMBOLS = [
     ("b2v_resident_upload", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
     ("b2v_submit_resident", C.c_int, [C.c_void_p, C.c_int32, C.c_int64]),
     ("b2v_submit_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64]),
+    ("b2v_submit_tensor", C.c_int, [C.c_void_p, C.POINTER(B2VTensor), C.c_void_p, C.c_int64]),
     ("b2v_flush", C.c_int, [C.c_void_p]),
     ("b2v_set_framerate", C.c_int, [C.c_void_p, C.c_double]),
     ("b2v_set_bitrate_kbps", C.c_int, [C.c_void_p, C.c_int32]),
@@ -83,6 +92,7 @@ SYMBOLS = [
     ("b2v_reset_stats", C.c_int, [C.c_void_p]),
     ("b2v_coded_size", C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("b2v_csc_nv12", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    ("b2v_csc_nv12_tensor", C.c_int, [C.c_void_p, C.POINTER(B2VTensor), C.c_void_p, C.c_void_p]),
     ("b2v_get_recon", C.c_int, [C.c_void_p, C.c_void_p]),
     ("b2v_bench_csc", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     ("b2v_bench_csc_burst", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),

@@ -221,9 +221,16 @@ void free_geometry(Session* s) {
   if (s->jenc) { jpeg_destroy(s->jenc); s->jenc = nullptr; }
 }
 
-CscParams csc_params(Session* s, const uint8_t* d_src, int stride, int fmt, uint8_t* d_nv12) {
-  CscParams p{};
-  p.src = d_src; p.src_w = s->src_w; p.src_h = s->src_h; p.src_stride = stride; p.fmt = fmt;
+// a source of packed 8-bit pixels
+CscSource packed_src(const uint8_t* d_src, int stride, int fmt) {
+  CscSource p{};
+  p.src = d_src; p.src_stride = stride; p.fmt = fmt;
+  return p;
+}
+
+// `p` describes the source; the rest is the session's geometry
+CscSource csc_params(Session* s, CscSource p, uint8_t* d_nv12) {
+  p.src_w = s->src_w; p.src_h = s->src_h;
   p.dst_w = s->dst_w; p.dst_h = s->dst_h; p.coded_w = s->coded_w; p.coded_h = s->coded_h;
   p.out_y = d_nv12; p.out_uv = d_nv12 + (size_t)s->coded_w * s->coded_h;
   p.tx = s->d_tx; p.ty = s->d_ty;
@@ -392,9 +399,10 @@ int submit_failed(Session* s, int out_idx, int in_slot, cudaError_t e, const cha
 #define CKS(call)                                                                              \
   do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return submit_failed(s, out_idx, in_slot, e_, #call); } while (0)
 
-// common tail of b2v_ring_submit / b2v_submit_device / b2v_submit_resident: CSC + encode + D2H + job.  `producer` (device
-// frames of the caller) is the stream the CSC is ordered after, and that is ordered after the CSC in turn; null: no such stream.
-int submit_common(Session* s, const uint8_t* d_src, int stride, int fmt, int in_slot, const cudaStream_t* producer, int64_t capture_ns) {
+// common tail of b2v_ring_submit / b2v_submit_device / b2v_submit_tensor / b2v_submit_resident: CSC + encode + D2H + job.
+// `producer` (device frames of the caller) is the stream the CSC is ordered after, and that is ordered after the CSC in turn;
+// null: no such stream.
+int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStream_t* producer, int64_t capture_ns) {
   int out_idx = 0;
   Job j{};
   EncodeFrameParams fp{};
@@ -436,7 +444,7 @@ int submit_common(Session* s, const uint8_t* d_src, int stride, int fmt, int in_
     s->submitted++;
     s->stats.frames_submitted++;
   }
-  CscParams cp = csc_params(s, d_src, stride, fmt, s->d_cur);
+  CscSource cp = csc_params(s, src, s->d_cur);
   cudaEvent_t* ev = j.timing ? s->ev_t[out_idx] : nullptr;
   if (producer) {
     CKS(cudaEventRecord(s->ev_dev_in, *producer));
@@ -506,8 +514,8 @@ void release_session(Session* s) {
   delete s;
 }
 
-// Checks of b2v_submit_device on the caller's frame (include/b2video.h), before anything is enqueued: the arguments first, with
-// no CUDA call; then what the driver knows of the memory.  Caller holds submit_mu.
+// Checks of b2v_submit_device and b2v_submit_tensor on the caller's frame (include/b2video.h), before anything is enqueued: the
+// arguments first, with no CUDA call; then what the driver knows of the memory.  Caller holds submit_mu.
 typedef CUresult (*AddressRangeFn)(CUdeviceptr* base, size_t* size, CUdeviceptr p);
 AddressRangeFn address_range_fn() {
   static const AddressRangeFn fn = [] {         // the runtime's driver entry point: libb2video does not link libcuda itself
@@ -522,12 +530,8 @@ AddressRangeFn address_range_fn() {
   return fn;
 }
 
-int check_device_frame(Session* s, const uint8_t* frame, int pitch, int fmt) {
-  const int bpp = fmt < B2V_PIX_BGR ? 4 : 3;
-  const int64_t row = (int64_t)s->src_w * bpp;
-  if (pitch < row) return fail(B2V_EINVAL, "pitch %d is below one row of the frame (%d pixels x %d bytes)", pitch, s->src_w, bpp);
-  if (bpp == 4 && (((uintptr_t)frame & 3) || (pitch & 3)))
-    return fail(B2V_EINVAL, "4-byte pixels need a frame address and a pitch that are multiples of 4 (frame %p, pitch %d)", (const void*)frame, pitch);
+// The memory: `extent` bytes from `frame` on, the last one being the last byte the conversion reads.
+int check_device_memory(Session* s, const uint8_t* frame, unsigned long long extent) {
   CK(cudaSetDevice(s->device));
   cudaPointerAttributes a{};
   cudaError_t e = cudaPointerGetAttributes(&a, frame);
@@ -541,11 +545,72 @@ int check_device_frame(Session* s, const uint8_t* frame, int pitch, int fmt) {
   CUdeviceptr base = 0;
   size_t size = 0;
   if (range(&base, &size, (CUdeviceptr)(uintptr_t)frame) != CUDA_SUCCESS) return fail(B2V_EINVAL, "frame %p: no device allocation holds it", (const void*)frame);
-  const unsigned long long end = (unsigned long long)(uintptr_t)frame + (unsigned long long)pitch * (s->src_h - 1) + (unsigned long long)row;
+  const unsigned long long end = (unsigned long long)(uintptr_t)frame + extent;
   if (end > (unsigned long long)base + size)
-    return fail(B2V_EINVAL, "frame %p: %d rows at pitch %d end %llu bytes past the end of its allocation (%zu bytes at 0x%llx)", (const void*)frame,
-                s->src_h, pitch, end - ((unsigned long long)base + size), size, (unsigned long long)base);
+    return fail(B2V_EINVAL, "frame %p: its %dx%d picture ends %llu bytes past the end of its allocation (%zu bytes at 0x%llx)", (const void*)frame,
+                s->src_w, s->src_h, end - ((unsigned long long)base + size), size, (unsigned long long)base);
   return 0;
+}
+
+int check_device_frame(Session* s, const uint8_t* frame, int pitch, int fmt) {
+  const int bpp = fmt < B2V_PIX_BGR ? 4 : 3;
+  const int64_t row = (int64_t)s->src_w * bpp;
+  if (pitch < row) return fail(B2V_EINVAL, "pitch %d is below one row of the frame (%d pixels x %d bytes)", pitch, s->src_w, bpp);
+  if (bpp == 4 && (((uintptr_t)frame & 3) || (pitch & 3)))
+    return fail(B2V_EINVAL, "4-byte pixels need a frame address and a pitch that are multiples of 4 (frame %p, pitch %d)", (const void*)frame, pitch);
+  return check_device_memory(s, frame, (unsigned long long)pitch * (s->src_h - 1) + (unsigned long long)row);
+}
+
+constexpr int kElemBytes[4] = {1, 2, 2, 4};      // by B2V_DT_*
+
+// What of a b2v_tensor can be checked without the session or a CUDA call.
+int check_tensor_args(const b2v_tensor* t) {
+  if (!t) return fail(B2V_EINVAL, "null tensor description");
+  if (t->dtype < B2V_DT_U8 || t->dtype > B2V_DT_F32) return fail(B2V_EINVAL, "unknown dtype %d", t->dtype);
+  if (t->pixel_format < B2V_PIX_BGRA || t->pixel_format > B2V_PIX_RGB) return fail(B2V_EINVAL, "unknown pixel format %d", t->pixel_format);
+  const int elem = kElemBytes[t->dtype];
+  const int64_t strides[3] = {t->stride_c, t->stride_y, t->stride_x};
+  const char* const names[3] = {"stride_c", "stride_y", "stride_x"};
+  for (int i = 0; i < 3; i++) {
+    if (strides[i] <= 0 || strides[i] % elem != 0)
+      return fail(B2V_EINVAL, "%s %lld: strides are positive multiples of the element size (%d)", names[i], (long long)strides[i], elem);
+    if (strides[i] >= (i == 0 ? 1LL << 48 : 1LL << 31)) return fail(B2V_EINVAL, "%s %lld is too large", names[i], (long long)strides[i]);
+  }
+  if (!t->data) return fail(B2V_EINVAL, "null tensor data");
+  if ((uintptr_t)t->data % elem != 0) return fail(B2V_EINVAL, "tensor data %p is not aligned to its element size (%d)", t->data, elem);
+  return 0;
+}
+
+// The remaining checks of a tensor, and its description for the colour conversion.  A uint8 tensor whose channels are the
+// bytes of packed pixels is such a frame, and takes the kernels of b2v_submit_device.  Caller holds submit_mu.
+int tensor_source(Session* s, const b2v_tensor* t, CscSource* out) {
+  const int elem = kElemBytes[t->dtype], channels = t->pixel_format < B2V_PIX_BGR ? 4 : 3;
+  const uint8_t* data = (const uint8_t*)t->data;
+  int rc = check_device_memory(s, data, 2ULL * t->stride_c + (unsigned long long)t->stride_y * (s->src_h - 1) +
+                                            (unsigned long long)t->stride_x * (s->src_w - 1) + elem);
+  if (rc) return rc;
+  const bool packed = t->dtype == B2V_DT_U8 && t->stride_c == 1 && t->stride_x == channels && t->stride_y >= (int64_t)s->src_w * channels &&
+                      (channels == 3 || (((uintptr_t)data | (uintptr_t)t->stride_y) & 3) == 0);
+  *out = packed_src(data, (int)t->stride_y, t->pixel_format);
+  if (!packed) { out->dtype = t->dtype; out->stride_x = (int)t->stride_x; out->stride_c = t->stride_c; }
+  return 0;
+}
+
+// b2v_csc_nv12 / b2v_csc_nv12_tensor: the visible picture of `src` as host NV12, synchronously on st_enc.  Caller holds submit_mu.
+int cuda_rc(cudaError_t e) { return e == cudaSuccess ? 0 : fail(B2V_ECUDA, "%s", cudaGetErrorString(e)); }
+int csc_to_host(Session* s, const CscSource& src, void* nv12) {
+  uint8_t* d_out = nullptr;
+  const size_t out_bytes = (size_t)s->dst_w * s->dst_h * 3 / 2;
+  CK(cudaMalloc((void**)&d_out, out_bytes));
+  CscSource p = csc_params(s, src, d_out);
+  p.coded_w = s->dst_w; p.coded_h = s->dst_h;          // visible region only
+  p.out_uv = d_out + (size_t)s->dst_w * s->dst_h;
+  launch_csc(p, s->st_enc);
+  int rc = cuda_rc(cudaMemcpyAsync(nv12, d_out, out_bytes, cudaMemcpyDeviceToHost, s->st_enc));
+  if (!rc) rc = cuda_rc(cudaStreamSynchronize(s->st_enc));
+  cudaFree(d_out);
+  if (!rc) rc = cuda_rc(cudaGetLastError());
+  return rc;
 }
 
 // b2v_bench_csc (burst = false: each launch bracketed by its own event pair, the sum excludes host launch gaps) and
@@ -560,7 +625,7 @@ int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launc
   std::vector<uint8_t*> outs(n_resident, nullptr);
   size_t ob = (size_t)s->coded_w * s->coded_h * 3 / 2;
   for (auto& o : outs) CK(cudaMalloc((void**)&o, ob));
-  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, s->resident[i], s->src_w * 4, B2V_PIX_BGRA, outs[i]), s->st_enc);   // warm-up
+  for (int i = 0; i < n_resident; i++) launch_csc(csc_params(s, packed_src(s->resident[i], s->src_w * 4, B2V_PIX_BGRA), outs[i]), s->st_enc);   // warm-up
   CK(cudaStreamSynchronize(s->st_enc));
   const int pairs = burst ? 1 : iters;
   std::vector<cudaEvent_t> e0(pairs), e1(pairs);
@@ -569,7 +634,7 @@ int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launc
   for (int i = 0; i < iters; i++) {
     int k = i % n_resident;
     if (!burst) cudaEventRecord(e0[i], s->st_enc);
-    launch_csc(csc_params(s, s->resident[k], s->src_w * 4, B2V_PIX_BGRA, outs[k]), s->st_enc);
+    launch_csc(csc_params(s, packed_src(s->resident[k], s->src_w * 4, B2V_PIX_BGRA), outs[k]), s->st_enc);
     if (!burst) cudaEventRecord(e1[i], s->st_enc);
   }
   if (burst) cudaEventRecord(e1[0], s->st_enc);
@@ -711,7 +776,7 @@ int b2v_ring_submit(void* h, int32_t slot, int32_t stride, int64_t capture_ns) {
     s->stats.h2d_bytes += (int64_t)stride * s->src_h;
     s->stats.ns_submit += now_ns() - t0;
   }
-  return submit_common(s, s->dev_slot[slot], stride, B2V_PIX_BGRA, slot, nullptr, capture_ns);
+  return submit_common(s, packed_src(s->dev_slot[slot], stride, B2V_PIX_BGRA), slot, nullptr, capture_ns);
 }
 
 int b2v_resident_upload(void* h, int32_t index, const void* bgra, int32_t stride) {
@@ -731,7 +796,7 @@ int b2v_submit_resident(void* h, int32_t index, int64_t capture_ns) {
   if (!s || index < 0 || index >= (int)s->resident.size() || !s->resident[index]) return fail(B2V_EINVAL, "resident frame %d not uploaded", index);
   std::lock_guard<std::mutex> sub(s->submit_mu);
   CK(cudaSetDevice(s->device));
-  return submit_common(s, s->resident[index], s->src_w * 4, B2V_PIX_BGRA, -1, nullptr, capture_ns);
+  return submit_common(s, packed_src(s->resident[index], s->src_w * 4, B2V_PIX_BGRA), -1, nullptr, capture_ns);
 }
 
 int b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, void* cuda_stream, int64_t capture_ns) {
@@ -742,7 +807,20 @@ int b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t p
   int rc = check_device_frame(s, (const uint8_t*)frame, pitch_bytes, pixel_format);
   if (rc) return rc;
   const cudaStream_t producer = (cudaStream_t)cuda_stream;
-  return submit_common(s, (const uint8_t*)frame, pitch_bytes, pixel_format, -1, &producer, capture_ns);
+  return submit_common(s, packed_src((const uint8_t*)frame, pitch_bytes, pixel_format), -1, &producer, capture_ns);
+}
+
+int b2v_submit_tensor(void* h, const b2v_tensor* t, void* cuda_stream, int64_t capture_ns) {
+  Session* s = (Session*)h;
+  int rc = check_tensor_args(t);
+  if (rc) return rc;
+  if (!s) return fail(B2V_EINVAL, "null handle");
+  std::lock_guard<std::mutex> sub(s->submit_mu);         // the source size is stable from here on
+  CscSource src;
+  rc = tensor_source(s, t, &src);
+  if (rc) return rc;
+  const cudaStream_t producer = (cudaStream_t)cuda_stream;
+  return submit_common(s, src, -1, &producer, capture_ns);
 }
 
 int b2v_flush(void* h) {
@@ -854,20 +932,28 @@ int b2v_csc_nv12(void* h, const void* bgra, int32_t stride, void* nv12) {
   if (rc) return rc;
   std::lock_guard<std::mutex> sub(s->submit_mu);
   CK(cudaSetDevice(s->device));
-  uint8_t *d_in = nullptr, *d_out = nullptr;
-  size_t out_bytes = (size_t)s->dst_w * s->dst_h * 3 / 2;
+  uint8_t* d_in = nullptr;
   CK(cudaMalloc((void**)&d_in, (size_t)s->src_w * 4 * s->src_h));
-  CK(cudaMalloc((void**)&d_out, out_bytes));
-  CK(cudaMemcpy2DAsync(d_in, (size_t)s->src_w * 4, bgra, stride, (size_t)s->src_w * 4, s->src_h, cudaMemcpyHostToDevice, s->st_enc));
-  CscParams p = csc_params(s, d_in, s->src_w * 4, B2V_PIX_BGRA, d_out);
-  p.coded_w = s->dst_w; p.coded_h = s->dst_h;          // visible region only
-  p.out_uv = d_out + (size_t)s->dst_w * s->dst_h;
-  launch_csc(p, s->st_enc);
-  CK(cudaMemcpyAsync(nv12, d_out, out_bytes, cudaMemcpyDeviceToHost, s->st_enc));
-  CK(cudaStreamSynchronize(s->st_enc));
-  cudaFree(d_in); cudaFree(d_out);
-  CK(cudaGetLastError());
-  return 0;
+  rc = cuda_rc(cudaMemcpy2DAsync(d_in, (size_t)s->src_w * 4, bgra, stride, (size_t)s->src_w * 4, s->src_h, cudaMemcpyHostToDevice, s->st_enc));
+  if (!rc) rc = csc_to_host(s, packed_src(d_in, s->src_w * 4, B2V_PIX_BGRA), nv12);
+  cudaFree(d_in);
+  return rc;
+}
+
+int b2v_csc_nv12_tensor(void* h, const b2v_tensor* t, void* cuda_stream, void* nv12) {
+  Session* s = (Session*)h;
+  int rc = check_tensor_args(t);
+  if (rc) return rc;
+  if (!s || !nv12) return fail(B2V_EINVAL, "null argument");
+  rc = b2v_flush(h);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> sub(s->submit_mu);
+  CscSource src;
+  rc = tensor_source(s, t, &src);
+  if (rc) return rc;
+  CK(cudaEventRecord(s->ev_dev_in, (cudaStream_t)cuda_stream));
+  CK(cudaStreamWaitEvent(s->st_enc, s->ev_dev_in, 0));
+  return csc_to_host(s, src, nv12);          // synchronous: the tensor has been read when this returns
 }
 
 int b2v_get_recon(void* h, void* nv12) {

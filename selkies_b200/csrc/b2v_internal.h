@@ -58,8 +58,18 @@ struct CscParams {
                           // 4-byte orders
 };
 
+// CscParams plus where a source that is not packed 8-bit pixels keeps its samples (b2v_submit_tensor).  The 1:1 kernels of packed
+// pixels go on taking the CscParams part alone.
+struct CscSource : CscParams {
+  int dtype = B2V_DT_U8;     // B2V_DT_*: what one element is
+  int stride_x = 0;          // bytes between two columns
+  long long stride_c = 0;    // bytes between two channels; 0: packed 8-bit pixels, read as `fmt` says, and the two fields above are
+                             // unused.  Otherwise element (c, y, x) is at src + c * stride_c + y * src_stride + x * stride_x,
+                             // `fmt` tells only whether channel 0 is blue (even) or red (odd), and src is aligned to the element
+};
+
 // returns number of kernel launches issued (1)
-int launch_csc(const CscParams& p, cudaStream_t st);
+int launch_csc(const CscSource& p, cudaStream_t st);
 void make_taps_host(Tap* t, int dn, int sn);
 
 }  // namespace b2v

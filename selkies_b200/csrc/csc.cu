@@ -18,7 +18,15 @@
 //              16 B of CbCr.
 //   channel order: RGBA and RGB swap the coefficients of bytes 0 and 2 (at compile time in the 1:1 kernels, by matrix row in
 //              the others); the pixels are never reordered.
+//   planar 1:1 path (b2v_submit_tensor: three planes of uint8, fp16, bf16 or fp32 with contiguous rows): one thread = the
+//              pixels of one 16-byte load (16 / 8 / 8 / 4) x 2 rows: six 16-byte loads, one per plane and row, all issued before
+//              the first use; the elements are quantised in registers (DESIGN.md §3) and woven into the pixel words of the
+//              4-byte kernel.  4.5 / 7.5 / 7.5 / 13.5 B/px algorithmic.  Which plane is blue is decided on the host.
 //   general path (scaled or ragged widths): one thread per 2x2 output block, taps from tables.
+//   any other tensor (interleaved floats, strided columns, unaligned windows, scaled): the general and scaled kernels, whose
+//              per-pixel loader reads three strided elements and quantises them.
+#include <cuda_fp16.h>
+
 #include <mutex>
 
 #include "b2v_internal.h"
@@ -203,23 +211,96 @@ __global__ void __launch_bounds__(C3_WARPS * 32) csc_rgb24_nv12_fast(CscParams p
   }
 }
 
+// ---- planar 1:1 fast path (three planes of B2V_DT_* elements; rows contiguous; planes, row stride and outputs 16-byte aligned) ----
+// element -> 8-bit sample (DESIGN.md §3): rint_half_even(255 * min(max(x, 0), 1)), one fp32 multiplication; __saturatef(NaN) is 0
+__device__ __forceinline__ unsigned quant(float x) { return (unsigned)__float2int_rn(__saturatef(x) * 255.0f); }
+__device__ __forceinline__ unsigned quant_h2(unsigned two) {            // two fp16 -> samples in bytes 0 and 1
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&two));
+  return quant(f.x) | (quant(f.y) << 8);
+}
+__device__ __forceinline__ unsigned quant_b2(unsigned two) {            // two bf16: each is the high half of its fp32
+  return quant(__uint_as_float(two << 16)) | (quant(__uint_as_float(two & 0xffff0000u)) << 8);
+}
+__host__ __device__ constexpr int planar_px(int dt) { return dt == B2V_DT_U8 ? 16 : dt == B2V_DT_F32 ? 4 : 8; }   // elements of one 16-byte load
+// one 16-byte load -> its samples, four to a word
+template <int DT>
+__device__ __forceinline__ void quant16(const uint4& v, unsigned (&w)[planar_px(DT) / 4]) {
+  if constexpr (DT == B2V_DT_U8) { w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w; }
+  else if constexpr (DT == B2V_DT_F16) { w[0] = quant_h2(v.x) | (quant_h2(v.y) << 16); w[1] = quant_h2(v.z) | (quant_h2(v.w) << 16); }
+  else if constexpr (DT == B2V_DT_BF16) { w[0] = quant_b2(v.x) | (quant_b2(v.y) << 16); w[1] = quant_b2(v.z) | (quant_b2(v.w) << 16); }
+  else w[0] = quant(__uint_as_float(v.x)) | (quant(__uint_as_float(v.y)) << 8) | (quant(__uint_as_float(v.z)) << 16) | (quant(__uint_as_float(v.w)) << 24);
+}
+// four samples of each plane -> four pixel words (byte 0 = B, 1 = G, 2 = R; byte 3 is left over and weighs 0)
+__device__ __forceinline__ uint4 weave(unsigned b, unsigned g, unsigned r) {
+  const unsigned bg01 = __byte_perm(b, g, 0x5140), bg23 = __byte_perm(b, g, 0x7362);
+  return make_uint4(__byte_perm(bg01, r, 0x4410), __byte_perm(bg01, r, 0x5532), __byte_perm(bg23, r, 0x6610), __byte_perm(bg23, r, 0x7732));
+}
+template <int Q>
+__device__ __forceinline__ void st_words(uint8_t* p, const unsigned (&w)[Q]) {
+  if constexpr (Q == 4) st_stream4(p, w[0], w[1], w[2], w[3]);
+  else if constexpr (Q == 2) asm volatile("st.global.cs.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(w[0]), "r"(w[1]) : "memory");
+  else st_stream(p, w[0]);
+}
+// p.src is the blue plane, pg and pr the green and red ones.  grid.x covers the units (one 16-byte load wide) of a row, grid.y
+// strides over row pairs.
+template <int M, int DT>
+__global__ void __launch_bounds__(256) csc_planar_nv12_fast(CscParams p, const uint8_t* __restrict__ pg, const uint8_t* __restrict__ pr, int units, int pairs) {
+  constexpr int PX = planar_px(DT), Q = PX / 4;
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p.ts && threadIdx.x == 0) {
+    unsigned long long t0; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0)); atomicMin(p.ts, t0);
+  }
+  if (u < units)
+  for (int pair = blockIdx.y; pair < pairs; pair += gridDim.y) {
+    const int r0 = min(2 * pair, p.src_h - 1), r1 = min(2 * pair + 1, p.src_h - 1);   // bottom padding rows replicate
+    const size_t o0 = (size_t)r0 * p.src_stride + (size_t)u * 16, o1 = (size_t)r1 * p.src_stride + (size_t)u * 16;
+    const uint4 vb0 = ld_stream(p.src + o0), vg0 = ld_stream(pg + o0), vr0 = ld_stream(pr + o0);
+    const uint4 vb1 = ld_stream(p.src + o1), vg1 = ld_stream(pg + o1), vr1 = ld_stream(pr + o1);
+    unsigned b0[Q], g0[Q], c0[Q], b1[Q], g1[Q], c1[Q], y0[Q], y1[Q], uv[Q];
+    quant16<DT>(vb0, b0); quant16<DT>(vg0, g0); quant16<DT>(vr0, c0);
+    quant16<DT>(vb1, b1); quant16<DT>(vg1, g1); quant16<DT>(vr1, c1);
+#pragma unroll
+    for (int k = 0; k < Q; k++) convert_quad<M, false>(weave(b0[k], g0[k], c0[k]), weave(b1[k], g1[k], c1[k]), y0[k], y1[k], uv[k]);
+    st_words<Q>(p.out_y + (size_t)(2 * pair) * p.coded_w + u * PX, y0);
+    st_words<Q>(p.out_y + (size_t)(2 * pair + 1) * p.coded_w + u * PX, y1);
+    st_words<Q>(p.out_uv + (size_t)pair * p.coded_w + u * PX, uv);
+  }
+  if (p.ts) {
+    __syncthreads();
+    if (threadIdx.x == 0) { unsigned long long t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); atomicMax(p.ts + 1, t1); }
+  }
+}
+
 // ---- general path: bilinear scale and/or ragged width, one thread per 2x2 output block -----
-// pixel word of pixel x of a row: bytes 0..2 are its colour bytes in memory order (3-byte formats: any alignment)
-__device__ __forceinline__ unsigned load_px(const uint8_t* row, int x, int fmt) {
-  if (fmt < B2V_PIX_BGR) return *(const unsigned*)(row + x * 4);
-  const uint8_t* q = row + x * 3;
-  return (unsigned)q[0] | ((unsigned)q[1] << 8) | ((unsigned)q[2] << 16);
+__device__ __forceinline__ unsigned load_elem(const uint8_t* e, int dtype) {
+  switch (dtype) {
+    case B2V_DT_U8: return *e;
+    case B2V_DT_F16: return quant(__half2float(*reinterpret_cast<const __half*>(e)));
+    case B2V_DT_BF16: return quant(__uint_as_float((unsigned)*reinterpret_cast<const uint16_t*>(e) << 16));
+    default: return quant(*reinterpret_cast<const float*>(e));
+  }
+}
+// pixel word of pixel x of a row: bytes 0..2 are its colour bytes in memory order (3-byte formats: any alignment), or the
+// quantised elements of channels 0..2 of a tensor, wherever its strides put them
+__device__ __forceinline__ unsigned load_px(const uint8_t* row, int x, const CscSource& p) {
+  if (p.stride_c == 0) {
+    if (p.fmt < B2V_PIX_BGR) return *(const unsigned*)(row + x * 4);
+    const uint8_t* q = row + x * 3;
+    return (unsigned)q[0] | ((unsigned)q[1] << 8) | ((unsigned)q[2] << 16);
+  }
+  const uint8_t* e = row + (size_t)x * p.stride_x;
+  return load_elem(e, p.dtype) | (load_elem(e + p.stride_c, p.dtype) << 8) | (load_elem(e + 2 * p.stride_c, p.dtype) << 16);
 }
 // B = byte 0, R = byte 2 of the pixel word: swapped for RGBA / RGB, which the matrix row c_mx[2 * matrix + 1] accounts for
-__device__ __forceinline__ void fetch_bgr(const CscParams& p, int x, int y, int& B, int& G, int& R) {
+__device__ __forceinline__ void fetch_bgr(const CscSource& p, int x, int y, int& B, int& G, int& R) {
   int x0, x1, fx, y0, y1, fy;
   if (p.tx) { Tap t = p.tx[x]; x0 = t.i0; x1 = t.i1; fx = t.f; } else { x0 = x1 = x; fx = 0; }
   if (p.ty) { Tap t = p.ty[y]; y0 = t.i0; y1 = t.i1; fy = t.f; } else { y0 = y1 = y; fy = 0; }
   const uint8_t* r0 = p.src + (size_t)y0 * p.src_stride;
   const uint8_t* r1 = p.src + (size_t)y1 * p.src_stride;
-  unsigned p00 = load_px(r0, x0, p.fmt);
+  unsigned p00 = load_px(r0, x0, p);
   if (fx == 0 && fy == 0) { B = p00 & 255; G = (p00 >> 8) & 255; R = (p00 >> 16) & 255; return; }
-  unsigned p01 = load_px(r0, x1, p.fmt), p10 = load_px(r1, x0, p.fmt), p11 = load_px(r1, x1, p.fmt);
+  unsigned p01 = load_px(r0, x1, p), p10 = load_px(r1, x0, p), p11 = load_px(r1, x1, p);
   int out[3];
 #pragma unroll
   for (int c = 0; c < 3; c++) {
@@ -231,7 +312,7 @@ __device__ __forceinline__ void fetch_bgr(const CscParams& p, int x, int y, int&
   B = out[0]; G = out[1]; R = out[2];
 }
 
-__global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscParams p) {
+__global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscSource p) {
   int bx = blockIdx.x * blockDim.x + threadIdx.x;   // 2x2 block column
   int by = blockIdx.y * blockDim.y + threadIdx.y;
   if (bx * 2 >= p.coded_w || by * 2 >= p.coded_h) return;
@@ -259,7 +340,8 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscParams p) {
 // staged in shared memory with 16-byte loads; every tap is then a shared-memory read.  The arithmetic is the spec's (oracle/
 // csc_ref.c fetch_bgr): per channel top/bottom horizontal blends at full precision (B and R ride in the two 16-bit halves of one
 // word: 255*256 fits), one vertical blend, one rounding.  Roofline: 4 B per source pixel read + 1.5 B per output pixel written.
-// Packed 3-byte sources are staged as the same pixel words (any alignment), so everything after the staging is shared.
+// Packed 3-byte sources and tensors are staged as the same pixel words (any alignment, quantised once), so everything after the
+// staging is shared.
 constexpr int SC_TW = 64, SC_TH = 8, SC_THREADS = (SC_TW / 2) * (SC_TH / 2);
 
 __device__ __forceinline__ void blend_px(const uint32_t* r0, const uint32_t* r1, int x0, int x1, int fx, int fy, int& B, int& G, int& R) {
@@ -274,7 +356,7 @@ __device__ __forceinline__ void blend_px(const uint32_t* r0, const uint32_t* r1,
   G = (int)((tg * wy0 + bg * wy1 + (1u << 15)) >> 16);
 }
 
-__global__ void __launch_bounds__(SC_THREADS) csc_bgra_nv12_scaled(CscParams p, int fw_cap, int fh_cap) {
+__global__ void __launch_bounds__(SC_THREADS) csc_bgra_nv12_scaled(CscSource p, int fw_cap, int fh_cap) {
   extern __shared__ __align__(16) uint32_t sc_tile[];            // fh_cap rows of fw_cap pixels (fw_cap % 4 == 0)
   const int tid = threadIdx.x;
   const int ox0 = blockIdx.x * SC_TW, oy0 = blockIdx.y * SC_TH;
@@ -287,12 +369,12 @@ __global__ void __launch_bounds__(SC_THREADS) csc_bgra_nv12_scaled(CscParams p, 
     const int r = i / fw4, c = i - r * fw4, sx = xs0 + 4 * c;
     const uint8_t* row = p.src + (size_t)(ys0 + r) * p.src_stride;
     uint4 v;
-    if (sx + 3 < p.src_w && p.fmt < B2V_PIX_BGR) v = ld_stream(row + (size_t)sx * 4);
-    else {                          // packed 3-byte pixels, or the last quad of a row whose width is not a multiple of 4
-      v.x = load_px(row, sx, p.fmt);
-      v.y = sx + 1 < p.src_w ? load_px(row, sx + 1, p.fmt) : 0u;
-      v.z = sx + 2 < p.src_w ? load_px(row, sx + 2, p.fmt) : 0u;
-      v.w = sx + 3 < p.src_w ? load_px(row, sx + 3, p.fmt) : 0u;
+    if (sx + 3 < p.src_w && p.stride_c == 0 && p.fmt < B2V_PIX_BGR) v = ld_stream(row + (size_t)sx * 4);
+    else {                          // packed 3-byte pixels, a tensor's elements, or the last quad of a row whose width is not a multiple of 4
+      v.x = load_px(row, sx, p);
+      v.y = sx + 1 < p.src_w ? load_px(row, sx + 1, p) : 0u;
+      v.z = sx + 2 < p.src_w ? load_px(row, sx + 2, p) : 0u;
+      v.w = sx + 3 < p.src_w ? load_px(row, sx + 3, p) : 0u;
     }
     *reinterpret_cast<uint4*>(&sc_tile[r * fw_cap + 4 * c]) = v;
   }
@@ -347,13 +429,39 @@ static void opt_in_smem(const void* fn, int* granted, int smem) {
   if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess && dev >= 0 && dev < kAttrDevices) granted[dev] = smem;
 }
 
-int launch_csc(const CscParams& p, cudaStream_t st) {
-  const bool swap = (p.fmt & 1) != 0, packed3 = p.fmt >= B2V_PIX_BGR;
+template <int M>
+static void launch_planar(const CscSource& p, const uint8_t* pg, const uint8_t* pr, dim3 grid, int block, int units, int pairs, cudaStream_t st) {
+  switch (p.dtype) {
+    case B2V_DT_U8: csc_planar_nv12_fast<M, B2V_DT_U8><<<grid, block, 0, st>>>(p, pg, pr, units, pairs); break;
+    case B2V_DT_F16: csc_planar_nv12_fast<M, B2V_DT_F16><<<grid, block, 0, st>>>(p, pg, pr, units, pairs); break;
+    case B2V_DT_BF16: csc_planar_nv12_fast<M, B2V_DT_BF16><<<grid, block, 0, st>>>(p, pg, pr, units, pairs); break;
+    default: csc_planar_nv12_fast<M, B2V_DT_F32><<<grid, block, 0, st>>>(p, pg, pr, units, pairs); break;
+  }
+}
+
+int launch_csc(const CscSource& p, cudaStream_t st) {
+  const bool tensor = p.stride_c != 0, swap = (p.fmt & 1) != 0, packed3 = p.fmt >= B2V_PIX_BGR;
   const bool one_to_one = p.tx == nullptr && p.ty == nullptr && p.dst_w == p.src_w && p.dst_h == p.src_h && p.coded_w == p.dst_w;
   const bool aligned16 = (p.src_stride % 16) == 0 && ((uintptr_t)p.src % 16) == 0;
-  const bool fast = one_to_one && !packed3 && (p.coded_w % 4) == 0 && aligned16 && ((uintptr_t)p.out_y % 4) == 0 && ((uintptr_t)p.out_uv % 4) == 0;
-  const bool fast3 = one_to_one && packed3 && (p.coded_w % 16) == 0 && aligned16 && ((uintptr_t)p.out_y % 16) == 0 && ((uintptr_t)p.out_uv % 16) == 0;
-  if (fast) {
+  const bool fast = !tensor && one_to_one && !packed3 && (p.coded_w % 4) == 0 && aligned16 && ((uintptr_t)p.out_y % 4) == 0 && ((uintptr_t)p.out_uv % 4) == 0;
+  const bool fast3 = !tensor && one_to_one && packed3 && (p.coded_w % 16) == 0 && aligned16 && ((uintptr_t)p.out_y % 16) == 0 && ((uintptr_t)p.out_uv % 16) == 0;
+  const int ppx = planar_px(p.dtype), elem = 16 / ppx;       // pixels per 16-byte load of a plane, bytes per element
+  const bool planar = tensor && one_to_one && p.stride_x == elem && aligned16 && (p.stride_c % 16) == 0 && (p.coded_w % ppx) == 0 &&
+                      ((uintptr_t)p.out_y % ppx) == 0 && ((uintptr_t)p.out_uv % ppx) == 0;
+  if (planar) {
+    const int units = p.coded_w / ppx, pairs = p.coded_h / 2;
+    int block = 256;                                           // the block that leaves the fewest idle threads in a row of units
+    for (int b = 224; b >= 64; b -= 32)
+      if ((units + b - 1) / b * b < (units + block - 1) / block * block) block = b;
+    const dim3 grid((units + block - 1) / block, pairs < 65535 ? pairs : 65535);
+    // channel order: which plane feeds which byte of the pixel word.  The kernel's p.src is the blue plane.
+    CscSource q = p;
+    q.src = p.src + (swap ? 2 * p.stride_c : 0);
+    const uint8_t* pg = p.src + p.stride_c;
+    const uint8_t* pr = p.src + (swap ? 0 : 2 * p.stride_c);
+    if (p.matrix == 1) launch_planar<1>(q, pg, pr, grid, block, units, pairs, st);
+    else launch_planar<0>(q, pg, pr, grid, block, units, pairs, st);
+  } else if (fast) {
     const int quads = p.coded_w / 4, pairs = p.coded_h / 2;
     int block = CSC_BLOCK;
     while (block > 64 && quads % block != 0) block -= 32;   // prefer a divisor of the row
@@ -382,8 +490,9 @@ int launch_csc(const CscParams& p, cudaStream_t st) {
     }
   } else {
     // scaled: the tiled kernel when the tile's source footprint fits shared memory (any sane scale factor), else the general one.
-    // 4-byte pixels are staged with 16-byte loads, so they need a 16-byte aligned source; 3-byte pixels are read bytewise.
-    if (p.tx && p.ty && (packed3 || aligned16)) {
+    // 4-byte pixels are staged with 16-byte loads, so they need a 16-byte aligned source; 3-byte pixels are read bytewise and a
+    // tensor element by element.
+    if (p.tx && p.ty && (tensor || packed3 || aligned16)) {
       const long long fw = ((long long)SC_TW * p.src_w + p.dst_w - 1) / p.dst_w + 8, fh = ((long long)SC_TH * p.src_h + p.dst_h - 1) / p.dst_h + 3;
       const int fw_cap = (int)((fw + 3) & ~3LL), fh_cap = (int)fh;
       const long long smem = (long long)fw_cap * fh_cap * 4;

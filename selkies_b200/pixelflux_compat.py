@@ -132,6 +132,18 @@ class DeviceFrameSource:
         raise NotImplementedError
 
 
+class TensorFrameSource(DeviceFrameSource):
+    """Producer of device tensors as a model leaves them.  `frame(index)` returns a 3-D device array covering the whole
+    surface: uint8, or fp16 / bf16 / fp32 in [0, 1]; `layout` names its axes ("CHW" or "HWC"; the strides are the array's own),
+    `channels` their number and order ("RGB", "BGR", "RGBA", "BGRA"), `dtype` the element type where the array cannot ("bf16"
+    for arrays that are not torch tensors).  Encoded in place by Session.submit_tensor; window and stream rules as for
+    DeviceFrameSource."""
+
+    channels = "RGB"
+    layout = "CHW"
+    dtype = None
+
+
 class SyntheticDesktopSource(FrameSource):
     """Flat regions, text-like 1-px patterns and a region scrolling 8 px/frame (SURVEY.md §8d S3)."""
 
@@ -358,9 +370,14 @@ class ScreenCapture:
             f = self._source.frame(index)
             if f is None:
                 return False
+            src = self._source
             try:
-                session.submit_device(f, pixel_format=self._source.pixel_format, stream=self._source.stream, origin=self._origin,
-                                      capture_ns=time.monotonic_ns())
+                if isinstance(src, TensorFrameSource):
+                    session.submit_tensor(f, channels=src.channels, layout=src.layout, dtype=src.dtype, stream=src.stream,
+                                          origin=self._origin, capture_ns=time.monotonic_ns())
+                else:
+                    session.submit_device(f, pixel_format=src.pixel_format, stream=src.stream, origin=self._origin,
+                                          capture_ns=time.monotonic_ns())
             except N.B2VError as e:
                 if e.code == N.B2V_EINVAL:        # the source handed over something the library cannot read: say so
                     raise

@@ -33,6 +33,41 @@ class EncodedFrame:
 PIXEL_FORMATS = {"BGRA": (N.B2V_PIX_BGRA, 4), "RGBA": (N.B2V_PIX_RGBA, 4), "BGR": (N.B2V_PIX_BGR, 3), "RGB": (N.B2V_PIX_RGB, 3)}
 
 
+def _array_interface(frame, device: int, entry: str):
+    """The `__cuda_array_interface__` of `frame`, and torch when `frame` is one of its tensors (else None).  The checks every
+    device entry shares: there is such an interface, a torch tensor is on the session's device, no mask."""
+    cai = getattr(frame, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError(f"{type(frame).__name__} has no __cuda_array_interface__: {entry} takes device arrays (host frames go "
+                        "through submit())")
+    torch = sys.modules.get("torch")                   # a torch tensor means torch is imported already; never import it here
+    if torch is not None and not isinstance(frame, torch.Tensor):
+        torch = None
+    if torch is not None and (frame.device.type != "cuda" or frame.device.index != device):
+        raise ValueError(f"frame is on {frame.device}, the session runs on cuda:{device}")
+    if cai.get("mask") is not None:
+        raise ValueError("masked arrays are not supported")
+    return cai, torch
+
+
+def _producer_stream(frame, cai, torch, stream) -> int:
+    """The producer's stream handle, by the rules in device_frame_args."""
+    if stream is not None:
+        return int(getattr(stream, "cuda_stream", stream))
+    if "stream" in cai:
+        return 0 if cai["stream"] is None else int(cai["stream"])
+    if torch is not None:
+        return torch.cuda.current_stream(frame.device).cuda_stream
+    return 0
+
+
+def _window(origin, width: int, height: int, full_w: int, full_h: int):
+    x, y = (int(v) for v in origin)
+    if x < 0 or y < 0 or x + width > full_w or y + height > full_h:
+        raise ValueError(f"window {width}x{height} at ({x}, {y}) lies outside the {full_w}x{full_h} frame")
+    return x, y
+
+
 def device_frame_args(frame, width: int, height: int, device: int, pixel_format: str = "BGRA", origin=(0, 0), stream=None):
     """Reads the `__cuda_array_interface__` of `frame` and returns the arguments of b2v_submit_device for its `width` x `height`
     window at `origin` = (x, y): (pointer, pitch in bytes, B2V_PIX_* code, producer stream handle).  The array must be uint8,
@@ -46,16 +81,7 @@ def device_frame_args(frame, width: int, height: int, device: int, pixel_format:
     if pixel_format not in PIXEL_FORMATS:
         raise ValueError(f"unknown pixel format {pixel_format!r} (one of {', '.join(PIXEL_FORMATS)})")
     fmt, bpp = PIXEL_FORMATS[pixel_format]
-    cai = getattr(frame, "__cuda_array_interface__", None)
-    if cai is None:
-        raise TypeError(f"{type(frame).__name__} has no __cuda_array_interface__: submit_device takes device arrays (host frames go "
-                        "through submit())")
-    torch = sys.modules.get("torch")                   # a torch tensor means torch is imported already; never import it here
-    is_torch = torch is not None and isinstance(frame, torch.Tensor)
-    if is_torch and (frame.device.type != "cuda" or frame.device.index != device):
-        raise ValueError(f"frame is on {frame.device}, the session runs on cuda:{device}")
-    if cai.get("mask") is not None:
-        raise ValueError("masked arrays are not supported")
+    cai, torch = _array_interface(frame, device, "submit_device")
     if str(cai["typestr"])[1:] != "u1":
         raise TypeError(f"frame dtype {cai['typestr']!r}: uint8 pixels are needed")
     shape = tuple(int(v) for v in cai["shape"])
@@ -67,19 +93,56 @@ def device_frame_args(frame, width: int, height: int, device: int, pixel_format:
         raise ValueError(f"frame strides {tuple(strides)}: pixels must be packed ({bpp}, 1); only the row stride is free")
     if pitch < shape[1] * bpp or pitch >= 1 << 31:
         raise ValueError(f"row stride {pitch} does not hold a row of {shape[1]} pixels")
-    x, y = (int(v) for v in origin)
-    if x < 0 or y < 0 or x + width > shape[1] or y + height > shape[0]:
-        raise ValueError(f"window {width}x{height} at ({x}, {y}) lies outside the {shape[1]}x{shape[0]} frame")
+    x, y = _window(origin, width, height, shape[1], shape[0])
     ptr = int(cai["data"][0]) + y * pitch + x * bpp
-    if stream is not None:
-        handle = int(getattr(stream, "cuda_stream", stream))
-    elif "stream" in cai:
-        handle = 0 if cai["stream"] is None else int(cai["stream"])
-    elif is_torch:
-        handle = torch.cuda.current_stream(frame.device).cuda_stream
+    return ptr, pitch, fmt, _producer_stream(frame, cai, torch, stream)
+
+
+# element types of tensors: name -> (B2V_DT_* code, bytes per element), and the typestr (without byte order) that names each
+DTYPES = {"u8": (N.B2V_DT_U8, 1), "f16": (N.B2V_DT_F16, 2), "bf16": (N.B2V_DT_BF16, 2), "f32": (N.B2V_DT_F32, 4)}
+_TYPESTR = {"u1": "u8", "f2": "f16", "f4": "f32"}
+
+
+def tensor_frame_args(frame, width: int, height: int, device: int, *, channels: str = "RGB", layout: str = "CHW", dtype=None,
+                      origin=(0, 0), stream=None):
+    """Reads the `__cuda_array_interface__` of a 3-D `frame` and returns (filled b2v_tensor, producer stream handle) for its
+    `width` x `height` window at `origin` = (x, y).  `channels` ("RGB", "BGR", "RGBA", "BGRA") says how many channels there are
+    and whether channel 0 is red or blue; `layout` ("CHW" or "HWC") only names the axes of the shape: the strides are the
+    array's own, so channels_last tensors, slices of a batch and other views need no flag.  Elements are uint8, or fp16 / bf16
+    / fp32 in [0, 1] (include/b2video.h has the rounding).  bf16 has no typestr: a 2-byte void element ('<V2', what torch
+    exports) is taken as bf16 when `frame` is a torch tensor of dtype bfloat16 or the caller says dtype="bf16".  `dtype`, when
+    given, must agree with the array otherwise.  Producer stream: as device_frame_args."""
+    if channels not in PIXEL_FORMATS:
+        raise ValueError(f"unknown channel order {channels!r} (one of {', '.join(PIXEL_FORMATS)})")
+    if layout not in ("CHW", "HWC"):
+        raise ValueError(f"unknown layout {layout!r} (CHW or HWC)")
+    if dtype is not None and dtype not in DTYPES:
+        raise ValueError(f"unknown dtype {dtype!r} (one of {', '.join(DTYPES)})")
+    fmt, nch = PIXEL_FORMATS[channels]
+    cai, torch = _array_interface(frame, device, "submit_tensor")
+    code = str(cai["typestr"])[1:]
+    if code == "V2" and (dtype == "bf16" or (torch is not None and frame.dtype == torch.bfloat16)):
+        name = "bf16"
+    elif code in _TYPESTR and str(cai["typestr"])[0] in "<|=":
+        name = _TYPESTR[code]
     else:
-        handle = 0
-    return ptr, pitch, fmt, handle
+        raise TypeError(f"frame dtype {cai['typestr']!r}: elements are uint8, float16, bfloat16 or float32")
+    if dtype is not None and dtype != name:
+        raise TypeError(f"frame dtype {cai['typestr']!r} is not the {dtype} the caller names")
+    dt, elem = DTYPES[name]
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) != 3:
+        raise ValueError(f"frame shape {shape}: a 3-D array is needed ({layout}); encode a batch one tensor at a time")
+    strides = cai.get("strides")
+    strides = (shape[1] * shape[2] * elem, shape[2] * elem, elem) if strides is None else tuple(int(v) for v in strides)
+    (c, sc), (h, sy), (w, sx) = (sorted(zip(layout, shape, strides))[i][1:] for i in range(3))      # "C" < "H" < "W"
+    if c != nch:
+        raise ValueError(f"frame shape {shape}: {channels} in {layout} needs {nch} channels, the array has {c}")
+    if min(sc, sy, sx) <= 0 or max(sy, sx) >= 1 << 31:
+        raise ValueError(f"frame strides {strides}: every stride must be positive (rows and columns below 2 GiB)")
+    x, y = _window(origin, width, height, w, h)
+    t = N.B2VTensor(int(cai["data"][0]) + y * sy + x * sx, dt, fmt, sc, sy, sx)
+    return t, _producer_stream(frame, cai, torch, stream)
 
 
 class Session:
@@ -161,6 +224,16 @@ class Session:
         ptr, pitch, fmt, handle = device_frame_args(frame, self.width, self.height, self.device, pixel_format, origin, stream)
         N.check(self._lib.b2v_submit_device(self._h, ptr, pitch, fmt, handle, capture_ns))
 
+    def submit_tensor(self, frame, *, channels: str = "RGB", layout: str = "CHW", dtype=None, stream=None, origin=(0, 0),
+                      capture_ns: int = 0) -> None:
+        """Encode the `width` x `height` window at `origin` of a 3-D tensor in device memory of the session's GPU as it is: uint8,
+        or fp16 / bf16 / fp32 in [0, 1], planar or interleaved, any strides (tensor_frame_args).  The colour conversion
+        quantises the elements as it reads them: no clamp / scale / cast / permute pass is needed in front.  Stream order as
+        submit_device."""
+        t, handle = tensor_frame_args(frame, self.width, self.height, self.device, channels=channels, layout=layout, dtype=dtype,
+                                      origin=origin, stream=stream)
+        N.check(self._lib.b2v_submit_tensor(self._h, C.byref(t), handle, capture_ns))
+
     def flush(self) -> None:
         N.check(self._lib.b2v_flush(self._h))
 
@@ -207,6 +280,14 @@ class Session:
         dw, dh = self.dst_width, self.dst_height
         out = np.empty(dw * dh * 3 // 2, np.uint8)
         N.check(self._lib.b2v_csc_nv12(self._h, bgra.ctypes.data, self.width * 4, out.ctypes.data))
+        return out[: dw * dh].reshape(dh, dw), out[dw * dh:].reshape(dh // 2, dw)
+
+    def csc_nv12_tensor(self, frame, **kw):
+        """csc_nv12 of a device tensor read in place; keywords as submit_tensor (without capture_ns)."""
+        t, handle = tensor_frame_args(frame, self.width, self.height, self.device, **kw)
+        dw, dh = self.dst_width, self.dst_height
+        out = np.empty(dw * dh * 3 // 2, np.uint8)
+        N.check(self._lib.b2v_csc_nv12_tensor(self._h, C.byref(t), handle, out.ctypes.data))
         return out[: dw * dh].reshape(dh, dw), out[dw * dh:].reshape(dh // 2, dw)
 
     def recon(self):
