@@ -29,7 +29,7 @@ def stripe_rows_of(h, stripe_rows):
 # 640x96 in one stripe: at quality 92 its FF bytes sit at the last byte of a thread's 16-byte chunk and past the first 4096-byte
 # round of the stuffing copy (test_escape_cases_oracle.py checks that it reaches both)
 @pytest.mark.parametrize("w,h,stripe_rows", [(64, 48, 0), (320, 192, 3), (130, 70, 2), (640, 362, 0), (1920, 1080, 0), (640, 96, 6)])
-@pytest.mark.parametrize("quality", [35, 60, 92])
+@pytest.mark.parametrize("quality", [1, 35, 60, 92, 100])
 def test_jpeg_stripes_bit_exact(w, h, stripe_rows, quality):
     f = synth.desktop(w, h, 1) if w >= 128 else synth.noise(w, h, 1)
     got = run(w, h, [f], quality, stripe_rows)

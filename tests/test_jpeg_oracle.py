@@ -61,3 +61,25 @@ def test_jfif_matrix_known_answers():
         f[..., :3] = bgr
         y, uv = oracle.csc_nv12(f, matrix=1)
         assert (int(y[0, 0]), int(uv[0, 0]), int(uv[0, 1])) == want
+
+
+def test_jfif_matrix_within_one_lsb_of_float64():
+    """Matrix 1 against a float64 evaluation of JFIF full-range BT.601 with 2x2 box chroma (the mean of the four pixels'
+    Cb / Cr): never more than 1 LSB off, and the correctly rounded value almost everywhere."""
+    f = synth.noise(256, 128, 3)
+    y, uv = oracle.csc_nv12(f, matrix=1)
+    b, g, r = [f[..., i].astype(np.float64) for i in range(3)]
+    fy = 0.299 * r + 0.587 * g + 0.114 * b
+    box = lambda a: (a[0::2, 0::2] + a[0::2, 1::2] + a[1::2, 0::2] + a[1::2, 1::2]) / 4
+    fcb, fcr = box(128 + (b - fy) / 1.772), box(128 + (r - fy) / 1.402)
+    for got, want in ((y, fy), (uv[:, 0::2], fcb), (uv[:, 1::2], fcr)):
+        assert np.abs(got - want).max() <= 1.0
+        assert (got != np.rint(want)).mean() < 0.01
+
+
+def test_jfif_matrix_keeps_every_grey():
+    """Y = v and Cb = Cr = 128 for every grey level: the identity on which the grey comparisons with libjpeg-turbo rest."""
+    f = np.zeros((2, 512, 4), np.uint8)
+    f[..., :3] = (np.arange(512) // 2).astype(np.uint8)[None, :, None]
+    y, uv = oracle.csc_nv12(f, matrix=1)
+    assert (y == f[..., 0]).all() and (uv == 128).all()
