@@ -96,12 +96,16 @@ enum {
   B2V_FLAG_TIMING        = 4,   /* bracket every kernel with CUDA events (b2v_get_stats)        */
   B2V_FLAG_DEVICE_TIMER  = 8,   /* with TIMING: the CSC kernel also stamps %globaltimer (ms_csc_device) */
   B2V_FLAG_TIMING_CSC    = 16,  /* a CUDA-event pair around the CSC launch of every 4th picture (ms_csc / n_csc)  */
-  B2V_FLAG_JPEG          = 32   /* CaptureSettings.output_mode = 0 (selkies.py:3209-3212): JPEG stripes instead of H.264.  The picture is cut
+  B2V_FLAG_JPEG          = 32,  /* CaptureSettings.output_mode = 0 (selkies.py:3209-3212): JPEG stripes instead of H.264.  The picture is cut
                                    into stripes of stripe_rows x 16 rows (0 = about eight stripes); each stripe that changed is delivered by its
                                    own callback as one baseline JFIF file (JFIF colour, 4:2:0), y_start/height set; with B2V_HDR_PIXELFLUX the
                                    file is preceded by frame_id u16be | y_start u16be (the reference adds 03 00 in front, selkies.py:3118).
                                    crf = jpeg_quality, paintover_crf = paint_over_jpeg_quality, paintover_trigger_frames as for H.264.
                                    A key-frame request re-sends every stripe. */
+  B2V_FLAG_QUALITY       = 64   /* measure every delivered record on the GPU (b2v_frame_quality): SSE per plane and luma SSIM of the
+                                   reconstruction against the picture the encoder coded.  H.264 only: b2v_create rejects it with
+                                   B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE (B2V_EINVAL), which have no reconstruction.  The access units
+                                   are the same bytes with and without it; it costs one kernel launch per picture (kernel_launches). */
 };
 
 /* One encoded frame, the native image of the pixelflux callback result
@@ -120,6 +124,27 @@ typedef struct b2v_frame {
 } b2v_frame;
 
 typedef void (*b2v_cb)(const b2v_frame* frame, void* user);
+
+/* B2V_FLAG_QUALITY: the measurement of one delivered record (the whole picture in full-frame mode, one band in striped mode).
+ * S is the NV12 picture the encoder coded (after colour conversion and scaling), R its reconstruction, which is what a decoder
+ * outputs.  Both are taken on the record's rows y_start .. y_start + height - 1 and columns 0 .. dst_w - 1; chroma on rows
+ * y_start / 2 .. and half the width.  Padding below or right of the visible picture is never counted.
+ *   sse_*: exact sums of (S - R)^2 per plane; samples_y = dst_w * height, samples_c = samples_y / 4.
+ *   PSNR of a plane = 10 log10(255^2 * samples / sse) (infinite when sse is 0).
+ *   ssim_y (luma): the mean over the 8x8 windows whose origins lie on a 4-sample grid anchored at (0, y_start) and that lie
+ *   wholly inside the record.  Per window, over its 64 samples: Sx = sum s, Sy = sum r, Q = sum (s^2 + r^2), P = sum s*r,
+ *   V = 64 Q - Sx^2 - Sy^2, C = 64 P - Sx Sy (exact integers), and in IEEE fp64 (the four factors converted, the two products
+ *   formed, then one division):
+ *     ssim = ((2 Sx Sy + 416) (2 C + 235963)) / ((Sx^2 + Sy^2 + 416) (V + 235963))
+ *   (416 = round(0.01^2 255^2 64), 235963 = round(0.03^2 255^2 64 63), as x264 --ssim).  ssim_windows counts the windows;
+ *   when it is 0 (a record with fewer than 8 rows or columns) ssim_y is NaN.  The mean is exact to within 2^-41: each window's
+ *   value is summed as round(ssim * 2^40) in int64, so the result does not depend on the order of summation. */
+typedef struct b2v_quality {
+  int64_t sse_y, sse_cb, sse_cr;
+  int64_t samples_y, samples_c;
+  double  ssim_y;
+  int64_t ssim_windows;
+} b2v_quality;
 
 /* Per-session counters; kernel times are CUDA-event milliseconds accumulated on
  * the launching stream (only when B2V_FLAG_TIMING is set). */
@@ -228,6 +253,12 @@ int  b2v_set_gop(void* h, int32_t frames);               /* b2v_settings.gop, li
                                                             SECONDS, settings.py:163, with the current fps) */
 int  b2v_set_resolution(void* h, int32_t src_w, int32_t src_h, int32_t dst_w, int32_t dst_h);
 int  b2v_request_idr(void* h);
+
+/* ---- quality of the record being delivered (B2V_FLAG_QUALITY) --------------
+ * Valid only inside this session's frame callback, on its output thread: fills *out with the measurement of the record the
+ * callback is delivering (the same lifetime rule as b2v_frame.data).  B2V_ESTATE outside a callback of this session or on a
+ * session created without B2V_FLAG_QUALITY; B2V_EINVAL for a null handle or out. */
+int  b2v_frame_quality(void* h, b2v_quality* out);
 
 /* ---- introspection / test hooks ------------------------------------------- */
 int  b2v_get_stats(void* h, b2v_stats* out);

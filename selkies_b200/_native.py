@@ -17,6 +17,7 @@ B2V_OK, B2V_EINVAL, B2V_ECUDA, B2V_ENOMEM, B2V_ESTATE, B2V_ETIMEOUT = 0, -1, -2,
 B2V_RC_CBR, B2V_RC_CQP = 0, 1
 B2V_HDR_NONE, B2V_HDR_PIXELFLUX = 0, 1
 B2V_FLAG_SPS_EVERY_IDR, B2V_FLAG_NO_ENCODE, B2V_FLAG_TIMING, B2V_FLAG_DEVICE_TIMER, B2V_FLAG_TIMING_CSC, B2V_FLAG_JPEG = 1, 2, 4, 8, 16, 32
+B2V_FLAG_QUALITY = 64
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
 B2V_DT_U8, B2V_DT_F16, B2V_DT_BF16, B2V_DT_F32 = 0, 1, 2, 3
 
@@ -66,6 +67,14 @@ class B2VTensor(C.Structure):
     ]
 
 
+class B2VQuality(C.Structure):
+    _fields_ = [
+        ("sse_y", C.c_int64), ("sse_cb", C.c_int64), ("sse_cr", C.c_int64),
+        ("samples_y", C.c_int64), ("samples_c", C.c_int64),
+        ("ssim_y", C.c_double), ("ssim_windows", C.c_int64),
+    ]
+
+
 FRAME_CB = C.CFUNCTYPE(None, C.POINTER(B2VFrame), C.c_void_p)
 
 # every symbol include/b2video.h declares: (name, restype, argtypes)
@@ -88,6 +97,7 @@ SYMBOLS = [
     ("b2v_set_gop", C.c_int, [C.c_void_p, C.c_int32]),
     ("b2v_set_resolution", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("b2v_request_idr", C.c_int, [C.c_void_p]),
+    ("b2v_frame_quality", C.c_int, [C.c_void_p, C.POINTER(B2VQuality)]),
     ("b2v_get_stats", C.c_int, [C.c_void_p, C.POINTER(B2VStats)]),
     ("b2v_reset_stats", C.c_int, [C.c_void_p]),
     ("b2v_coded_size", C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),

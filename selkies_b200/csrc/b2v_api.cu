@@ -37,6 +37,9 @@
 using namespace b2v;
 
 static thread_local char g_err[512] = "";
+// B2V_FLAG_QUALITY: the session whose frame callback runs on this thread, and the measurement of the record it delivers
+static thread_local const void* g_cb_session = nullptr;
+static thread_local const b2v_quality* g_cb_quality = nullptr;
 static int fail(int code, const char* fmt, ...) {
   va_list ap; va_start(ap, fmt); vsnprintf(g_err, sizeof g_err, fmt, ap); va_end(ap);
   return code;
@@ -93,7 +96,7 @@ struct Session {
   b2v_settings cfg{};
   int device = 0;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
-  bool encode = true, timing = false, timing_csc_only = false;
+  bool encode = true, timing = false, timing_csc_only = false, quality = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;
 
   // ingest ring
@@ -189,6 +192,7 @@ int alloc_geometry(Session* s) {
     ec.slice_rows = s->cfg.slice_rows;          // <= 0: the encoder's default rule
     ec.stripe_rows = s->cfg.stripe_rows > 0 ? s->cfg.stripe_rows : 0;
     ec.idr_slice_mbs = s->cfg.idr_slice_mbs;
+    ec.quality = s->quality;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
     s->lay = encoder_layout(s->enc);
@@ -304,10 +308,10 @@ void put_pixelflux_header(uint8_t* h, const Job& j, int y0, int bh) {
 }
 
 // Runs the callback once per band of job j's access unit (`size` bytes) that carries data, in picture order; a full frame is the
-// one band {off 0, size, coded} of height hdr_h.  The band table is copied into `tab` first: the header of band k is written
-// over the tail of band k-1 (already delivered) or the table slack (the AuHeader, already read, for a full frame).
-// Returns the bytes delivered, headers included.
-int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab, int64_t* ns_cb) {
+// one band {off 0, size, coded} of height hdr_h.  The band table (and the quality table) is copied into `tab` (`qtab`) first: the
+// header of band k is written over the tail of band k-1 (already delivered) or the table slack (the AuHeader or the quality table,
+// already read, for band 0).  Returns the bytes delivered, headers included.
+int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab, std::vector<QualityEntry>& qtab, int64_t* ns_cb) {
   uint8_t* base = s->h_out[j.out_idx];
   uint8_t* au = base + s->lay.data_off;
   const int qp = ((const AuHeader*)base)->qp;
@@ -318,6 +322,10 @@ int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab,
     tab.resize(s->lay.n_bands);
     memcpy(tab.data(), base + sizeof(AuHeader), sizeof(BandEntry) * s->lay.n_bands);
     rows = s->lay.band_rows * 16;
+  }
+  if (s->lay.quality_off) {
+    qtab.resize(tab.size());
+    memcpy(qtab.data(), base + s->lay.quality_off, sizeof(QualityEntry) * tab.size());
   }
   const bool hdr = s->cfg.header_mode == B2V_HDR_PIXELFLUX;
   int64_t bytes = 0;
@@ -340,7 +348,21 @@ int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab,
     f.frame_id = j.frame_id; f.is_key = j.is_key; f.qp = qp; f.pts90k = j.pts; f.capture_ns = j.capture_ns;
     f.y_start = y0; f.height = bh;
     bytes += f.size;
-    if (s->cb) { const int64_t tc = now_ns(); s->cb(&f, s->user); *ns_cb += now_ns() - tc; }
+    b2v_quality q{};
+    if (s->lay.quality_off) {
+      const QualityEntry& e = qtab[b];
+      q.sse_y = e.sse[0]; q.sse_cb = e.sse[1]; q.sse_cr = e.sse[2];
+      q.samples_y = (int64_t)j.hdr_w * bh; q.samples_c = q.samples_y / 4;
+      q.ssim_windows = e.windows;
+      q.ssim_y = e.windows ? (double)e.ssim_q40 / 1099511627776.0 / (double)e.windows : __builtin_nan("");
+    }
+    if (s->cb) {
+      const int64_t tc = now_ns();
+      g_cb_session = s; g_cb_quality = s->lay.quality_off ? &q : nullptr;
+      s->cb(&f, s->user);
+      g_cb_session = nullptr; g_cb_quality = nullptr;
+      *ns_cb += now_ns() - tc;
+    }
   }
   return bytes;
 }
@@ -348,7 +370,8 @@ int64_t deliver(Session* s, const Job& j, int size, std::vector<BandEntry>& tab,
 void output_loop(Session* s) {
   cudaSetDevice(s->device);
   prctl(PR_SET_TIMERSLACK, 1000UL, 0, 0, 0);     // this thread's short sleeps (wait_event_polling) are not rounded up by 50 us
-  std::vector<BandEntry> tab;                    // deliver()'s copy of the band table, kept across pictures
+  std::vector<BandEntry> tab;                    // deliver()'s copies of the band and quality tables, kept across pictures
+  std::vector<QualityEntry> qtab;
   for (;;) {
     Job j;
     {
@@ -364,7 +387,7 @@ void output_loop(Session* s) {
     int64_t ns_event = 0, ns_cb = 0, bytes = 0; bool slept = false;
     const int size = wait_au(s, j, &ns_event, &slept);
     if (j.timing) add_timing(s, j, size > 0);
-    if (size > 0) bytes = deliver(s, j, size, tab, &ns_cb);
+    if (size > 0) bytes = deliver(s, j, size, tab, qtab, &ns_cb);
     {
       std::lock_guard<std::mutex> lk(s->mu);
       if (j.in_slot >= 0) s->slot_state[j.in_slot] = SLOT_FREE;
@@ -667,6 +690,9 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if (!size_ok(sw, sh)) return fail(B2V_EINVAL, "source size %dx%d unsupported (even, 16..7680 x 16..4320)", sw, sh);
   if (!size_ok(dw, dh)) return fail(B2V_EINVAL, "encoded size %dx%d unsupported", dw, dh);
   if (cfg->idr_slice_mbs < 0) return fail(B2V_EINVAL, "idr_slice_mbs %d out of range (0 = default, n > 0 macroblocks per slice)", cfg->idr_slice_mbs);
+  if ((cfg->flags & B2V_FLAG_QUALITY) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
+    return fail(B2V_EINVAL, "B2V_FLAG_QUALITY measures the H.264 reconstruction: %s has none",
+                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(B2V_EINVAL, "device %d out of range (%d devices)", cfg->device, ndev);
@@ -676,6 +702,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->src_w = sw; s->src_h = sh; s->dst_w = dw; s->dst_h = dh;
   s->encode = !(cfg->flags & B2V_FLAG_NO_ENCODE);
   s->jpeg = (cfg->flags & B2V_FLAG_JPEG) != 0;
+  s->quality = (cfg->flags & B2V_FLAG_QUALITY) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;
@@ -900,6 +927,14 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   s->resizing = false;
   s->cv_slot.notify_all();
   return rc;
+}
+
+int b2v_frame_quality(void* h, b2v_quality* out) {
+  if (!h || !out) return fail(B2V_EINVAL, "null argument");
+  if (g_cb_session != h) return fail(B2V_ESTATE, "b2v_frame_quality is valid only inside this session's frame callback");
+  if (!g_cb_quality) return fail(B2V_ESTATE, "the session was created without B2V_FLAG_QUALITY");
+  *out = *g_cb_quality;
+  return 0;
 }
 
 int b2v_get_stats(void* h, b2v_stats* out) {

@@ -27,13 +27,37 @@ static_assert(sizeof(AuHeader) == 64, "AuHeader must be 64 bytes");
 // banded output (striped H.264, JPEG stripes): one record per band right after the AuHeader (offsets relative to the first data byte)
 struct BandEntry { int32_t off, size, coded, frame_num; };
 
+// B2V_FLAG_QUALITY: one record per band (one for a full frame) in front of the first data byte, written by k_quality (quality.cu)
+struct QualityEntry {
+  long long sse[3];        // exact sums of (S - R)^2: Y, Cb, Cr
+  long long ssim_q40;      // sum over the band's SSIM windows of round(ssim * 2^40)
+  long long windows;       // SSIM windows counted
+};
+static_assert(sizeof(QualityEntry) == 40, "QualityEntry must be 40 bytes");
+
 // shape of an encoder's access-unit buffers
 struct AuLayout {
   size_t cap;              // bytes of one buffer
-  int data_off;            // bytes in front of the first data byte: AuHeader [+ band table] (+ slack for an in-place stripe header)
+  int data_off;            // bytes in front of the first data byte: AuHeader [+ band table] [+ quality table] (+ slack for an in-place
+                           // stripe header)
   int n_bands;             // band table entries; 0 = full frame, no band table
   int band_rows;           // macroblock rows (16 luma rows) per band; 0 when n_bands == 0
+  int quality_off = 0;     // bytes from the AuHeader to the QualityEntry table (max(n_bands, 1) entries); 0 = no table
 };
+
+// k_quality: the measurement of one picture (DESIGN.md §5.11).  S = the coded picture, R = its reconstruction, both NV12 at
+// coded_w x coded_h; records of band_px luma rows (the last one cut at dst_h), columns 0 .. dst_w - 1.
+struct QualityParams {
+  const uint8_t* src;      // S
+  const uint8_t* recon;    // R
+  int coded_w, coded_h, dst_w, dst_h;
+  int band_px, n_bands;
+  QualityEntry* out;       // n_bands records in the access-unit buffer
+  QualityEntry* acc;       // n_bands zeroed accumulators; k_quality leaves them zeroed
+  unsigned int* done;      // zeroed block counter; k_quality leaves it zeroed
+};
+// returns number of kernel launches issued (1)
+int launch_quality(const QualityParams& q, cudaStream_t st);
 
 // ---- colour conversion spec (DESIGN.md §3; BT.709 limited range, 14-bit coefficients) ----
 constexpr int KYR = 2991, KYG = 10064, KYB = 1016;

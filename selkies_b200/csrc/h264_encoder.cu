@@ -49,6 +49,8 @@ struct Encoder {
   uint8_t* param_sets = nullptr; int param_len = 0, param_len_last = 0;
   int band_rows = 0, n_bands = 1, striped = 0, au_data_off = (int)sizeof(AuHeader);
   int *band_fn = nullptr, *band_coded = nullptr;
+  int quality_off = 0;                                    // B2V_FLAG_QUALITY: the QualityEntry table in the access unit (0 = none)
+  QualityEntry* q_acc = nullptr; unsigned int* q_done = nullptr;   // k_quality's accumulators (zero between launches)
   cudaEvent_t ev_analysed[2] = {nullptr, nullptr}, ev_packed[2] = {nullptr, nullptr};   // two-stream schedule, by picture parity
   long long pic = 0;       // pictures encoded so far
   size_t au_cap = 0;
@@ -231,6 +233,14 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     ps.insert(ps.end(), last.begin(), last.end());
     e->au_data_off = (int)sizeof(AuHeader) + ((e->n_bands * (int)sizeof(BandEntry) + 16 + 63) & ~63);
   }
+  if (cfg->quality) {     // the quality table sits between the band table (if any) and the first data byte
+    e->quality_off = e->au_data_off;
+    e->au_data_off += (e->n_bands * (int)sizeof(QualityEntry) + 63) & ~63;
+    ECK(cudaMalloc((void**)&e->q_acc, e->n_bands * sizeof(QualityEntry)));
+    ECK(cudaMemset(e->q_acc, 0, e->n_bands * sizeof(QualityEntry)));
+    ECK(cudaMalloc((void**)&e->q_done, sizeof(unsigned int)));
+    ECK(cudaMemset(e->q_done, 0, sizeof(unsigned int)));
+  }
   ECK(cudaMalloc((void**)&e->param_sets, ps.size()));
   ECK(cudaMemcpy(e->param_sets, ps.data(), ps.size(), cudaMemcpyHostToDevice));
   ECK(cudaMalloc((void**)&e->band_fn, e->n_bands * sizeof(int)));
@@ -250,7 +260,8 @@ void encoder_destroy(Encoder* e) {
   if (!e) return;
   void* ptrs[] = {e->recon[0], e->recon[1], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
-                  e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done};
+                  e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
+                  e->q_acc, e->q_done};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -260,7 +271,7 @@ void encoder_destroy(Encoder* e) {
 }
 
 AuLayout encoder_layout(const Encoder* e) {
-  return {e->au_cap, e->au_data_off, e->striped ? e->n_bands : 0, e->striped ? e->band_rows : 0};
+  return {e->au_cap, e->au_data_off, e->striped ? e->n_bands : 0, e->striped ? e->band_rows : 0, e->quality_off};
 }
 const uint8_t* encoder_recon(const Encoder* e) { return e->recon[e->cur]; }
 
@@ -294,9 +305,19 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   //    of picture k-1 — possibly still running — never touches;
   //  * the analysis of picture k waits for the pack of picture k-2: that releases this parity's side data, the reconstruction
   //    buffer it is about to overwrite (the pack's copy kernel reads I_PCM samples from it) and the record of k-2.
+  // k_quality runs right behind the analysis, on `st`: the only moment both of its inputs are complete and intact (the next
+  // picture's colour conversion on `st` overwrites `cur`, the analysis of picture k+2 this reconstruction).
   const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
   if (overlap) cudaStreamWaitEvent(st, e->ev_packed[par], 0);           // pack of picture k-2 (no-op before the first two)
   n += idr ? launch_intra(f, st) : launch_inter(f, st);
+  if (e->quality_off) {
+    QualityParams q{};
+    q.src = p->cur; q.recon = f.recon;
+    q.coded_w = e->cfg.coded_w; q.coded_h = e->cfg.coded_h; q.dst_w = e->cfg.width; q.dst_h = e->cfg.height;
+    q.band_px = e->band_rows * 16; q.n_bands = e->n_bands;
+    q.out = reinterpret_cast<QualityEntry*>(p->au + e->quality_off); q.acc = e->q_acc; q.done = e->q_done;
+    n += launch_quality(q, st);
+  }
   if (p->ev) cudaEventRecord(p->ev[2], st);
   cudaStream_t sp = st;
   if (overlap) {

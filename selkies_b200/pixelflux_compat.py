@@ -75,6 +75,7 @@ class CaptureSettings:
         self.h264_stripe_rows = 0                # striped mode (h264_fullframe False): macroblock rows per stripe; 0 = about 8 stripes
         self.output_width = 0                    # != capture size => fused bilinear scale
         self.output_height = 0
+        self.quality_metrics = False             # measure every delivered record on the GPU: results carry `quality` (H.264 only)
 
 
 class StripeCallback:
@@ -90,7 +91,7 @@ class StripeCallback:
 
 
 class _Result:
-    __slots__ = ("data", "size", "frame_id", "is_key", "qp", "pts90k")
+    __slots__ = ("data", "size", "frame_id", "is_key", "qp", "pts90k", "quality")
 
 
 class _ResultPtr:
@@ -251,6 +252,7 @@ class ScreenCapture:
             s.header_mode = N.B2V_HDR_PIXELFLUX       # callers strip / keep the 10-byte header themselves
             s.ring_slots = 4
             s.flags = 0
+            s.quality = bool(getattr(settings, "quality_metrics", False))      # b2v_create refuses it in JPEG mode
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)
@@ -403,6 +405,7 @@ class ScreenCapture:
         r.is_key = f.is_key
         r.qp = f.qp
         r.pts90k = f.pts90k
+        r.quality = self._session.frame_quality()      # a FrameQuality, or None without quality_metrics
         self.frames_emitted += 1
         try:
             self._user_cb(_ResultPtr(r), None)

@@ -7,19 +7,35 @@ pixelflux_compat.ScreenCapture, bench.py and the tests.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import sys
 import threading
-from typing import Callable, Optional
+from typing import Callable, NamedTuple, Optional
 
 import numpy as np
 
 from . import _native as N
 
 
-class EncodedFrame:
-    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height")
+class FrameQuality(NamedTuple):
+    """The GPU's measurement of one delivered record against the picture the encoder coded (include/b2video.h, b2v_quality)."""
+    sse: tuple              # (y, cb, cr): exact sums of squared differences
+    samples: tuple          # (y, c): samples per luma plane, per chroma plane
+    psnr: tuple             # (y, cb, cr) in dB: 10 log10(255^2 samples / sse), inf when sse is 0
+    ssim: Optional[float]   # luma SSIM (mean over 8x8 windows on a 4-sample grid); None when the record holds no window
 
-    def __init__(self, data: bytes, frame_id: int, is_key: bool, qp: int, pts90k: int, capture_ns: int, y_start: int = 0, height: int = 0):
+    @classmethod
+    def from_native(cls, q: "N.B2VQuality") -> "FrameQuality":
+        sse, samples = (q.sse_y, q.sse_cb, q.sse_cr), (q.samples_y, q.samples_c)
+        psnr = tuple(10.0 * math.log10(255.0 ** 2 * n / e) if e else math.inf for e, n in zip(sse, (samples[0], samples[1], samples[1])))
+        return cls(sse, samples, psnr, q.ssim_y if q.ssim_windows else None)
+
+
+class EncodedFrame:
+    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height", "quality")
+
+    def __init__(self, data: bytes, frame_id: int, is_key: bool, qp: int, pts90k: int, capture_ns: int, y_start: int = 0, height: int = 0,
+                 quality: Optional[FrameQuality] = None):
         self.data = data
         self.frame_id = frame_id
         self.is_key = is_key
@@ -27,6 +43,7 @@ class EncodedFrame:
         self.pts90k = pts90k
         self.capture_ns = capture_ns
         self.y_start, self.height = y_start, height
+        self.quality = quality          # None unless the session measures quality (Session(quality=True))
 
 
 # pixel formats of device frames: name -> (B2V_PIX_* code, bytes per pixel); the name is the byte order in memory
@@ -150,8 +167,11 @@ class Session:
                  device: int = 0, rc_mode: int = N.B2V_RC_CBR, bitrate_kbps: int = 8000, crf: int = 26,
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
-                 collect: bool = True):
+                 collect: bool = True, quality: bool = False):
         self._lib = N.lib()
+        if quality:
+            flags |= N.B2V_FLAG_QUALITY
+        self.quality = bool(flags & N.B2V_FLAG_QUALITY)
         self.device = device
         self.width, self.height = width, height
         self.dst_width, self.dst_height = dst_width or width, dst_height or height
@@ -178,9 +198,19 @@ class Session:
             self._on_frame(fptr)
         if self._collect:
             f = fptr.contents
-            rec = EncodedFrame(C.string_at(f.data, f.size), f.frame_id, bool(f.is_key), f.qp, f.pts90k, f.capture_ns, f.y_start, f.height)
+            rec = EncodedFrame(C.string_at(f.data, f.size), f.frame_id, bool(f.is_key), f.qp, f.pts90k, f.capture_ns, f.y_start, f.height,
+                               self.frame_quality())
             with self._lock:
                 self.frames.append(rec)
+
+    def frame_quality(self) -> Optional[FrameQuality]:
+        """Inside `on_frame` (the library's output thread): the quality of the record being delivered, or None when the session
+        does not measure it."""
+        if not self.quality:
+            return None
+        q = N.B2VQuality()
+        N.check(self._lib.b2v_frame_quality(self._h, C.byref(q)))
+        return FrameQuality.from_native(q)
 
     # -- ingest ---------------------------------------------------------------------------------
     def submit(self, bgra: np.ndarray, capture_ns: int = 0) -> None:

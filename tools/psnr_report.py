@@ -1,11 +1,11 @@
-"""PSNR / bitrate table of the CUDA encoder (SURVEY.md §8c.4 iii: decoded-vs-source PSNR per config and bitrate).
+"""PSNR / SSIM / bitrate table of the CUDA encoder (SURVEY.md §8c.4 iii: decoded-vs-source quality per config and bitrate).
+Every picture is measured on the GPU by the session itself (Session(quality=True), B2V_FLAG_QUALITY): the reconstruction, which
+is what a decoder outputs, against the picture the encoder coded.
 Run on the GPU box:  python tools/psnr_report.py  -> gpurun_out/psnr_report.json
 The x264 comparator is absent from this image (probed at run time), so the table is absolute."""
-import json, os, shutil, sys, time
+import json, os, shutil, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
-import oracle
-from oracle import avdec
 from selkies_b200 import _native as N
 from selkies_b200.session import Session
 from tests import synth
@@ -31,35 +31,26 @@ _cache = {}
 
 
 def prepared(w, h, name, n):
-    """frames + their oracle NV12 (computed once per content and reused for every bitrate)."""
+    """frames (made once per content and reused for every bitrate)."""
     key = (w, h, name, n)
     if key not in _cache:
         _cache.clear()
-        frames = content(name, w, h, n)
-        src = {}
-        for f in frames:
-            if id(f) not in src:
-                src[id(f)] = oracle.csc_nv12(f)
-        _cache[key] = (frames, [src[id(f)] for f in frames])
+        _cache[key] = content(name, w, h, n)
     return _cache[key]
 
 
 def run(w, h, name, kbps, fps, n):
-    frames, nv12 = prepared(w, h, name, n)
-    with Session(w, h, fps=fps, rc_mode=N.B2V_RC_CBR, bitrate_kbps=kbps, ring_slots=4) as s:
+    frames = prepared(w, h, name, n)
+    with Session(w, h, fps=fps, rc_mode=N.B2V_RC_CBR, bitrate_kbps=kbps, ring_slots=4, quality=True) as s:
         for f in frames:
             s.submit(f)
         s.flush()
         got = s.take_frames()
-    dec = avdec.decode_stream([g.data for g in got], quiet=True)
-    assert len(dec) == n
+    assert len(got) == n
     tail = range(n // 2, n)              # steady state: the second half, after the key-frame burst has been absorbed
-    ps = {}
-    for i in [0] + list(tail)[::3]:
-        (Y, U, V), (sy, suv) = dec[i], nv12[i]
-        ps[i] = (avdec.psnr(Y, sy), avdec.psnr(U, suv[:, 0::2]), avdec.psnr(V, suv[:, 1::2]))
+    ps = {i: got[i].quality.psnr for i in range(n)}
     sizes = [len(g.data) for g in got]
-    tl = [i for i in ps if i != 0 or n == 1]
+    tl = [i for i in tail if i != 0] or [0]
     win = int(fps)
     tb = kbps * 1000.0 / fps / 8.0             # target bytes per picture
     windows = [sum(sizes[i:i + win]) / (tb * win) for i in range(0, max(1, n - win + 1))]
@@ -71,6 +62,8 @@ def run(w, h, name, kbps, fps, n):
             "qp_pinned": "max" if min(qps[n // 2:]) >= 51 else "min" if max(qps[n // 2:]) <= 10 else None, "idr_bytes": sizes[0],
             "psnr_y_steady": float(np.mean([ps[i][0] for i in tl])), "psnr_u_steady": float(np.mean([ps[i][1] for i in tl])),
             "psnr_v_steady": float(np.mean([ps[i][2] for i in tl])), "psnr_y_idr": ps[0][0],
+            "ssim_y_steady": float(np.mean([got[i].quality.ssim for i in tl])), "ssim_y_idr": got[0].quality.ssim,
+            "psnr_y_min": float(min(ps[i][0] for i in range(n))),
             "qp_first_last": [got[0].qp, got[-1].qp], "qp_steady_mean": float(np.mean([got[i].qp for i in tail]))}
 
 
