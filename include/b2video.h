@@ -102,10 +102,26 @@ enum {
                                    file is preceded by frame_id u16be | y_start u16be (the reference adds 03 00 in front, selkies.py:3118).
                                    crf = jpeg_quality, paintover_crf = paint_over_jpeg_quality, paintover_trigger_frames as for H.264.
                                    A key-frame request re-sends every stripe. */
-  B2V_FLAG_QUALITY       = 64   /* measure every delivered record on the GPU (b2v_frame_quality): SSE per plane and luma SSIM of the
+  B2V_FLAG_QUALITY       = 64,  /* measure every delivered record on the GPU (b2v_frame_quality): SSE per plane and luma SSIM of the
                                    reconstruction against the picture the encoder coded.  H.264 only: b2v_create rejects it with
                                    B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE (B2V_EINVAL), which have no reconstruction.  The access units
                                    are the same bytes with and without it; it costs one kernel launch per picture (kernel_launches). */
+  B2V_FLAG_DROPPABLE     = 128  /* two temporal layers, so that a consumer that falls behind can shed pictures without corrupting the
+                                   stream.  The pictures of a session are counted from each IDR (the IDR is 0; b2v_request_idr,
+                                   gop and b2v_set_resolution restart the count).  Every P picture at an odd count is a
+                                   non-reference picture: all its slices have nal_ref_idc = 0 and no dec_ref_pic_marking().  Every
+                                   other picture is a reference picture, as without the flag.  A P picture at an even count
+                                   predicts from the reference picture two before it, one at an odd count from the picture just
+                                   before it.  frame_num advances by one after each reference picture only: a non-reference picture
+                                   carries the frame_num of the reference picture that follows it.  The SPS does not change
+                                   (max_num_ref_frames 1, no frame_num gaps).  A consumer may drop any set of non-reference access
+                                   units; the rest decodes to exactly the encoder's reconstructions of the pictures it kept.  It
+                                   tells a droppable access unit by the NAL header byte of its first slice (nal_ref_idc, bits 5..6,
+                                   is 0).  b2v_get_recon returns the last coded picture, droppable or not.  H.264 full-frame only:
+                                   b2v_create rejects it (B2V_EINVAL) with B2V_FLAG_JPEG, B2V_FLAG_NO_ENCODE or in striped mode
+                                   (stripe_rows > 0 and less than the picture's macroblock rows), and b2v_set_resolution rejects a
+                                   size at which stripe_rows would stripe.  It costs a third reconstruction buffer (coded
+                                   width x height x 1.5 bytes). */
 };
 
 /* One encoded frame, the native image of the pixelflux callback result

@@ -96,7 +96,7 @@ struct Session {
   b2v_settings cfg{};
   int device = 0;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
-  bool encode = true, timing = false, timing_csc_only = false, quality = false;
+  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;
 
   // ingest ring
@@ -156,6 +156,8 @@ int round16(int v) { return (v + 15) & ~15; }
 
 // frame sizes a session takes, source and encoded alike: even, 16..7680 x 16..4320
 bool size_ok(int w, int h) { return w >= 16 && h >= 16 && w <= 7680 && h <= 4320 && !(w & 1) && !(h & 1); }
+// H.264 striped mode at an encoded height of dst_h rows (the encoder's rule: stripe_rows > 0 and less than the macroblock rows)
+bool stripes_active(int stripe_rows, int dst_h) { return stripe_rows > 0 && stripe_rows < round16(dst_h) / 16; }
 
 int alloc_geometry(Session* s) {
   // (re)allocate everything that depends on the frame size
@@ -193,6 +195,7 @@ int alloc_geometry(Session* s) {
     ec.stripe_rows = s->cfg.stripe_rows > 0 ? s->cfg.stripe_rows : 0;
     ec.idr_slice_mbs = s->cfg.idr_slice_mbs;
     ec.quality = s->quality;
+    ec.droppable = s->droppable;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
     s->lay = encoder_layout(s->enc);
@@ -693,6 +696,12 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if ((cfg->flags & B2V_FLAG_QUALITY) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
     return fail(B2V_EINVAL, "B2V_FLAG_QUALITY measures the H.264 reconstruction: %s has none",
                 (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+  if ((cfg->flags & B2V_FLAG_DROPPABLE) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
+    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE layers H.264 pictures: %s codes none",
+                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+  if ((cfg->flags & B2V_FLAG_DROPPABLE) && stripes_active(cfg->stripe_rows, dh))
+    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
+                "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(B2V_EINVAL, "device %d out of range (%d devices)", cfg->device, ndev);
@@ -703,6 +712,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->encode = !(cfg->flags & B2V_FLAG_NO_ENCODE);
   s->jpeg = (cfg->flags & B2V_FLAG_JPEG) != 0;
   s->quality = (cfg->flags & B2V_FLAG_QUALITY) != 0;
+  s->droppable = (cfg->flags & B2V_FLAG_DROPPABLE) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;
@@ -901,6 +911,9 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   if (dw <= 0) dw = sw;
   if (dh <= 0) dh = sh;
   if (!size_ok(sw, sh) || !size_ok(dw, dh)) return fail(B2V_EINVAL, "size unsupported");
+  if (s->droppable && stripes_active(s->cfg.stripe_rows, dh))
+    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d would stripe a picture of %d macroblock rows",
+                s->cfg.stripe_rows, round16(dh) / 16);
   // Submitters are locked out FIRST; then everything in flight drains (the output thread needs `mu`, not `submit_mu`, so it
   // keeps delivering); a producer still holding an acquired slot would be writing into memory about to be freed: refuse.
   std::lock_guard<std::mutex> sub(s->submit_mu);

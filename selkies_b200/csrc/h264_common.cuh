@@ -61,8 +61,10 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   int pic;                 // picture counter of this encoder (parity selects the feedback record and the double-buffered side data)
   long long target_bits;
   int frame_num, idr_pic_id;
+  int nal_ref_idc;         // 3 IDR, 2 reference P picture, 0 non-reference P picture (B2V_FLAG_DROPPABLE)
+  int ref_dist, prev_ref_dist;   // pictures back to this picture's reference, and to the previous picture's (1 or 2; temporal predictor)
   const uint8_t* cur;      // NV12 coded size
-  const uint8_t* ref;      // previous reconstruction (NV12)
+  const uint8_t* ref;      // reconstruction of the last reference picture (NV12)
   uint8_t* recon;          // reconstruction being written
   MbInfo* mbinfo;          // this picture's records (double-buffered: the entropy kernels of picture k read them while picture k+1 is analysed)
   const MbInfo* mbinfo_prev;   // the previous picture's records (temporal motion predictor)

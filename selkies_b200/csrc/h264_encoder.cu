@@ -30,8 +30,10 @@ struct Encoder {
   EncoderConfig cfg{};
   int mbw = 0, mbh = 0;
   SliceGrid p_grid, idr_grid;
-  uint8_t* recon[2] = {nullptr, nullptr};
-  int cur = 0;
+  // NV12 reconstructions: two, or three with B2V_FLAG_DROPPABLE (buffer rule in encoder_encode).  `last` holds the last coded
+  // picture's, `ref_buf` the last reference picture's (the same one unless the last picture was a non-reference picture).
+  uint8_t* recon[3] = {nullptr, nullptr, nullptr};
+  int n_recon = 2, last = 0, ref_buf = 0;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
   // of picture k (packing stream) overlaps the analysis of picture k+1 (main stream)
   MbInfo* mbinfo[2] = {nullptr, nullptr};
@@ -56,6 +58,10 @@ struct Encoder {
   size_t au_cap = 0;
   int frame_num = 0, idr_count = 0;
   bool have_ref = false;
+  // B2V_FLAG_DROPPABLE: pictures since the last IDR (the IDR is 0), and the layer and reference distance of the last picture
+  long long since_idr = 0;
+  bool last_was_ref = true;
+  int last_ref_dist = 1;
 };
 
 namespace {
@@ -179,10 +185,11 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     e->idr_grid = slice_grid(e->mbw, e->mbh, 1, cols);
   }
   const size_t mbs = (size_t)e->mbw * e->mbh, fb = (size_t)cfg->coded_w * cfg->coded_h * 3 / 2;
-  ECK(cudaMalloc((void**)&e->recon[0], fb));
-  ECK(cudaMalloc((void**)&e->recon[1], fb));
-  ECK(cudaMemset(e->recon[0], 0, fb));
-  ECK(cudaMemset(e->recon[1], 0, fb));
+  e->n_recon = cfg->droppable ? 3 : 2;
+  for (int b = 0; b < e->n_recon; b++) {
+    ECK(cudaMalloc((void**)&e->recon[b], fb));
+    ECK(cudaMemset(e->recon[b], 0, fb));
+  }
   for (int b = 0; b < 2; b++) {
     ECK(cudaMalloc((void**)&e->mbinfo[b], mbs * sizeof(MbInfo)));
     ECK(cudaMemset(e->mbinfo[b], 0, mbs * sizeof(MbInfo)));
@@ -222,6 +229,7 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   // bands: full-frame coding is one band of mbh rows; striped mode gives every band its own SPS (height = the band's)
   const int crop_b = (cfg->coded_h - cfg->height) / 2;
   e->striped = cfg->stripe_rows > 0 && cfg->stripe_rows < e->mbh;
+  if (e->striped && cfg->droppable) { snprintf(g_enc_err, sizeof g_enc_err, "non-reference pictures are not coded in striped mode"); encoder_destroy(e); return -1; }
   if (e->striped && cfg->stripe_rows % cfg->slice_rows) { snprintf(g_enc_err, sizeof g_enc_err, "stripe_rows must be a multiple of slice_rows"); encoder_destroy(e); return -1; }
   e->band_rows = e->striped ? cfg->stripe_rows : e->mbh;
   e->n_bands = (e->mbh + e->band_rows - 1) / e->band_rows;
@@ -258,7 +266,7 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
 
 void encoder_destroy(Encoder* e) {
   if (!e) return;
-  void* ptrs[] = {e->recon[0], e->recon[1], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
+  void* ptrs[] = {e->recon[0], e->recon[1], e->recon[2], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
                   e->q_acc, e->q_done};
@@ -273,20 +281,27 @@ void encoder_destroy(Encoder* e) {
 AuLayout encoder_layout(const Encoder* e) {
   return {e->au_cap, e->au_data_off, e->striped ? e->n_bands : 0, e->striped ? e->band_rows : 0, e->quality_off};
 }
-const uint8_t* encoder_recon(const Encoder* e) { return e->recon[e->cur]; }
+const uint8_t* encoder_recon(const Encoder* e) { return e->recon[e->last]; }
 
 int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   const bool idr = p->idr || !e->have_ref;
-  e->cur ^= 1;
   const int par = (int)(e->pic & 1);          // parity of this picture: feedback record, side-data buffers, events
-  if (idr) e->frame_num = 0;
+  if (idr) { e->frame_num = 0; e->since_idr = 0; }
+  // B2V_FLAG_DROPPABLE: counted from the IDR, every P picture at an odd count is a non-reference picture.  Every P picture predicts
+  // from the last reference picture: the one just before it, or two before it when that one was a non-reference picture.
+  const bool is_ref = !e->cfg.droppable || idr || (e->since_idr & 1) == 0;
+  const int ref_dist = e->last_was_ref ? 1 : 2;
+  // the buffer this picture writes: neither the last picture's reconstruction nor this picture's reference (see the schedule below)
+  int wb = 0;
+  while (wb == e->last || wb == e->ref_buf) wb++;
   FrameCtx f{};
   f.cw = e->cfg.coded_w; f.ch = e->cfg.coded_h; f.mbw = e->mbw; f.mbh = e->mbh;
   const SliceGrid& g = idr ? e->idr_grid : e->p_grid;
   f.slice_rows = g.rows; f.slice_cols = g.cols; f.n_slices = g.n; f.slice_words = g.words; f.chunks_per_slice = g.chunks;
   f.idr = idr; f.rc_mode = p->rc_mode; f.qp_fixed = p->qp_fixed; f.target_bits = p->target_bits;
   f.frame_num = e->frame_num; f.idr_pic_id = e->idr_count; f.pic = (int)(e->pic & 0x7fffffff);
-  f.cur = p->cur; f.ref = e->recon[e->cur ^ 1]; f.recon = e->recon[e->cur];
+  f.nal_ref_idc = idr ? 3 : is_ref ? 2 : 0; f.ref_dist = ref_dist; f.prev_ref_dist = e->last_ref_dist;
+  f.cur = p->cur; f.ref = e->recon[e->ref_buf]; f.recon = e->recon[wb];
   f.mbinfo = e->mbinfo[par]; f.mbinfo_prev = e->mbinfo[par ^ 1]; f.i4modes = e->i4modes[par]; f.coef = e->coef[par]; f.nnz = e->nnz[par];
   f.me_pub = e->me_pub; f.me_queue = e->me_queue; f.search_blocks = e->search_blocks;
   f.chunk_agg = (ChunkAgg*)e->chunk_agg; f.chunk_inc = (ChunkInc*)e->chunk_inc; f.slice_done = e->slice_done;
@@ -304,7 +319,13 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   //  * the rate controller feeds back two pictures late: picture k reads the record left by picture k-2 (RcFb), which the scan
   //    of picture k-1 — possibly still running — never touches;
   //  * the analysis of picture k waits for the pack of picture k-2: that releases this parity's side data, the reconstruction
-  //    buffer it is about to overwrite (the pack's copy kernel reads I_PCM samples from it) and the record of k-2.
+  //    buffer it is about to overwrite (the pack's copy kernel reads I_PCM samples from it) and the record of k-2;
+  //  * the reconstruction picture k writes is neither picture k-1's (the pack of k-1 may still be reading its I_PCM samples) nor
+  //    picture k's reference.  Two buffers: that leaves the one picture k-2 wrote, released by the wait above.  Three buffers
+  //    (B2V_FLAG_DROPPABLE): after a reference picture k-1 two qualify, picture k-2's and one last written by k-3 or earlier;
+  //    after a non-reference picture k-1 the reference is picture k-2's and the one left was last written by k-3 or earlier.  The
+  //    pack of k-3 precedes that of k-2 on the pack stream, so the wait above has released it too.  Which of two qualifying
+  //    buffers is taken changes no output.
   // k_quality runs right behind the analysis, on `st`: the only moment both of its inputs are complete and intact (the next
   // picture's colour conversion on `st` overwrites `cur`, the analysis of picture k+2 this reconstruction).
   const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
@@ -333,8 +354,12 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   if (p->ev) cudaEventRecord(p->ev[5], st);
   if (overlap) cudaEventRecord(e->ev_packed[par], sp);
   if (idr) e->idr_count++;
-  e->frame_num = (e->frame_num + 1) & 255;
+  if (is_ref) e->frame_num = (e->frame_num + 1) & 255;     // a non-reference picture carries the frame_num of the next reference
   e->have_ref = true;
+  e->last = wb;
+  if (is_ref) e->ref_buf = wb;
+  e->last_was_ref = is_ref; e->last_ref_dist = ref_dist;
+  e->since_idr++;
   e->pic++;
   return n;
 }

@@ -18,6 +18,7 @@ struct EncoderConfig {
   int stripe_rows;         // macroblock rows per band (multiple of slice_rows); 0 = full-frame
   int idr_slice_mbs;       // IDR pictures, whatever slice_rows is: macroblocks per slice inside a row; 0 = default rule (>= 0)
   bool quality;            // B2V_FLAG_QUALITY: k_quality measures every band into the access unit's quality table
+  bool droppable;          // B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture (full frame only)
 };
 
 struct EncodeFrameParams {

@@ -197,7 +197,8 @@ __device__ __forceinline__ void slice_header(S& s, const FrameCtx& f, int first_
   s.put(8, (uint32_t)(frame_num & 255));
   if (f.idr) put_ue(s, (uint32_t)(f.idr_pic_id & 15));
   if (!f.idr) { s.put(1, 0); s.put(1, 0); }
-  if (f.idr) { s.put(1, 0); s.put(1, 0); } else s.put(1, 0);
+  // dec_ref_pic_marking(), present in reference pictures only
+  if (f.idr) { s.put(1, 0); s.put(1, 0); } else if (f.nal_ref_idc) s.put(1, 0);
   put_se(s, qp - 26);
   put_ue(s, 1);
 }
@@ -543,7 +544,7 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
     long long o = base;
     if (start_len == 4) au[o++] = 0;
     au[o++] = 0; au[o++] = 0; au[o++] = 1;
-    au[o++] = (uint8_t)(((f.idr ? 3 : 2) << 5) | (f.idr ? 5 : 1));
+    au[o++] = (uint8_t)((f.nal_ref_idc << 5) | (f.idr ? 5 : 1));
   }
   copy_escaped<H264Escape>(f.slice_buf + (size_t)s * f.slice_words, n, f.slice_words, au, base + start_len + 1, cap, s_wsum);
   if (band_first) {

@@ -164,11 +164,22 @@ __device__ __forceinline__ MbPos mb_pos(const FrameCtx& f, int mb) {
   return p;
 }
 
+// With B2V_FLAG_DROPPABLE the previous picture's vector spans f.prev_ref_dist pictures and this picture's reference lies f.ref_dist
+// pictures back (1 or 2 each), so as a temporal predictor the vector is scaled by ref_dist / prev_ref_dist: doubled exactly, or halved
+// rounding half away from zero, v -> sign(v) * ((|v| + 1) >> 1) (oracle/h264_layers_ref.c scale_mv).  Both distances are 1 without the flag;
+// the kernels are instantiated with SCALE = false for pictures whose two distances are equal, which then run the code of a build
+// without layers.
+__device__ __forceinline__ int scale_mv(int v, int num, int den) {
+  const int s = v >> 31, h = ((((v ^ s) - s) + 1) >> 1 ^ s) - s;
+  return num == den ? v : num > den ? 2 * v : h;
+}
+
 // The start of a macroblock in both passes: one batch of independent global loads — the source block, staged into the tile, the
 // co-located luma block z and, speculatively (otherwise they cost a dependent-load latency later), the co-located chroma reference
-// (the chroma prediction of a zero vector) and the previous picture's record (temporal predictor) — and SAD(0,0) from the source and
-// z as loaded.  The tile is read by other lanes after a __syncwarp.
+// (the chroma prediction of a zero vector) and the previous picture's record (temporal predictor; its vector scaled to this
+// picture's reference distance) — and SAD(0,0) from the source and z as loaded.  The tile is read by other lanes after a __syncwarp.
 struct MbStart { uint32_t uv_coloc; uint2 z; MbInfo prev; int sad0; };
+template <bool SCALE>
 __device__ __forceinline__ MbStart start_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p) {
   const size_t ysz = (size_t)f.cw * f.ch;
   const int x0 = p.mbx * 16, r8 = lane >> 1, c8 = (lane & 1) * 8;
@@ -176,6 +187,7 @@ __device__ __forceinline__ MbStart start_mb(const FrameCtx& f, MbTile& t, int la
   s.uv_coloc = __ldg(reinterpret_cast<const uint32_t*>(f.ref + ysz + (size_t)(p.mby * 8 + (lane >> 2)) * f.cw + x0 + (lane & 3) * 4));
   s.z = __ldg(reinterpret_cast<const uint2*>(f.ref + (size_t)(p.mby * 16 + r8) * f.cw + x0 + c8));
   s.prev = f.mbinfo_prev[p.mb];
+  if (SCALE) { s.prev.mvx = (int16_t)scale_mv(s.prev.mvx, f.ref_dist, f.prev_ref_dist); s.prev.mvy = (int16_t)scale_mv(s.prev.mvy, f.ref_dist, f.prev_ref_dist); }
   const uint2 c = stage_source(f, t, lane, x0, p.mby, ysz);
   s.sad0 = __reduce_add_sync(FULL, (int)sad4acc(c.x, s.z.x, sad4acc(c.y, s.z.y, 0u)));
   return s;
@@ -191,7 +203,7 @@ __device__ __forceinline__ bool full_sample_candidate(int mvx, int mvy, int& kx,
 // content repeats it; the zero vector counts: static content whose co-located SAD sits just above the early-termination threshold
 // would otherwise search only to find (0,0) again), and the 24 rows x 8 words of the window from (ra, wa) on that its test, a refinement
 // around it and its prediction touch: rows [13+cdy, 36+cdy] and bytes [13+cdx, 34+cdx] cover the 3x3 test (rows 15+cdy..32+cdy), the
-// 6-tap support (-3..+18) and the prediction, clamped so that they stay inside the window.
+// 6-tap support (-3..+18) and the prediction, clamped so that they stay inside the window.  `prev`: as start_mb scaled it.
 struct TemporalPred { int cdx, cdy, ra, wa; bool try_pred; };
 __device__ __forceinline__ TemporalPred temporal_predictor(const MbInfo& prev) {
   TemporalPred tp;
@@ -320,6 +332,7 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 // a temporal-predictor hit that needs no refinement are finished here; every other one goes into a queue for k_inter_search —
 // anchors into the anchor queue, the rest into the other.  No search and no 48 x 48 window: the registers and shared memory of
 // the search do not cap the occupancy of the common case.
+template <bool SCALE>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) {
   __shared__ __align__(16) LeanSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -331,7 +344,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
   MbTile& t = sm.t;
   const int qp = frame_qp(f), lambda = me_lambda[qp];
   const int ylo = p.band_r0 * 16, yhi = min(f.mbh, p.band_r0 + f.band_rows) * 16 - 1;
-  const MbStart s = start_mb(f, t, lane, p);
+  const MbStart s = start_mb<SCALE>(f, t, lane, p);
   __syncwarp();
 
   // zero-motion early termination: co-located block within the quantisation noise of this QP
@@ -370,6 +383,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
 // One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
 // previous picture's records are not written during the analysis of a picture).  Its co-located block failed the zero-motion test
 // there and fails it again here, so that test is not repeated; its temporal predictor fails, or hits, as it did there.
+template <bool SCALE>
 __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int lane, const MbPos& p) {
   const int mb = p.mb, x0 = p.mbx * 16, y0 = p.mby * 16;
   const bool anchor = p.anchor;
@@ -379,7 +393,7 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   // reference rows this macroblock may touch: its own band (the band's decoder pads at the band's edges, 8.4.2.2.1)
   const int ylo = p.band_r0 * 16, yhi = min(f.mbh, p.band_r0 + f.band_rows) * 16 - 1;
   const uint8_t* __restrict__ ref_y = f.ref;
-  const MbStart s = start_mb(f, t, lane, p);
+  const MbStart s = start_mb<SCALE>(f, t, lane, p);
   *reinterpret_cast<uint2*>(&sm.win[16 + (lane >> 1)][4 + (lane & 1) * 2]) = s.z;     // the co-located block: window rows 16..31, words 4..7
   __syncwarp();
 
@@ -531,13 +545,14 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
 
 // Passes B and C: the queue k_inter_lean filled (0: anchors, 1: the rest), walked by a grid of the kernel's resident capacity.  No
 // decision here depends on another entry of the same queue, so the order inside a queue does not matter.
+template <bool SCALE>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search(FrameCtx f, int queue) {
   __shared__ __align__(16) InterSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = f.me_queue[queue];
   const int* q = f.me_queue + 2 + (size_t)queue * f.mbw * f.mbh;
   for (int i = blockIdx.x * WARPS_PER_BLOCK + warp; i < n; i += gridDim.x * WARPS_PER_BLOCK) {
-    search_mb(f, sm_all[warp], lane, mb_pos(f, q[i]));
+    search_mb<SCALE>(f, sm_all[warp], lane, mb_pos(f, q[i]));
     __syncwarp();
   }
 }
@@ -546,7 +561,7 @@ cudaError_t inter_search_grid(int* blocks) {
   int dev = 0, sms = 0, per_sm = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search, 32 * WARPS_PER_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search<false>, 32 * WARPS_PER_BLOCK, 0);
   *blocks = sms * per_sm;
   return e;
 }
@@ -554,9 +569,16 @@ cudaError_t inter_search_grid(int* blocks) {
 int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
-  k_inter_lean<<<(f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-  k_inter_search<<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
-  k_inter_search<<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+  const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+  if (f.ref_dist == f.prev_ref_dist) {      // every picture without B2V_FLAG_DROPPABLE
+    k_inter_lean<false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_search<false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
+    k_inter_search<false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+  } else {
+    k_inter_lean<true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_search<true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+    k_inter_search<true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+  }
   return 3;
 }
 

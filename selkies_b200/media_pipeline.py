@@ -90,7 +90,8 @@ class MediaPipelineB200(MediaPipeline):
     def __init__(self, async_event_loop: asyncio.AbstractEventLoop, encoder_rtc: str = "x264enc", framerate: int = 30,
                  video_bitrate: int = 8, audio_bitrate: int = 128000, width: int = 1920, height: int = 1080,
                  audio_channels: int = 2, audio_enabled: bool = False, audio_device_name="output.monitor",
-                 crf: int = 23, rc_mode: RateControlMode = RateControlMode.CBR, gpu_id: int = 0, frame_source=None):
+                 crf: int = 23, rc_mode: RateControlMode = RateControlMode.CBR, gpu_id: int = 0, frame_source=None,
+                 droppable_frames: bool = False):
         self.async_event_loop = async_event_loop
         self.async_lock = asyncio.Lock()
         # what selkies reads back
@@ -98,6 +99,8 @@ class MediaPipelineB200(MediaPipeline):
         self.width, self.height, self.framerate = width, height, framerate
         self.video_bitrate, self.h264_crf, self.rc_mode = video_bitrate, crf, rc_mode        # Mbit/s, QP, mode
         self.capture_cursor = False
+        # every second P picture a non-reference picture, which the WebRTC mailbox (rtc_bridge.PipelineBridge) drops first
+        self.droppable_frames = droppable_frames
         self.last_resize_success = True
         # audio parameters are only carried
         self.audio_bitrate, self.audio_channels = audio_bitrate, audio_channels
@@ -203,6 +206,7 @@ class MediaPipelineB200(MediaPipeline):
             cs.h264_bitrate_kbps = self.video_bitrate * 1000
             cs.vaapi_render_node_index = -1
             cs.use_cpu = self.encoder_rtc == "x264enc"      # carried for compatibility; the encode always runs on the GPU
+            cs.h264_droppable_frames = bool(self.droppable_frames)
         return cs
 
     def _on_encoded(self, result_ptr, _user) -> None:

@@ -76,6 +76,7 @@ class CaptureSettings:
         self.output_width = 0                    # != capture size => fused bilinear scale
         self.output_height = 0
         self.quality_metrics = False             # measure every delivered record on the GPU: results carry `quality` (H.264 only)
+        self.h264_droppable_frames = False       # every second P picture a non-reference picture a lagging consumer may drop (full frame only)
 
 
 class StripeCallback:
@@ -253,6 +254,10 @@ class ScreenCapture:
             s.ring_slots = 4
             s.flags = 0
             s.quality = bool(getattr(settings, "quality_metrics", False))      # b2v_create refuses it in JPEG mode
+            s.droppable = bool(getattr(settings, "h264_droppable_frames", False))
+            if s.droppable and (jpeg or not bool(getattr(settings, "h264_fullframe", True))):
+                raise ValueError("h264_droppable_frames needs full-frame H.264 (output_mode 1, h264_fullframe True): "
+                                 "JPEG has no reference pictures and every H.264 stripe is a stream of its own")
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)

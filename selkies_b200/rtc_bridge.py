@@ -12,22 +12,37 @@ import asyncio
 from fractions import Fraction
 from typing import Any, Optional
 
+from .h264_nal import is_droppable
+
 RTP_VIDEO_CLOCK_RATE = 90000
 
 
 class PipelineBridge:
     """Newest-sample-wins mailbox between the encoder callback and the RTP sender: same contract as the reference's bridge
     (rtc.py:102-118: a lagging consumer sees the newest sample only; `get_data` waits for one).  Everything happens on the
-    event loop and `set_data` never yields between the drop and the put, so no lock is involved."""
+    event loop and `set_data` never yields between the drop and the put, so no lock is involved.
+
+    A reference sample is never dropped while a droppable one can go (B2V_FLAG_DROPPABLE: nothing predicts from a droppable
+    sample, so the stream stays decodable without it): a waiting droppable sample is replaced; a new droppable sample arriving
+    while a reference sample waits is dropped itself; of two reference samples the older is dropped, as without the flag, and
+    also counted in `dropped_reference` (the decoder predicts from a picture it never got until the next IDR).  A sample
+    without a `droppable` attribute counts as a reference sample."""
 
     def __init__(self):
         self._slot: asyncio.Queue = asyncio.Queue(maxsize=1)
         self.dropped = 0
+        self.dropped_reference = 0
 
     async def set_data(self, data: Any):
         while self._slot.full():
-            self._slot.get_nowait()
+            old = self._slot.get_nowait()
             self.dropped += 1
+            if getattr(old, "droppable", False):
+                continue
+            if getattr(data, "droppable", False):
+                self._slot.put_nowait(old)             # the waiting reference sample stays, the new droppable one goes
+                return
+            self.dropped_reference += 1
         self._slot.put_nowait(data)
 
     async def get_data(self):
@@ -35,13 +50,15 @@ class PipelineBridge:
 
 
 class VideoSample:
-    """What the sender needs of `av.Packet`: bytes(sample), .pts, .dts, .time_base, .is_keyframe."""
-    __slots__ = ("data", "pts", "dts", "time_base", "is_keyframe")
+    """What the sender needs of `av.Packet`: bytes(sample), .pts, .dts, .time_base, .is_keyframe; and .droppable, read from the
+    access unit: a non-reference picture (B2V_FLAG_DROPPABLE) that PipelineBridge sheds first."""
+    __slots__ = ("data", "pts", "dts", "time_base", "is_keyframe", "droppable")
 
     def __init__(self, data: bytes, pts: Optional[int], is_keyframe: bool = False):
         self.data, self.pts, self.dts = data, pts, pts
         self.time_base = Fraction(1, RTP_VIDEO_CLOCK_RATE)
         self.is_keyframe = is_keyframe
+        self.droppable = is_droppable(data)
 
     def __bytes__(self):
         return self.data

@@ -15,6 +15,7 @@ from typing import Callable, NamedTuple, Optional
 import numpy as np
 
 from . import _native as N
+from .h264_nal import is_droppable
 
 
 class FrameQuality(NamedTuple):
@@ -32,10 +33,10 @@ class FrameQuality(NamedTuple):
 
 
 class EncodedFrame:
-    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height", "quality")
+    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height", "quality", "droppable")
 
     def __init__(self, data: bytes, frame_id: int, is_key: bool, qp: int, pts90k: int, capture_ns: int, y_start: int = 0, height: int = 0,
-                 quality: Optional[FrameQuality] = None):
+                 quality: Optional[FrameQuality] = None, droppable: bool = False):
         self.data = data
         self.frame_id = frame_id
         self.is_key = is_key
@@ -44,6 +45,7 @@ class EncodedFrame:
         self.capture_ns = capture_ns
         self.y_start, self.height = y_start, height
         self.quality = quality          # None unless the session measures quality (Session(quality=True))
+        self.droppable = droppable      # a non-reference picture a consumer may drop (Session(droppable=True)); read from the data
 
 
 # pixel formats of device frames: name -> (B2V_PIX_* code, bytes per pixel); the name is the byte order in memory
@@ -167,11 +169,15 @@ class Session:
                  device: int = 0, rc_mode: int = N.B2V_RC_CBR, bitrate_kbps: int = 8000, crf: int = 26,
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
-                 collect: bool = True, quality: bool = False):
+                 collect: bool = True, quality: bool = False, droppable: bool = False):
         self._lib = N.lib()
         if quality:
             flags |= N.B2V_FLAG_QUALITY
+        if droppable:
+            flags |= N.B2V_FLAG_DROPPABLE
         self.quality = bool(flags & N.B2V_FLAG_QUALITY)
+        self.droppable = bool(flags & N.B2V_FLAG_DROPPABLE)
+        self._hdr_len = 10 if header_mode == N.B2V_HDR_PIXELFLUX else 0
         self.device = device
         self.width, self.height = width, height
         self.dst_width, self.dst_height = dst_width or width, dst_height or height
@@ -198,8 +204,9 @@ class Session:
             self._on_frame(fptr)
         if self._collect:
             f = fptr.contents
-            rec = EncodedFrame(C.string_at(f.data, f.size), f.frame_id, bool(f.is_key), f.qp, f.pts90k, f.capture_ns, f.y_start, f.height,
-                               self.frame_quality())
+            data = C.string_at(f.data, f.size)
+            rec = EncodedFrame(data, f.frame_id, bool(f.is_key), f.qp, f.pts90k, f.capture_ns, f.y_start, f.height,
+                               self.frame_quality(), self.droppable and is_droppable(data, self._hdr_len))
             with self._lock:
                 self.frames.append(rec)
 
