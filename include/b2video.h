@@ -106,7 +106,7 @@ enum {
                                    reconstruction against the picture the encoder coded.  H.264 only: b2v_create rejects it with
                                    B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE (B2V_EINVAL), which have no reconstruction.  The access units
                                    are the same bytes with and without it; it costs one kernel launch per picture (kernel_launches). */
-  B2V_FLAG_DROPPABLE     = 128  /* two temporal layers, so that a consumer that falls behind can shed pictures without corrupting the
+  B2V_FLAG_DROPPABLE     = 128, /* two temporal layers, so that a consumer that falls behind can shed pictures without corrupting the
                                    stream.  The pictures of a session are counted from each IDR (the IDR is 0; b2v_request_idr,
                                    gop and b2v_set_resolution restart the count).  Every P picture at an odd count is a
                                    non-reference picture: all its slices have nal_ref_idc = 0 and no dec_ref_pic_marking().  Every
@@ -122,6 +122,17 @@ enum {
                                    (stripe_rows > 0 and less than the picture's macroblock rows), and b2v_set_resolution rejects a
                                    size at which stripe_rows would stripe.  It costs a third reconstruction buffer (coded
                                    width x height x 1.5 bytes). */
+  B2V_FLAG_WIDE_MOTION   = 256  /* find motion vectors beyond the +-16 samples of the P-picture search, for fast scrolls and window
+                                   drags.  Every picture gets a 1/4 x 1/4 decimated luma plane; in every 4 x 4-macroblock group
+                                   whose anchor's co-located block changed, that block is searched in the reference picture's
+                                   plane over +-128 samples horizontally and +-256 vertically, inside the picture and the band.
+                                   The anchor then also searches +-16 samples around that coarse vector, and a temporal or anchor
+                                   predictor beyond the co-located window is tested in a window centred on it.  Every vector
+                                   component stays within [-256, 255.75] samples, the range the SPS's VUI asserts.  The SPS and
+                                   the syntax do not change; the access units do (that is the point).  Works with stripes,
+                                   scaling, B2V_FLAG_DROPPABLE and B2V_FLAG_QUALITY.  H.264 only: b2v_create rejects it
+                                   (B2V_EINVAL) with B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE.  It costs one kernel launch per picture
+                                   (kernel_launches) and coded width x height / 16 bytes per reconstruction buffer. */
 };
 
 /* One encoded frame, the native image of the pixelflux callback result

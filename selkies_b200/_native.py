@@ -19,6 +19,7 @@ B2V_HDR_NONE, B2V_HDR_PIXELFLUX = 0, 1
 B2V_FLAG_SPS_EVERY_IDR, B2V_FLAG_NO_ENCODE, B2V_FLAG_TIMING, B2V_FLAG_DEVICE_TIMER, B2V_FLAG_TIMING_CSC, B2V_FLAG_JPEG = 1, 2, 4, 8, 16, 32
 B2V_FLAG_QUALITY = 64
 B2V_FLAG_DROPPABLE = 128
+B2V_FLAG_WIDE_MOTION = 256
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
 B2V_DT_U8, B2V_DT_F16, B2V_DT_BF16, B2V_DT_F32 = 0, 1, 2, 3
 

@@ -96,7 +96,7 @@ struct Session {
   b2v_settings cfg{};
   int device = 0;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
-  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false;
+  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false, wide_motion = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;
 
   // ingest ring
@@ -196,6 +196,7 @@ int alloc_geometry(Session* s) {
     ec.idr_slice_mbs = s->cfg.idr_slice_mbs;
     ec.quality = s->quality;
     ec.droppable = s->droppable;
+    ec.wide_motion = s->wide_motion;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
     s->lay = encoder_layout(s->enc);
@@ -699,6 +700,9 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if ((cfg->flags & B2V_FLAG_DROPPABLE) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
     return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE layers H.264 pictures: %s codes none",
                 (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+  if ((cfg->flags & B2V_FLAG_WIDE_MOTION) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
+    return fail(B2V_EINVAL, "B2V_FLAG_WIDE_MOTION searches H.264 P pictures: %s codes none",
+                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
   if ((cfg->flags & B2V_FLAG_DROPPABLE) && stripes_active(cfg->stripe_rows, dh))
     return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
                 "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
@@ -713,6 +717,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->jpeg = (cfg->flags & B2V_FLAG_JPEG) != 0;
   s->quality = (cfg->flags & B2V_FLAG_QUALITY) != 0;
   s->droppable = (cfg->flags & B2V_FLAG_DROPPABLE) != 0;
+  s->wide_motion = (cfg->flags & B2V_FLAG_WIDE_MOTION) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;

@@ -69,6 +69,7 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   MbInfo* mbinfo;          // this picture's records (double-buffered: the entropy kernels of picture k read them while picture k+1 is analysed)
   const MbInfo* mbinfo_prev;   // the previous picture's records (temporal motion predictor)
   unsigned long long* me_pub;  // [mbs] anchor macroblocks publish (pic+1) << 32 | new-content flag << 16 | (mvx & 0xff) << 8 | mvy & 0xff as soon as motion estimation is done
+                               // (wide: (mvx & 0xfff) << 20 | flag << 16 | mvy & 0xfff, h264_inter.cu publish_anchor)
   int* me_queue;               // [2 + 2 * mbs] macroblocks k_inter_lean left to k_inter_search: anchor count, rest count, anchors [mbs], rest [mbs]
   int search_blocks;           // k_inter_search grid: its resident capacity on this device
   uint8_t* i4modes;        // [mbs][16] Intra4x4PredMode per block (raster), valid for MB_I4
@@ -96,6 +97,11 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   const unsigned long long* csc_ts;            // device stamps of this picture's CSC launch (or null)
   uint8_t* au;             // AuHeader + access unit
   int* overflow;
+  // B2V_FLAG_WIDE_MOTION (h264_inter.cu k_coarse): 0 without the flag, and then the three pointers are null
+  int wide;
+  uint8_t* dec_cur;        // [ch/4][cw/4] this picture's decimated luma, kept with the reconstruction buffer it writes
+  const uint8_t* dec_ref;  // the reference picture's
+  int* coarse;             // [mbs] at each anchor: its group's coarse vector (dx & 0xffff | dy << 16, decimated samples) or COARSE_NONE
 };
 
 __device__ __forceinline__ int clip3i(int lo, int hi, int v) { return min(hi, max(lo, v)); }

@@ -34,6 +34,9 @@ struct Encoder {
   // picture's, `ref_buf` the last reference picture's (the same one unless the last picture was a non-reference picture).
   uint8_t* recon[3] = {nullptr, nullptr, nullptr};
   int n_recon = 2, last = 0, ref_buf = 0;
+  // B2V_FLAG_WIDE_MOTION: each reconstruction buffer's decimated luma (dec[b] belongs to recon[b]), and the anchors' coarse vectors
+  uint8_t* dec[3] = {nullptr, nullptr, nullptr};
+  int* coarse = nullptr;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
   // of picture k (packing stream) overlaps the analysis of picture k+1 (main stream)
   MbInfo* mbinfo[2] = {nullptr, nullptr};
@@ -190,6 +193,13 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     ECK(cudaMalloc((void**)&e->recon[b], fb));
     ECK(cudaMemset(e->recon[b], 0, fb));
   }
+  if (cfg->wide_motion) {
+    for (int b = 0; b < e->n_recon; b++) {
+      ECK(cudaMalloc((void**)&e->dec[b], fb / 24));      // fb / 24 = (coded_w / 4) x (coded_h / 4)
+      ECK(cudaMemset(e->dec[b], 0, fb / 24));
+    }
+    ECK(cudaMalloc((void**)&e->coarse, mbs * sizeof(int)));
+  }
   for (int b = 0; b < 2; b++) {
     ECK(cudaMalloc((void**)&e->mbinfo[b], mbs * sizeof(MbInfo)));
     ECK(cudaMemset(e->mbinfo[b], 0, mbs * sizeof(MbInfo)));
@@ -269,7 +279,7 @@ void encoder_destroy(Encoder* e) {
   void* ptrs[] = {e->recon[0], e->recon[1], e->recon[2], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
-                  e->q_acc, e->q_done};
+                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -311,6 +321,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.band_rows = e->band_rows; f.n_bands = e->n_bands; f.striped = e->striped; f.param_len_last = e->param_len_last;
   f.band_fn = e->band_fn; f.band_coded = e->band_coded; f.au_data_off = e->au_data_off;
   f.param_sets = e->param_sets; f.param_len = e->param_len; f.csc_ts = p->csc_ts; f.au = p->au; f.overflow = e->overflow;
+  if (e->cfg.wide_motion) { f.wide = 1; f.dec_cur = e->dec[wb]; f.dec_ref = e->dec[e->ref_buf]; f.coarse = e->coarse; }
   int n = 0;
   // Two-stream schedule (no per-stage events requested): ANALYSIS of picture k on `st` (CSC before it, by the caller), ENTROPY
   // coding of picture k (CAVLC, slice build with the rate-control step, pack) on `st_pack`, overlapping
@@ -330,6 +341,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   // picture's colour conversion on `st` overwrites `cur`, the analysis of picture k+2 this reconstruction).
   const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
   if (overlap) cudaStreamWaitEvent(st, e->ev_packed[par], 0);           // pack of picture k-2 (no-op before the first two)
+  if (f.wide) n += launch_coarse(f, st);      // every picture: its decimated plane; P pictures: the coarse vectors
   n += idr ? launch_intra(f, st) : launch_inter(f, st);
   if (e->quality_off) {
     QualityParams q{};

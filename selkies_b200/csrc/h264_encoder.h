@@ -19,6 +19,7 @@ struct EncoderConfig {
   int idr_slice_mbs;       // IDR pictures, whatever slice_rows is: macroblocks per slice inside a row; 0 = default rule (>= 0)
   bool quality;            // B2V_FLAG_QUALITY: k_quality measures every band into the access unit's quality table
   bool droppable;          // B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture (full frame only)
+  bool wide_motion;        // B2V_FLAG_WIDE_MOTION: coarse vectors per anchor group (k_coarse) and windows centred on far candidates
 };
 
 struct EncodeFrameParams {

@@ -56,6 +56,16 @@ constexpr int ME_FRAC_PENALTY_BITS = 4;   // fractional vectors pay 4 extra bits
 constexpr int ME_REFINE_MAX_SAD = 8192;   // no sub-sample refinement of a full-sample match this bad
 constexpr int ME_NEWCONTENT_DY = 2;       // vertical range of the reduced search on new content
 
+// ---- B2V_FLAG_WIDE_MOTION (DESIGN.md §5.3; oracle/h264_wide_ref.c coarse_search, encode_inter_mb_wide) ----
+// A full-sample vector is usable when each component lies in [-255, 255]: with a quarter-sample refinement (+-3/4) every coded
+// component then lies in [-1024, 1023] quarter samples, the range the SPS asserts (VUI log2_max_mv_length_* = 10), inside Table A-1's
+// MaxVmvR of every level it writes.
+constexpr int MV_MAX_FULL = 255;
+constexpr int WM_DX = 32, WM_DY = 64;      // coarse search: dx in [-32, 31], dy in [-64, 63] decimated samples (x4 luma samples)
+constexpr int COARSE_NONE = 0x7fffffff;
+constexpr int WM_MVD_BITS = 48;            // header budget of a P macroblock in a wide-motion picture: 48 more bits for two mvd of up to +-2046
+__device__ __forceinline__ bool mv_ok(int kx, int ky) { return kx >= -MV_MAX_FULL && kx <= MV_MAX_FULL && ky >= -MV_MAX_FULL && ky <= MV_MAX_FULL; }
+
 // Table 8-12 as data: every fractional position is one plane sample or the rounded average of two.
 // entry = p1 | dx1<<2 | dy1<<3 | p2<<4 | dx2<<7 | dy2<<8, planes 0 G (full sample), 1 b, 2 h, 3 j, p2 = 4: none
 __device__ const uint16_t subpel_tab[16] = {
@@ -109,8 +119,10 @@ __host__ __device__ constexpr int se_bits_c(int v) {
 // Full-sample search over dx in [-16,15] (one candidate column per lane) and dy in [-DYR,DYR]: every window row is byte-aligned once
 // per lane with funnel shifts and feeds the (row, dy) pairs it belongs to; 2*DYR+1 SAD accumulators live in registers.  Returns the
 // warp-wide minimum of cost << 11 | candidate index.  DYR = 16 is the exhaustive search, a small DYR the reduced one for new content.
-template <int DYR>
-__device__ __forceinline__ uint32_t search_rows(const InterSm& sm, int lane, int lambda) {
+// WIDE: the window is centred on the full-sample vector (ox, oy); costs are those of the real vectors and candidates outside
+// MV_MAX_FULL are skipped.
+template <int DYR, bool WIDE = false>
+__device__ __forceinline__ uint32_t search_rows(const InterSm& sm, int lane, int lambda, int ox = 0, int oy = 0) {
   const MbTile& t = sm.t;
   uint32_t c[16][4];
 #pragma unroll
@@ -135,13 +147,13 @@ __device__ __forceinline__ uint32_t search_rows(const InterSm& sm, int lane, int
         acc[k] = sad4acc(c[r][0], a0, sad4acc(c[r][1], a1, sad4acc(c[r][2], a2, sad4acc(c[r][3], a3, acc[k]))));
     }
   }
-  const int bits_x = se_bits_c(4 * (lane - 16));
+  const int bits_x = WIDE ? se_bits_dev(4 * (ox + lane - 16)) : se_bits_c(4 * (lane - 16));
   uint32_t best = 0xffffffffu;
 #pragma unroll
   for (int k = 0; k < N; k++) {
     const int dyi = k + Y0;                     // dy + 16
-    const uint32_t cost = acc[k] + (uint32_t)(lambda * (bits_x + se_bits_c(4 * (dyi - 16))));
-    best = min(best, (cost << 11) | (uint32_t)(dyi * 32 + lane));
+    const uint32_t cost = acc[k] + (uint32_t)(lambda * (bits_x + (WIDE ? se_bits_dev(4 * (oy + dyi - 16)) : se_bits_c(4 * (dyi - 16)))));
+    if (!WIDE || mv_ok(ox + lane - 16, oy + dyi - 16)) best = min(best, (cost << 11) | (uint32_t)(dyi * 32 + lane));
   }
   return __reduce_min_sync(FULL, best);
 }
@@ -204,22 +216,30 @@ __device__ __forceinline__ bool full_sample_candidate(int mvx, int mvy, int& kx,
 // would otherwise search only to find (0,0) again), and the 24 rows x 8 words of the window from (ra, wa) on that its test, a refinement
 // around it and its prediction touch: rows [13+cdy, 36+cdy] and bytes [13+cdx, 34+cdx] cover the 3x3 test (rows 15+cdy..32+cdy), the
 // 6-tap support (-3..+18) and the prediction, clamped so that they stay inside the window.  `prev`: as start_mb scaled it.
-struct TemporalPred { int cdx, cdy, ra, wa; bool try_pred; };
+// WIDE: a predictor outside the co-located window's test range but within MV_MAX_FULL is tested in the window centred on (wx, wy) =
+// (its x rounded down to a multiple of 4, so that the window's rows stay word-aligned, its y); (cdx, cdy) is relative to that centre.
+struct TemporalPred { int cdx, cdy, ra, wa; bool try_pred; int wx, wy; };
+template <bool WIDE>
 __device__ __forceinline__ TemporalPred temporal_predictor(const MbInfo& prev) {
   TemporalPred tp;
-  tp.try_pred = full_sample_candidate(prev.mvx, prev.mvy, tp.cdx, tp.cdy) && prev.type == MB_P16;
+  tp.wx = 0; tp.wy = 0;
+  bool in = full_sample_candidate(prev.mvx, prev.mvy, tp.cdx, tp.cdy);
+  if (WIDE && !in && mv_ok(tp.cdx, tp.cdy)) { tp.wx = tp.cdx & ~3; tp.wy = tp.cdy; tp.cdx -= tp.wx; tp.cdy = 0; in = true; }
+  tp.try_pred = in && prev.type == MB_P16;
   tp.ra = min(max(13 + tp.cdy, 0), WIN_ROWS - PW_ROWS); tp.wa = min(max((13 + tp.cdx) >> 2, 0), WIN_WORDS - PW_WORDS);
   return tp;
 }
+// the 48 columns of the window centred on (wx, *) lie inside the picture (MbPos::inside for wx = 0)
+__device__ __forceinline__ bool window_inside(const FrameCtx& f, const MbPos& p, int wx) { return p.mbx * 16 - 16 + wx >= 0 && p.mbx * 16 + 32 + wx <= f.cw; }
 // Those 24 rows x 8 words (a macroblock whose window lies inside the picture) into `dst`: the whole window or k_inter_lean's dense
 // copy of that part, so that both passes test the predictor on the same words at the same window coordinates.
 __device__ __forceinline__ void stage_pred_window(const FrameCtx& f, const WinView& dst, int lane, const MbPos& p, int ylo, int yhi, const TemporalPred& tp) {
-  const uint32_t* base = reinterpret_cast<const uint32_t*>(f.ref + p.mbx * 16 - 16);
+  const uint32_t* base = reinterpret_cast<const uint32_t*>(f.ref + p.mbx * 16 - 16 + tp.wx);
   uint32_t v[6];
 #pragma unroll
   for (int k = 0; k < 6; k++) {
     const int idx = lane + 32 * k;
-    v[k] = __ldg(base + (size_t)clip3i(ylo, yhi, p.mby * 16 - 16 + tp.ra + (idx >> 3)) * (f.cw >> 2) + tp.wa + (idx & 7));
+    v[k] = __ldg(base + (size_t)clip3i(ylo, yhi, p.mby * 16 - 16 + tp.wy + tp.ra + (idx >> 3)) * (f.cw >> 2) + tp.wa + (idx & 7));
   }
 #pragma unroll
   for (int k = 0; k < 6; k++) {
@@ -234,7 +254,8 @@ __device__ __forceinline__ int key_sad(uint32_t key, int lambda, int mvx, int mv
 
 // Candidate (kx,ky), full samples, window staged around it: true (and `best` = its key) when its SAD is within 4x the noise
 // threshold AND it is a strict local minimum of the cost over its 8 full-sample neighbours AND it costs no more than the zero vector.
-__device__ __forceinline__ bool test_candidate(const WinView& w, const MbTile& t, int lane, int kx, int ky, int lambda, int sad0, uint32_t& best) {
+// (kx, ky) relative to the window's centre (ox, oy); costs are those of the real vector.
+__device__ __forceinline__ bool test_candidate(const WinView& w, const MbTile& t, int lane, int kx, int ky, int lambda, int sad0, uint32_t& best, int ox = 0, int oy = 0) {
   const int r8 = lane >> 1, c8 = (lane & 1) * 8;
   const uint32_t c0 = *reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8]), c1 = *reinterpret_cast<const uint32_t*>(&t.cur_y[r8][c8 + 4]);
   uint32_t kc = 0, kmin = 0xffffffffu;
@@ -247,13 +268,13 @@ __device__ __forceinline__ bool test_candidate(const WinView& w, const MbTile& t
       const int sh = (bx & 3) * 8;
       const uint32_t a0 = __funnelshift_r(wr[0], wr[1], sh), a1 = __funnelshift_r(wr[1], wr[2], sh);
       const int sad = __reduce_add_sync(FULL, (int)sad4acc(c0, a0, sad4acc(c1, a1, 0u)));
-      const uint32_t cost = (uint32_t)(sad + lambda * (se_bits_dev(4 * (kx + i)) + se_bits_dev(4 * (ky + j))));
+      const uint32_t cost = (uint32_t)(sad + lambda * (se_bits_dev(4 * (ox + kx + i)) + se_bits_dev(4 * (oy + ky + j))));
       const uint32_t key = (cost << 11) | (uint32_t)((ky + j + 16) * 32 + (kx + i + 16));
       if (i == 0 && j == 0) kc = key; else kmin = min(kmin, key);
     }
   }
   const uint32_t key0 = ((uint32_t)(sad0 + 2 * lambda) << 11) | (uint32_t)(16 * 32 + 16);   // ... and it must not cost more than the zero vector
-  if (key_sad(kc, lambda, 4 * kx, 4 * ky) <= ME_PRED_SAD_FACTOR * ME_EARLY_SAD_PER_LAMBDA * lambda && kc < kmin && kc <= key0) { best = kc; return true; }
+  if (key_sad(kc, lambda, 4 * (ox + kx), 4 * (oy + ky)) <= ME_PRED_SAD_FACTOR * ME_EARLY_SAD_PER_LAMBDA * lambda && kc < kmin && kc <= key0) { best = kc; return true; }
   return false;
 }
 
@@ -267,13 +288,17 @@ __device__ __forceinline__ void full_sample_pred(const WinView& w, MbTile& t, in
   *reinterpret_cast<uint32_t*>(&t.pred_y[r8][c8 + 4]) = __funnelshift_r(wr[1], wr[2], sh);
 }
 
-// an anchor's vector for the rest of its group: one 8-byte store, tag and vector together
+// an anchor's vector for the rest of its group: one 8-byte store, tag and vector together.  WIDE: 12 bits per component,
+// (mvx & 0xfff) << 20 | new-content flag << 16 | mvy & 0xfff
+template <bool WIDE>
 __device__ __forceinline__ void publish_anchor(const FrameCtx& f, int mb, int sad_int, int mvx, int mvy) {
-  f.me_pub[mb] = ((unsigned long long)((uint32_t)f.pic + 1u) << 32) | (sad_int >= ME_REFINE_MAX_SAD ? 0x10000u : 0u) | (uint32_t)((mvx & 0xff) << 8) | (uint32_t)(mvy & 0xff);
+  if (WIDE) f.me_pub[mb] = ((unsigned long long)((uint32_t)f.pic + 1u) << 32) | (sad_int >= ME_REFINE_MAX_SAD ? 0x10000u : 0u) | ((uint32_t)(mvx & 0xfff) << 20) | (uint32_t)(mvy & 0xfff);
+  else f.me_pub[mb] = ((unsigned long long)((uint32_t)f.pic + 1u) << 32) | (sad_int >= ME_REFINE_MAX_SAD ? 0x10000u : 0u) | (uint32_t)((mvx & 0xff) << 8) | (uint32_t)(mvy & 0xff);
 }
 
 // chroma prediction, residual, reconstruction and the macroblock's record; the luma prediction is already in t.pred_y.
 // uv_coloc: this lane's word of the co-located chroma reference.
+template <bool WIDE>
 __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc) {
   const size_t ysz = (size_t)f.cw * f.ch;
   const uint8_t* __restrict__ ref_uv = f.ref + ysz;
@@ -315,7 +340,7 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
   const uint32_t mv = (uint32_t)(mvx & 0xffff) | ((uint32_t)mvy << 16);
   int luma_bits, chroma_bits;
   int cbp = transform_mb<false>(t, lane, qp, f.coef + (size_t)mb * COEF_BLOCKS * 16, f.nnz + (size_t)mb * 32, luma_bits, chroma_bits);
-  if (48 + luma_bits + chroma_bits > MB_BITS_LIMIT) { apply_pcm(t, lane, f.nnz + (size_t)mb * 32); cbp = -1; }   // A.3.1: send raw
+  if ((WIDE ? 48 + WM_MVD_BITS : 48) + luma_bits + chroma_bits > MB_BITS_LIMIT) { apply_pcm(t, lane, f.nnz + (size_t)mb * 32); cbp = -1; }   // A.3.1: send raw
   __syncwarp();
   {
     const int ry = mb / f.mbw;
@@ -332,7 +357,7 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 // a temporal-predictor hit that needs no refinement are finished here; every other one goes into a queue for k_inter_search —
 // anchors into the anchor queue, the rest into the other.  No search and no 48 x 48 window: the registers and shared memory of
 // the search do not cap the occupancy of the common case.
-template <bool SCALE>
+template <bool SCALE, bool WIDE>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) {
   __shared__ __align__(16) LeanSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -354,17 +379,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
   } else {
     // the temporal predictor on the part of the window around it.  A picture-edge macroblock, which needs per-sample clamping, is
     // deferred.
-    const TemporalPred tp = temporal_predictor(s.prev);
+    const TemporalPred tp = temporal_predictor<WIDE>(s.prev);
     bool hit = false;
-    if (tp.try_pred && p.inside) {
+    if (tp.try_pred && (WIDE ? window_inside(f, p, tp.wx) : p.inside)) {
       const WinView w{&sm.pw[0][0], PW_WORDS, tp.ra, tp.wa};
       stage_pred_window(f, w, lane, p, ylo, yhi, tp);
       uint32_t best;
       // a hit whose previous vector was fractional is refined: k_inter_search does that
-      hit = test_candidate(w, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best) && ((s.prev.mvx | s.prev.mvy) & 3) == 0;
+      hit = test_candidate(w, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best, tp.wx, tp.wy) && ((s.prev.mvx | s.prev.mvy) & 3) == 0;
       if (hit) {
         full_sample_pred(w, t, lane, 16 + tp.cdx, 16 + tp.cdy);
-        mvx = 4 * tp.cdx; mvy = 4 * tp.cdy;
+        mvx = 4 * (tp.wx + tp.cdx); mvy = 4 * (tp.wy + tp.cdy);
         sad_int = key_sad(best, lambda, mvx, mvy);
       }
     }
@@ -376,14 +401,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
       return;
     }
   }
-  if (p.anchor && lane == 0) publish_anchor(f, m, sad_int, mvx, mvy);
-  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
+  if (p.anchor && lane == 0) publish_anchor<WIDE>(f, m, sad_int, mvx, mvy);
+  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
 // One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
 // previous picture's records are not written during the analysis of a picture).  Its co-located block failed the zero-motion test
 // there and fails it again here, so that test is not repeated; its temporal predictor fails, or hits, as it did there.
-template <bool SCALE>
+// WIDE (B2V_FLAG_WIDE_MOTION): sm.win may hold the window centred on a full-sample vector (wx, wy) other than (0, 0) — a temporal or
+// anchor predictor outside the co-located window's test range, or an anchor's coarse vector x 4; candidate indices and (dx, dy) are
+// relative to that centre, costs are those of the real vector.
+template <bool SCALE, bool WIDE>
 __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int lane, const MbPos& p) {
   const int mb = p.mb, x0 = p.mbx * 16, y0 = p.mby * 16;
   const bool anchor = p.anchor;
@@ -400,10 +428,34 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   // ---- the reference.  A macroblock that carries a vector from the previous picture first gets only what the temporal-predictor
   // test, the refinement around it and the final prediction can touch — 24 rows x 8 words around the predicted position instead of
   // the 48 x 12 window; the rest follows only if the predictor is rejected and the search has to run.
-  const TemporalPred tp = temporal_predictor(s.prev);
-  bool window_complete = false;
+  const TemporalPred tp = temporal_predictor<WIDE>(s.prev);
+  bool window_complete = false;     // sm.win holds the whole co-located window
+  int wx = 0, wy = 0;               // WIDE: the centre of the window sm.win holds
+  // WIDE: the whole window centred on (cx, cy), centre block included; (0, 0) restores the co-located window after another
+  auto stage_at = [&](int cx, int cy) {
+    if (window_inside(f, p, cx)) {
+      const uint32_t* base = reinterpret_cast<const uint32_t*>(ref_y + x0 - 16 + cx);
+      for (int i = lane; i < WIN_ROWS * WIN_WORDS; i += 32) {
+        const int row = i / WIN_WORDS, w = i - row * WIN_WORDS;
+        sm.win[row][w] = __ldg(base + (size_t)clip3i(ylo, yhi, y0 - 16 + cy + row) * (f.cw >> 2) + w);
+      }
+    } else {
+      for (int i = lane; i < WIN_ROWS * WIN_WORDS; i += 32) {
+        const int row = i / WIN_WORDS, w = i - row * WIN_WORDS;
+        const uint8_t* rr = ref_y + (size_t)clip3i(ylo, yhi, y0 - 16 + cy + row) * f.cw;
+        uint32_t v = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) v |= (uint32_t)__ldg(rr + clip3i(0, f.cw - 1, x0 - 16 + cx + w * 4 + k)) << (8 * k);
+        sm.win[row][w] = v;
+      }
+    }
+    wx = cx; wy = cy;
+    window_complete = (cx | cy) == 0;
+    __syncwarp();
+  };
   auto stage_window = [&]() {
-    if (p.inside) {   // 512 more words: lanes 0..23 take (row pair j, word) = two rows of 12 words per step — no index arithmetic
+    if (WIDE && (wx | wy)) stage_at(0, 0);
+    else if (p.inside) {   // 512 more words: lanes 0..23 take (row pair j, word) = two rows of 12 words per step — no index arithmetic
       // beyond an add per step —, every load issued before the first shared-memory store
       uint32_t v[24];
       const int half = lane >= 12 ? 1 : 0, w = lane - 12 * half;
@@ -437,24 +489,30 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
     __syncwarp();
   };
   // k_inter_lean did not test the predictor of a picture-edge macroblock: it is tested here, on the full clamped window
-  if (p.inside && tp.try_pred) stage_pred_window(f, win, lane, p, ylo, yhi, tp); else stage_window();
+  if (WIDE && tp.try_pred && (tp.wx | tp.wy)) stage_at(tp.wx, tp.wy);
+  else if (p.inside && tp.try_pred) stage_pred_window(f, win, lane, p, ylo, yhi, tp); else stage_window();
   // ---- temporal predictor; quarter-sample refinement then runs as after a search ----
   uint32_t best = 0xffffffffu;
   bool pred_frac = false, reduced = false;
-  if (tp.try_pred && test_candidate(win, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best)) pred_frac = ((s.prev.mvx | s.prev.mvy) & 3) != 0;
+  if (tp.try_pred && test_candidate(win, t, lane, tp.cdx, tp.cdy, lambda, s.sad0, best, tp.wx, tp.wy)) pred_frac = ((s.prev.mvx | s.prev.mvy) & 3) != 0;
   // ---- anchor predictor (oracle/h264_ref.c encode_inter_mb): the temporal predictor failed (or there was none) — motion that
   // STARTS in this picture.  Instead of one exhaustive search per macroblock, try what this group's anchor has found. ----
   if (best == 0xffffffffu && !anchor) {
-    if (!window_complete) stage_window();       // any candidate position may be tried; needed by the search anyway if it is rejected
     // written by k_inter_lean or by the anchor pass, both earlier in stream order.  The tag is always there; were it missing, the
     // macroblock would run the exhaustive search and the stream would differ from the oracle's.
     const unsigned long long v = f.me_pub[(size_t)p.ay * f.mbw + p.ax];
     const bool have = (uint32_t)(v >> 32) == (uint32_t)f.pic + 1u;
-    const int amvx = (int)(int8_t)(v >> 8), amvy = (int)(int8_t)v;
+    const int amvx = WIDE ? (int)(uint32_t)v >> 20 : (int)(int8_t)(v >> 8), amvy = WIDE ? (int)((uint32_t)v << 20) >> 20 : (int)(int8_t)v;
     int kx, ky;
-    const bool in_window = full_sample_candidate(amvx, amvy, kx, ky);
-    const bool zero_again = (kx | ky) == 0 && tp.try_pred && (tp.cdx | tp.cdy) == 0;      // the zero vector is not tested twice
-    if (have && !zero_again && in_window && test_candidate(win, t, lane, kx, ky, lambda, s.sad0, best)) pred_frac = ((amvx | amvy) & 3) != 0;
+    bool in_window = full_sample_candidate(amvx, amvy, kx, ky);
+    int ox = 0, oy = 0;
+    if (WIDE && have && !in_window && mv_ok(kx, ky)) {     // far: the window centred on it, as for a far temporal predictor
+      ox = kx & ~3; oy = ky; kx -= ox; ky -= oy; in_window = true;
+      stage_at(ox, oy);
+    } else if (!window_complete) stage_window();   // any candidate position may be tried; needed by the search anyway if it is rejected
+    // (ox, oy) = (0, 0) for the zero vector: in a shifted window the test below cannot be the zero vector's
+    const bool zero_again = ((ox + kx) | (oy + ky)) == 0 && tp.try_pred && ((tp.wx + tp.cdx) | (tp.wy + tp.cdy)) == 0;      // the zero vector is not tested twice
+    if (have && !zero_again && in_window && test_candidate(win, t, lane, kx, ky, lambda, s.sad0, best, ox, oy)) pred_frac = ((amvx | amvy) & 3) != 0;
     // new content: the anchor's exhaustive search found nothing (bit 16) and the co-located block is as far off — the search
     // shrinks to the rows around dy = 0: picking the least bad of 1089 noise candidates buys hardly more than picking it of 160
     else reduced = have && ((v >> 16) & 1) != 0 && s.sad0 >= ME_REFINE_MAX_SAD;
@@ -462,13 +520,26 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   const bool searched = best == 0xffffffffu;
   if (searched && !window_complete) stage_window();          // predictor rejected: the search needs the whole window
   if (searched) best = reduced ? search_rows<ME_NEWCONTENT_DY>(sm, lane, lambda) : search_rows<16>(sm, lane, lambda);
+  // WIDE, an anchor that searched: the same search in the window centred on its group's coarse vector x 4 (k_coarse), unless the
+  // co-located search covered that vector with the 4 samples either way one decimated sample spans.  The cheaper result by true cost
+  // wins, the co-located window on equal cost (keys of two windows are compared by cost alone: their indices are window-relative).
+  if (WIDE && searched && anchor) {
+    const int cv = f.coarse[mb];
+    const int cx = 4 * (int)(int16_t)(cv & 0xffff), cy = 4 * (cv >> 16);
+    if (cv != COARSE_NONE && (cx < -12 || cx > 11 || cy < -12 || cy > 12)) {
+      const uint32_t best0 = best;
+      stage_at(cx, cy);
+      const uint32_t best1 = search_rows<16, true>(sm, lane, lambda, cx, cy);
+      if ((best1 >> 11) < (best0 >> 11)) best = best1; else stage_window();
+    }
+  }
   const int dyi = (best & 2047) >> 5, dxi = best & 31, dx = dxi - 16, dy = dyi - 16;
 
   // ---- quarter-sample refinement (DESIGN.md §5.3; oracle/h264_ref.c encode_inter_mb) ---------------------------------
-  int mvx = 4 * dx, mvy = 4 * dy;
+  int mvx = 4 * (wx + dx), mvy = 4 * (wy + dy);
   // refine only inside the window (6-tap support [-3,+18]) and when the full-sample match is not already within the
   // quantisation noise of this QP (same threshold as the zero-motion early termination)
-  const int sad_int = key_sad(best, lambda, 4 * dx, 4 * dy);
+  const int sad_int = key_sad(best, lambda, mvx, mvy);
   // a predictor hit whose previous vector was full-sample is not refined again: the previous refinement already preferred it
   // ... and not when the full-sample match is hopeless (mean absolute difference >= 32 per sample: new content, nothing to polish —
   // the refinement is a third of the work of a searched macroblock and bought 0 % bits on such pictures)
@@ -518,7 +589,7 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
         int sad = (int)sad4acc(cur4.x, pr[0], sad4acc(cur4.y, pr[1], sad4acc(cur4.z, pr[2], sad4acc(cur4.w, pr[3], 0u))));
         sad += __shfl_xor_sync(FULL, sad, 1); sad += __shfl_xor_sync(FULL, sad, 2);
         sad += __shfl_xor_sync(FULL, sad, 4); sad += __shfl_xor_sync(FULL, sad, 8);
-        const uint32_t cost = (uint32_t)(sad + lambda * (se_bits_dev(4 * dx + qx) + se_bits_dev(4 * dy + qy) + (((qx | qy) & 3) ? ME_FRAC_PENALTY_BITS : 0)));
+        const uint32_t cost = (uint32_t)(sad + lambda * (se_bits_dev(4 * (wx + dx) + qx) + se_bits_dev(4 * (wy + dy) + qy) + (((qx | qy) & 3) ? ME_FRAC_PENALTY_BITS : 0)));
         uint32_t key = (cost << 4) | (uint32_t)(cand + 1);
         key = min(key, __shfl_xor_sync(FULL, key, 16));
         bestk = min(bestk, key);
@@ -538,21 +609,21 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
       *reinterpret_cast<uint4*>(&t.pred_y[lane][0]) = make_uint4(pr[0], pr[1], pr[2], pr[3]);
     }
   }
-  if (anchor && lane == 0) publish_anchor(f, mb, sad_int, mvx, mvy);
+  if (anchor && lane == 0) publish_anchor<WIDE>(f, mb, sad_int, mvx, mvy);
   if (!refine) full_sample_pred(win, t, lane, dxi, dyi);
-  finish_mb(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
+  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
 // Passes B and C: the queue k_inter_lean filled (0: anchors, 1: the rest), walked by a grid of the kernel's resident capacity.  No
 // decision here depends on another entry of the same queue, so the order inside a queue does not matter.
-template <bool SCALE>
+template <bool SCALE, bool WIDE>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search(FrameCtx f, int queue) {
   __shared__ __align__(16) InterSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = f.me_queue[queue];
   const int* q = f.me_queue + 2 + (size_t)queue * f.mbw * f.mbh;
   for (int i = blockIdx.x * WARPS_PER_BLOCK + warp; i < n; i += gridDim.x * WARPS_PER_BLOCK) {
-    search_mb<SCALE>(f, sm_all[warp], lane, mb_pos(f, q[i]));
+    search_mb<SCALE, WIDE>(f, sm_all[warp], lane, mb_pos(f, q[i]));
     __syncwarp();
   }
 }
@@ -561,7 +632,7 @@ cudaError_t inter_search_grid(int* blocks) {
   int dev = 0, sms = 0, per_sm = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search<false>, 32 * WARPS_PER_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search<false, false>, 32 * WARPS_PER_BLOCK, 0);
   *blocks = sms * per_sm;
   return e;
 }
@@ -570,16 +641,128 @@ int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
   const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  if (f.ref_dist == f.prev_ref_dist) {      // every picture without B2V_FLAG_DROPPABLE
-    k_inter_lean<false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    k_inter_search<false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
-    k_inter_search<false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+  if (f.wide) {                             // B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream)
+    if (f.ref_dist == f.prev_ref_dist) {
+      k_inter_lean<false, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    } else {
+      k_inter_lean<true, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+      k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+      k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    }
+  } else if (f.ref_dist == f.prev_ref_dist) {      // every picture without B2V_FLAG_DROPPABLE
+    k_inter_lean<false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
+    k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
   } else {
-    k_inter_lean<true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    k_inter_search<true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-    k_inter_search<true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    k_inter_lean<true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+    k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
   }
   return 3;
+}
+
+// ---- k_coarse (B2V_FLAG_WIDE_MOTION): one block per anchor group (4 x 4 macroblocks, counted inside each band), every picture ----
+//  1. the group's samples of this picture's decimated luma (each the rounded mean of a 4x4 block of the coded luma) into f.dec_cur,
+//     the plane kept with the reconstruction buffer this picture writes (an IDR picture stops here);
+//  2. the anchor's co-located SAD; at or below the early-termination threshold the group gets no coarse vector;
+//  3. the group's decimated block (up to 16 x 16) against the reference picture's plane at dx in [-32, 31], dy in [-64, 63], every
+//     position inside the picture and the band: 256 threads, each a column dx of 16 consecutive dy twice, 16 SADs in registers fed
+//     row by row with VABSDIFF4 as search_rows does; the minimum of (SAD, |dx| + |dy|, dy, dx) as one 37-bit key.
+// oracle/h264_wide_ref.c decimate, coarse_search.
+constexpr int CO_ROWS = 2 * WM_DY + 16, CO_WORDS = (2 * WM_DX + 16) / 4 + 1;   // reference tile: decimated rows from Y0 - WM_DY, words from X0 - WM_DX (zero outside)
+__global__ void __launch_bounds__(256) k_coarse(FrameCtx f) {
+  __shared__ __align__(16) uint32_t tile[CO_ROWS][CO_WORDS];
+  __shared__ __align__(16) uint8_t cur[16][16];
+  __shared__ unsigned long long s_best;
+  __shared__ int s_sad0;
+  const int tid = threadIdx.x;
+  const int gpb = (f.band_rows + 3) >> 2;                      // group rows per band
+  const int band = blockIdx.y / gpb;
+  const int br0 = band * f.band_rows, br1 = min(f.mbh, br0 + f.band_rows), gy0 = br0 + 4 * (blockIdx.y - band * gpb);
+  if (gy0 >= br1) return;
+  const int gx0 = 4 * blockIdx.x, gx1 = min(gx0 + 4, f.mbw), gy1 = min(gy0 + 4, br1);
+  const int dw = f.cw >> 2, X0 = 4 * gx0, Y0 = 4 * gy0, W = 4 * (gx1 - gx0), H = 4 * (gy1 - gy0);
+  {
+    const int r = tid >> 4, c = tid & 15;
+    uint32_t d = 0;
+    if (r < H && c < W) {
+      const uint8_t* src = f.cur + (size_t)(4 * (Y0 + r)) * f.cw + 4 * (X0 + c);
+      uint32_t sum = 0;
+#pragma unroll
+      for (int k = 0; k < 4; k++) sum += __vsadu4(*reinterpret_cast<const uint32_t*>(src + (size_t)k * f.cw), 0u);
+      d = (sum + 8) >> 4;
+      f.dec_cur[(size_t)(Y0 + r) * dw + X0 + c] = (uint8_t)d;
+    }
+    cur[r][c] = (uint8_t)d;                                    // zero outside the group: those bytes are masked below
+  }
+  if (f.idr) return;
+  const int ax = min(gx0 + 1, f.mbw - 1), ay = min(gy0 + 1, br1 - 1), amb = ay * f.mbw + ax;
+  if (tid == 0) { s_sad0 = 0; s_best = ~0ull; }
+  __syncthreads();
+  {
+    const size_t o = (size_t)(ay * 16 + (tid >> 4)) * f.cw + ax * 16 + (tid & 15);
+    const int d = __reduce_add_sync(FULL, abs((int)f.cur[o] - (int)f.ref[o]));
+    if ((tid & 31) == 0) atomicAdd(&s_sad0, d);
+  }
+  __syncthreads();
+  if (s_sad0 <= ME_EARLY_SAD_PER_LAMBDA * me_lambda[frame_qp(f)]) { if (tid == 0) f.coarse[amb] = COARSE_NONE; return; }
+  const int ylo = 4 * br0, yhi = 4 * br1;                      // decimated rows of the band: [ylo, yhi)
+  for (int i = tid; i < CO_ROWS * CO_WORDS; i += 256) {
+    const int row = i / CO_WORDS, w = i - row * CO_WORDS;
+    const int y = Y0 - WM_DY + row, x = X0 - WM_DX + 4 * w;          // x and dw are multiples of 4: a word lies inside or outside whole
+    tile[row][w] = y >= ylo && y < yhi && x >= 0 && x < dw ? *reinterpret_cast<const uint32_t*>(f.dec_ref + (size_t)y * dw + x) : 0u;
+  }
+  __syncthreads();
+  const int dxi = tid & 63, dx = dxi - WM_DX, nw = W >> 2, wi = dxi >> 2, sh = (dxi & 3) * 8;
+  uint32_t c[16][4];
+#pragma unroll
+  for (int r = 0; r < 16; r++) {
+    const uint4 v = *reinterpret_cast<const uint4*>(&cur[r][0]);
+    c[r][0] = v.x; c[r][1] = v.y; c[r][2] = v.z; c[r][3] = v.w;
+  }
+  const bool x_ok = X0 + dx >= 0 && X0 + dx + W <= dw;
+  unsigned long long best = ~0ull;
+#pragma unroll 1
+  for (int chunk = tid >> 6; chunk < 8; chunk += 4) {
+    const int dy0 = -WM_DY + 16 * chunk;                       // this item: dy in [dy0, dy0 + 15], tile rows dy0 + WM_DY + k + r
+    uint32_t acc[16];
+#pragma unroll
+    for (int k = 0; k < 16; k++) acc[k] = 0;
+#pragma unroll
+    for (int y = 0; y < 31; y++) {
+      const uint32_t* wr = &tile[dy0 + WM_DY + y][wi];
+      const uint32_t w0 = wr[0], w1 = wr[1], w2 = wr[2], w3 = wr[3], w4 = wr[4];
+      const uint32_t a0 = __funnelshift_r(w0, w1, sh), a1 = nw > 1 ? __funnelshift_r(w1, w2, sh) : 0u;
+      const uint32_t a2 = nw > 2 ? __funnelshift_r(w2, w3, sh) : 0u, a3 = nw > 3 ? __funnelshift_r(w3, w4, sh) : 0u;
+#pragma unroll
+      for (int r = 0; r < 16; r++) {
+        const int k = y - r;
+        if (k >= 0 && k < 16 && r < H) acc[k] = sad4acc(c[r][0], a0, sad4acc(c[r][1], a1, sad4acc(c[r][2], a2, sad4acc(c[r][3], a3, acc[k]))));
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 16; k++) {
+      const int dy = dy0 + k;
+      const unsigned long long key = (unsigned long long)acc[k] << 20 | (unsigned long long)(abs(dx) + abs(dy)) << 13 | (unsigned long long)(dy + 64) << 6 | (unsigned long long)dxi;
+      if (x_ok && Y0 + dy >= ylo && Y0 + dy + H <= yhi) best = min(best, key);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(FULL, best, o));
+  if ((tid & 31) == 0) atomicMin(&s_best, best);
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned long long b = s_best;
+    f.coarse[amb] = b == ~0ull ? COARSE_NONE : (int)(((int)(b & 63) - 32) & 0xffff) | (int)((unsigned)((int)((b >> 6) & 127) - 64) << 16);
+  }
+}
+
+int launch_coarse(const FrameCtx& f, cudaStream_t st) {
+  const dim3 grid((f.mbw + 3) / 4, f.n_bands * ((f.band_rows + 3) / 4));
+  k_coarse<<<grid, 256, 0, st>>>(f);
+  return 1;
 }
 
 }  // namespace b2v

@@ -77,6 +77,7 @@ class CaptureSettings:
         self.output_height = 0
         self.quality_metrics = False             # measure every delivered record on the GPU: results carry `quality` (H.264 only)
         self.h264_droppable_frames = False       # every second P picture a non-reference picture a lagging consumer may drop (full frame only)
+        self.h264_wide_motion = False            # motion vectors up to 128 px across and 256 px down/up for fast scrolls and drags (H.264 only)
 
 
 class StripeCallback:
@@ -258,6 +259,9 @@ class ScreenCapture:
             if s.droppable and (jpeg or not bool(getattr(settings, "h264_fullframe", True))):
                 raise ValueError("h264_droppable_frames needs full-frame H.264 (output_mode 1, h264_fullframe True): "
                                  "JPEG has no reference pictures and every H.264 stripe is a stream of its own")
+            s.wide_motion = bool(getattr(settings, "h264_wide_motion", False))
+            if s.wide_motion and jpeg:
+                raise ValueError("h264_wide_motion needs H.264 (output_mode 1): JPEG has no motion search")
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)
