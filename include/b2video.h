@@ -122,7 +122,7 @@ enum {
                                    (stripe_rows > 0 and less than the picture's macroblock rows), and b2v_set_resolution rejects a
                                    size at which stripe_rows would stripe.  It costs a third reconstruction buffer (coded
                                    width x height x 1.5 bytes). */
-  B2V_FLAG_WIDE_MOTION   = 256  /* find motion vectors beyond the +-16 samples of the P-picture search, for fast scrolls and window
+  B2V_FLAG_WIDE_MOTION   = 256, /* find motion vectors beyond the +-16 samples of the P-picture search, for fast scrolls and window
                                    drags.  Every picture gets a 1/4 x 1/4 decimated luma plane; in every 4 x 4-macroblock group
                                    whose anchor's co-located block changed, that block is searched in the reference picture's
                                    plane over +-128 samples horizontally and +-256 vertically, inside the picture and the band.
@@ -133,6 +133,23 @@ enum {
                                    scaling, B2V_FLAG_DROPPABLE and B2V_FLAG_QUALITY.  H.264 only: b2v_create rejects it
                                    (B2V_EINVAL) with B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE.  It costs one kernel launch per picture
                                    (kernel_launches) and coded width x height / 16 bytes per reconstruction buffer. */
+  B2V_FLAG_LONG_TERM_REF = 512  /* keep one earlier picture as a long-term reference, so that content that comes back (a popup or
+                                   menu closing, a switch back to an application, a window dragged off the desktop) is predicted
+                                   from it instead of coded as new.  The SPS says max_num_ref_frames 2 and max_dec_frame_buffering 2.
+                                   P picture k marks picture k-1 long-term (adaptive dec_ref_pic_marking: MMCO 4, MMCO 3 with
+                                   long_term_frame_idx 0, preceded by MMCO 1 on the picture two back while no long-term picture
+                                   exists) when changed(k) >= max(ceil(macroblocks / 64), 8 x changed(k-1)), changed being the count
+                                   of macroblocks whose co-located block fails the zero-motion exit (an IDR counts all); every other
+                                   P picture uses the sliding window.  The GPU decides it per picture.  While a long-term picture
+                                   exists, P slices have two active references (the previous picture, then the long-term one) and a
+                                   macroblock whose zero vector into the long-term picture is within the zero-motion threshold is
+                                   coded from it (P_L0_16x16, ref_idx_l0 1, zero vector).  An IDR (requested, gop or
+                                   b2v_set_resolution) clears it.  Works with CQP and CBR, paint-over, scaling, cropping,
+                                   B2V_FLAG_QUALITY and B2V_FLAG_WIDE_MOTION.  H.264 full-frame only: b2v_create rejects it
+                                   (B2V_EINVAL) with B2V_FLAG_JPEG, B2V_FLAG_NO_ENCODE, B2V_FLAG_DROPPABLE or in striped mode, and
+                                   b2v_set_resolution rejects a size at which stripe_rows would stripe.  It costs one kernel launch
+                                   per P picture (kernel_launches), a copy of one picture on the pictures that mark, and coded
+                                   width x height x 1.5 bytes. */
 };
 
 /* One encoded frame, the native image of the pixelflux callback result

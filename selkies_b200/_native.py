@@ -20,6 +20,7 @@ B2V_FLAG_SPS_EVERY_IDR, B2V_FLAG_NO_ENCODE, B2V_FLAG_TIMING, B2V_FLAG_DEVICE_TIM
 B2V_FLAG_QUALITY = 64
 B2V_FLAG_DROPPABLE = 128
 B2V_FLAG_WIDE_MOTION = 256
+B2V_FLAG_LONG_TERM_REF = 512
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
 B2V_DT_U8, B2V_DT_F16, B2V_DT_BF16, B2V_DT_F32 = 0, 1, 2, 3
 

@@ -96,7 +96,7 @@ struct Session {
   b2v_settings cfg{};
   int device = 0;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
-  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false, wide_motion = false;
+  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false, wide_motion = false, long_term_ref = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;
 
   // ingest ring
@@ -197,6 +197,7 @@ int alloc_geometry(Session* s) {
     ec.quality = s->quality;
     ec.droppable = s->droppable;
     ec.wide_motion = s->wide_motion;
+    ec.long_term_ref = s->long_term_ref;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
     s->lay = encoder_layout(s->enc);
@@ -703,6 +704,15 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if ((cfg->flags & B2V_FLAG_WIDE_MOTION) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
     return fail(B2V_EINVAL, "B2V_FLAG_WIDE_MOTION searches H.264 P pictures: %s codes none",
                 (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
+    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF keeps an H.264 reference picture: %s codes none",
+                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && (cfg->flags & B2V_FLAG_DROPPABLE))
+    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF with B2V_FLAG_DROPPABLE: a non-reference picture cannot mark a long-term "
+                "picture, and its reference is two pictures back");
+  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && stripes_active(cfg->stripe_rows, dh))
+    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
+                "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
   if ((cfg->flags & B2V_FLAG_DROPPABLE) && stripes_active(cfg->stripe_rows, dh))
     return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
                 "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
@@ -718,6 +728,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->quality = (cfg->flags & B2V_FLAG_QUALITY) != 0;
   s->droppable = (cfg->flags & B2V_FLAG_DROPPABLE) != 0;
   s->wide_motion = (cfg->flags & B2V_FLAG_WIDE_MOTION) != 0;
+  s->long_term_ref = (cfg->flags & B2V_FLAG_LONG_TERM_REF) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;
@@ -918,6 +929,9 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   if (!size_ok(sw, sh) || !size_ok(dw, dh)) return fail(B2V_EINVAL, "size unsupported");
   if (s->droppable && stripes_active(s->cfg.stripe_rows, dh))
     return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d would stripe a picture of %d macroblock rows",
+                s->cfg.stripe_rows, round16(dh) / 16);
+  if (s->long_term_ref && stripes_active(s->cfg.stripe_rows, dh))
+    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF is full-frame only: stripe_rows %d would stripe a picture of %d macroblock rows",
                 s->cfg.stripe_rows, round16(dh) / 16);
   // Submitters are locked out FIRST; then everything in flight drains (the output thread needs `mu`, not `submit_mu`, so it
   // keeps delivering); a producer still holding an acquired slot would be writing into memory about to be freed: refuse.

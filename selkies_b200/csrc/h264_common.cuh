@@ -20,8 +20,28 @@ constexpr unsigned FULL = 0xffffffffu;
 struct __align__(8) MbInfo {
   int16_t mvx, mvy;        // quarter-sample units
   uint8_t type;            // MB_*
-  uint8_t i16_mode, chroma_mode;
+  uint8_t i16_mode;        // MB_I16: Intra16x16PredMode; MB_P16: ref_idx_l0 (1 = the long-term reference, B2V_FLAG_LONG_TERM_REF)
+  uint8_t chroma_mode;
   uint8_t cbp;             // luma bits 0..3 | chroma << 4
+};
+
+// B2V_FLAG_LONG_TERM_REF (DESIGN.md §5.13; oracle/h264_ltr_ref.c).  changed[k & 1] counts the macroblocks of P picture k whose
+// co-located block fails the zero-motion exit (k_inter_lean, one atomic per block; zeroed on the analysis stream before it);
+// k_ltr_mark reads it and picture k-1's.  `epoch` is the FrameCtx::ltr_epoch of the picture that last marked a long-term
+// picture: the picture in FrameCtx::lt is a reference while it equals the current picture's, so an IDR retires it without a
+// write.  pic[k & 1] is what k_ltr_mark decided for picture k, read by the entropy stage of picture k (double-buffered for the
+// same reason as the side data: that stage overlaps the analysis of picture k+1).
+struct LtrPic {
+  int32_t active;          // a long-term picture is a reference of this picture: two active references (override in the slice header)
+  int32_t mark;            // this picture marks the previous one long-term (adaptive dec_ref_pic_marking)
+  int32_t drop_st;         // ... and first unmarks the short-term picture two back (MMCO 1): there was no long-term picture
+  int32_t pad;
+};
+struct LtrState {
+  int32_t changed[2];
+  int32_t epoch;
+  int32_t pad;
+  LtrPic pic[2];
 };
 
 // Feedback record of the rate controller / paint-over scheduler.  fb[k & 1] is written after picture k (rc_step, last block of
@@ -102,6 +122,11 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   uint8_t* dec_cur;        // [ch/4][cw/4] this picture's decimated luma, kept with the reconstruction buffer it writes
   const uint8_t* dec_ref;  // the reference picture's
   int* coarse;             // [mbs] at each anchor: its group's coarse vector (dx & 0xffff | dy << 16, decimated samples) or COARSE_NONE
+  // B2V_FLAG_LONG_TERM_REF (h264_inter.cu k_ltr_mark): null without the flag
+  LtrState* ltr;
+  uint8_t* lt;             // the long-term reference picture's reconstruction (NV12, coded size), valid while ltr->epoch == ltr_epoch
+  int ltr_epoch;           // IDR pictures coded so far (>= 1 in every P picture)
+  int prev_idr;            // the previous picture is an IDR picture: changed(k-1) = mbs
 };
 
 __device__ __forceinline__ int clip3i(int lo, int hi, int v) { return min(hi, max(lo, v)); }

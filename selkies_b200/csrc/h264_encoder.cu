@@ -37,6 +37,10 @@ struct Encoder {
   // B2V_FLAG_WIDE_MOTION: each reconstruction buffer's decimated luma (dec[b] belongs to recon[b]), and the anchors' coarse vectors
   uint8_t* dec[3] = {nullptr, nullptr, nullptr};
   int* coarse = nullptr;
+  // B2V_FLAG_LONG_TERM_REF: the long-term reference picture, outside the recon[] rotation (the device decides when it changes,
+  // k_ltr_mark), and the marking state
+  uint8_t* lt = nullptr;
+  LtrState* ltr = nullptr;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
   // of picture k (packing stream) overlaps the analysis of picture k+1 (main stream)
   MbInfo* mbinfo[2] = {nullptr, nullptr};
@@ -119,7 +123,7 @@ std::vector<uint8_t> make_param_sets(const EncoderConfig& c, int mbw, int mbh, i
   b.ue(0);                 // seq_parameter_set_id
   b.ue(4);                 // log2_max_frame_num_minus4
   b.ue(2);                 // pic_order_cnt_type
-  b.ue(1);                 // max_num_ref_frames
+  b.ue(c.long_term_ref ? 2 : 1);   // max_num_ref_frames: the previous picture, and with B2V_FLAG_LONG_TERM_REF a long-term one
   b.put(1, 0);             // gaps_in_frame_num_value_allowed_flag
   b.ue(mbw - 1); b.ue(mbh - 1);
   b.put(1, 1);             // frame_mbs_only_flag
@@ -138,7 +142,7 @@ std::vector<uint8_t> make_param_sets(const EncoderConfig& c, int mbw, int mbh, i
   b.ue(0); b.ue(0);        // max_bytes_per_pic_denom, max_bits_per_mb_denom
   b.ue(10); b.ue(10);      // log2_max_mv_length_horizontal / vertical
   b.ue(0);                 // max_num_reorder_frames
-  b.ue(1);                 // max_dec_frame_buffering
+  b.ue(c.long_term_ref ? 2 : 1);   // max_dec_frame_buffering
   b.trailing();
   append_nal(out, 3, 7, b.buf);
   HostBits p;
@@ -200,6 +204,12 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     }
     ECK(cudaMalloc((void**)&e->coarse, mbs * sizeof(int)));
   }
+  if (cfg->long_term_ref) {
+    ECK(cudaMalloc((void**)&e->lt, fb));
+    ECK(cudaMemset(e->lt, 0, fb));
+    ECK(cudaMalloc((void**)&e->ltr, sizeof(LtrState)));
+    ECK(cudaMemset(e->ltr, 0, sizeof(LtrState)));     // epoch 0: no long-term picture (every P picture has ltr_epoch >= 1)
+  }
   for (int b = 0; b < 2; b++) {
     ECK(cudaMalloc((void**)&e->mbinfo[b], mbs * sizeof(MbInfo)));
     ECK(cudaMemset(e->mbinfo[b], 0, mbs * sizeof(MbInfo)));
@@ -240,6 +250,10 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   const int crop_b = (cfg->coded_h - cfg->height) / 2;
   e->striped = cfg->stripe_rows > 0 && cfg->stripe_rows < e->mbh;
   if (e->striped && cfg->droppable) { snprintf(g_enc_err, sizeof g_enc_err, "non-reference pictures are not coded in striped mode"); encoder_destroy(e); return -1; }
+  if (cfg->long_term_ref && (e->striped || cfg->droppable)) {
+    snprintf(g_enc_err, sizeof g_enc_err, "a long-term reference is not kept in striped mode or with non-reference pictures");
+    encoder_destroy(e); return -1;
+  }
   if (e->striped && cfg->stripe_rows % cfg->slice_rows) { snprintf(g_enc_err, sizeof g_enc_err, "stripe_rows must be a multiple of slice_rows"); encoder_destroy(e); return -1; }
   e->band_rows = e->striped ? cfg->stripe_rows : e->mbh;
   e->n_bands = (e->mbh + e->band_rows - 1) / e->band_rows;
@@ -279,7 +293,7 @@ void encoder_destroy(Encoder* e) {
   void* ptrs[] = {e->recon[0], e->recon[1], e->recon[2], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
-                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse};
+                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse, e->lt, e->ltr};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -322,6 +336,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.band_fn = e->band_fn; f.band_coded = e->band_coded; f.au_data_off = e->au_data_off;
   f.param_sets = e->param_sets; f.param_len = e->param_len; f.csc_ts = p->csc_ts; f.au = p->au; f.overflow = e->overflow;
   if (e->cfg.wide_motion) { f.wide = 1; f.dec_cur = e->dec[wb]; f.dec_ref = e->dec[e->ref_buf]; f.coarse = e->coarse; }
+  if (e->cfg.long_term_ref) { f.ltr = e->ltr; f.lt = e->lt; f.ltr_epoch = e->idr_count; f.prev_idr = e->since_idr == 1; }
   int n = 0;
   // Two-stream schedule (no per-stage events requested): ANALYSIS of picture k on `st` (CSC before it, by the caller), ENTROPY
   // coding of picture k (CAVLC, slice build with the rate-control step, pack) on `st_pack`, overlapping
@@ -339,10 +354,20 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   //    buffers is taken changes no output.
   // k_quality runs right behind the analysis, on `st`: the only moment both of its inputs are complete and intact (the next
   // picture's colour conversion on `st` overwrites `cur`, the analysis of picture k+2 this reconstruction).
+  // B2V_FLAG_LONG_TERM_REF: k_ltr_mark of P picture k runs on `st` behind its analysis and before ev_analysed.  Everything it reads
+  // and writes is ordered by that stream or by the rules above:
+  //  * the count changed(k) is zeroed, then summed by k_inter_lean of picture k, then read by k_ltr_mark of k and k+1 — all on `st`;
+  //  * the long-term buffer is read only by k_inter_lean of pictures k and k+1 on `st`, before and after the copy k_ltr_mark of k
+  //    makes into it; the entropy stage never reads reference samples;
+  //  * the copy's source, f.ref, is picture k-1's reconstruction, which only the analysis of picture k+1 overwrites;
+  //  * the decision record pic[k & 1] is read by the entropy stage of picture k (after ev_analysed) and rewritten by k_ltr_mark of
+  //    picture k+2, whose analysis waits for the pack of picture k (ev_packed, or the single stream).
   const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
   if (overlap) cudaStreamWaitEvent(st, e->ev_packed[par], 0);           // pack of picture k-2 (no-op before the first two)
   if (f.wide) n += launch_coarse(f, st);      // every picture: its decimated plane; P pictures: the coarse vectors
+  if (f.ltr && !idr) cudaMemsetAsync(&e->ltr->changed[par], 0, sizeof(int32_t), st);
   n += idr ? launch_intra(f, st) : launch_inter(f, st);
+  if (f.ltr && !idr) n += launch_ltr_mark(f, st);
   if (e->quality_off) {
     QualityParams q{};
     q.src = p->cur; q.recon = f.recon;

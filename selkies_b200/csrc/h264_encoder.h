@@ -20,6 +20,7 @@ struct EncoderConfig {
   bool quality;            // B2V_FLAG_QUALITY: k_quality measures every band into the access unit's quality table
   bool droppable;          // B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture (full frame only)
   bool wide_motion;        // B2V_FLAG_WIDE_MOTION: coarse vectors per anchor group (k_coarse) and windows centred on far candidates
+  bool long_term_ref;      // B2V_FLAG_LONG_TERM_REF: one long-term reference picture, marked on the GPU (k_ltr_mark; full frame only)
 };
 
 struct EncodeFrameParams {

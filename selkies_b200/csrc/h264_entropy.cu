@@ -23,9 +23,9 @@ namespace b2v {
 // ------------------------------------------------------------------------------------------------ mv prediction (8.4.1.3, 8.4.1.1)
 __device__ __forceinline__ int median3(int a, int b, int c) { return max(min(a, b), min(max(a, b), c)); }
 
-// avX: neighbour partition available (inside the slice); rX: it is an inter macroblock with refIdx 0.
-// Intra (I_PCM) and unavailable neighbours contribute mv 0 / refIdx -1.
-struct MvCtx { bool avA, avB, avC, rA, rB, rC; int ax, ay, bx, by, cx, cy; };
+// avX: neighbour partition available (inside the slice); refX: its refIdx (0, or 1 for the long-term picture of
+// B2V_FLAG_LONG_TERM_REF).  Intra (I_PCM) and unavailable neighbours contribute mv 0 / refIdx -1.
+struct MvCtx { bool avA, avB, avC; int refA, refB, refC; int ax, ay, bx, by, cx, cy; };
 __device__ __forceinline__ MvCtx mv_ctx(const FrameCtx& f, int mbx, int mby) {
   MvCtx m;
   const bool top = top_in_slice(f, mby);
@@ -33,23 +33,26 @@ __device__ __forceinline__ MvCtx mv_ctx(const FrameCtx& f, int mbx, int mby) {
   int cxi = mbx + 1;
   if (!m.avC) { cxi = mbx - 1; m.avC = top && mbx > 0; }      // C unavailable -> D
   m.ax = m.ay = m.bx = m.by = m.cx = m.cy = 0;
-  m.rA = m.rB = m.rC = false;
-  if (m.avA) { const MbInfo a = f.mbinfo[mby * f.mbw + mbx - 1]; if (a.type == MB_P16) { m.rA = true; m.ax = a.mvx; m.ay = a.mvy; } }
-  if (m.avB) { const MbInfo b = f.mbinfo[(mby - 1) * f.mbw + mbx]; if (b.type == MB_P16) { m.rB = true; m.bx = b.mvx; m.by = b.mvy; } }
-  if (m.avC) { const MbInfo c = f.mbinfo[(mby - 1) * f.mbw + cxi]; if (c.type == MB_P16) { m.rC = true; m.cx = c.mvx; m.cy = c.mvy; } }
+  m.refA = m.refB = m.refC = -1;
+  if (m.avA) { const MbInfo a = f.mbinfo[mby * f.mbw + mbx - 1]; if (a.type == MB_P16) { m.refA = a.i16_mode; m.ax = a.mvx; m.ay = a.mvy; } }
+  if (m.avB) { const MbInfo b = f.mbinfo[(mby - 1) * f.mbw + mbx]; if (b.type == MB_P16) { m.refB = b.i16_mode; m.bx = b.mvx; m.by = b.mvy; } }
+  if (m.avC) { const MbInfo c = f.mbinfo[(mby - 1) * f.mbw + cxi]; if (c.type == MB_P16) { m.refC = c.i16_mode; m.cx = c.mvx; m.cy = c.mvy; } }
   return m;
 }
-__device__ __forceinline__ void mv_pred16(const MvCtx& m, int& px, int& py) {
+// 8.4.1.3 for refIdx `ref`: a neighbour with the other refIdx keeps its vector in the median but is not a match
+__device__ __forceinline__ void mv_pred16(const MvCtx& m, int ref, int& px, int& py) {
   if (!m.avB && !m.avC && m.avA) { px = m.ax; py = m.ay; return; }
-  const int cnt = (int)m.rA + (int)m.rB + (int)m.rC;
-  if (cnt == 1) { px = m.rA ? m.ax : m.rB ? m.bx : m.cx; py = m.rA ? m.ay : m.rB ? m.by : m.cy; return; }
+  const bool rA = m.refA == ref, rB = m.refB == ref, rC = m.refC == ref;
+  const int cnt = (int)rA + (int)rB + (int)rC;
+  if (cnt == 1) { px = rA ? m.ax : rB ? m.bx : m.cx; py = rA ? m.ay : rB ? m.by : m.cy; return; }
   px = median3(m.ax, m.bx, m.cx); py = median3(m.ay, m.by, m.cy);
 }
+// 8.4.1.1: P_Skip has refIdx 0
 __device__ __forceinline__ void mv_pred_skip(const MvCtx& m, int& px, int& py) {
   px = py = 0;
   if (!m.avA || !m.avB) return;
-  if ((m.rA && m.ax == 0 && m.ay == 0) || (m.rB && m.bx == 0 && m.by == 0)) return;
-  mv_pred16(m, px, py);
+  if ((m.refA == 0 && m.ax == 0 && m.ay == 0) || (m.refB == 0 && m.bx == 0 && m.by == 0)) return;
+  mv_pred16(m, 0, px, py);
 }
 
 // I_NxN macroblock header (7.3.5, 7.3.5.1): mb_type, 16 x (prev_intra4x4_pred_mode_flag [rem_intra4x4_pred_mode]),
@@ -74,15 +77,18 @@ __device__ __forceinline__ void mb_header_i4(S& h, const FrameCtx& f, const MbIn
 }
 
 // macroblock header of a coded (not I_PCM) macroblock: I_NxN above; I_16x16 (mb_type with prediction mode and cbp, intra_chroma_pred_mode,
-// mb_qp_delta); P_L0_16x16 (mb_type, mvd_l0, coded_block_pattern (inter me(v) mapping), mb_qp_delta)
+// mb_qp_delta); P_L0_16x16 (mb_type, ref_idx_l0 when the picture has two references: te(v) of range 1, one inverted bit, mvd_l0,
+// coded_block_pattern (inter me(v) mapping), mb_qp_delta)
 template <class S>
-__device__ __forceinline__ void mb_header(S& h, const FrameCtx& f, const MbInfo& mi, int mb, int mbx, int mby, int mvdx, int mvdy) {
+__device__ __forceinline__ void mb_header(S& h, const FrameCtx& f, const MbInfo& mi, int mb, int mbx, int mby, int mvdx, int mvdy, bool two_refs) {
   if (mi.type == MB_I4) mb_header_i4(h, f, mi, mb, mbx, mby);
   else if (mi.type == MB_I16) {
     const int tcode = 1 + mi.i16_mode + 4 * (mi.cbp >> 4) + ((mi.cbp & 15) ? 12 : 0);
     put_ue(h, (uint32_t)(f.idr ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
   } else {
-    put_ue(h, 0); put_se(h, mvdx); put_se(h, mvdy); put_ue(h, cbp_to_codenum_inter[mi.cbp]);
+    put_ue(h, 0);
+    if (two_refs) h.put(1, mi.i16_mode ? 0u : 1u);
+    put_se(h, mvdx); put_se(h, mvdy); put_ue(h, cbp_to_codenum_inter[mi.cbp]);
     if (mi.cbp) put_se(h, 0);
   }
 }
@@ -104,10 +110,11 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   // (most macroblocks of a desktop picture leave through the P_Skip exit: nothing that only a coded macroblock needs — the bit
   // scratch, the mvd — is touched before it)
   const int cbp_l = mi.cbp & 15, cbp_c = mi.cbp >> 4;
+  const bool two_refs = f.ltr && !f.idr && f.ltr->pic[f.pic & 1].active;     // B2V_FLAG_LONG_TERM_REF (k_ltr_mark)
   int mvdx = 0, mvdy = 0;
   if (!f.idr) {
     const MvCtx mc = mv_ctx(f, mbx, mby);
-    if (mi.type == MB_P16 && mi.cbp == 0) {
+    if (mi.type == MB_P16 && mi.cbp == 0 && mi.i16_mode == 0) {
       int sx, sy;
       mv_pred_skip(mc, sx, sy);
       if (mi.mvx == sx && mi.mvy == sy) {        // P_Skip: no bits; the slice scan folds it into mb_skip_run
@@ -116,7 +123,7 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
       }
     }
     int px, py;
-    mv_pred16(mc, px, py);
+    mv_pred16(mc, mi.i16_mode, px, py);
     mvdx = mi.mvx - px; mvdy = mi.mvy - py;
   }
 #pragma unroll
@@ -169,7 +176,7 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   CountSink cs;
   if (coded) cavlc_block(cs, lv, maxc, nC);
   CountSink hs;
-  mb_header(hs, f, mi, mb, mbx, mby, mvdx, mvdy);
+  mb_header(hs, f, mi, mb, mbx, mby, mvdx, mvdy, two_refs);
   const int hdr_bits = hs.n;
   int incl = cs.n;
 #pragma unroll
@@ -178,7 +185,7 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   const int my_off = hdr_bits + incl - cs.n;
 
   // ---- pass 2: write -----------------------------------------------------------------------------------
-  if (lane == 0) { BitWriter h{words, 0, MB_WORDS * 32}; mb_header(h, f, mi, mb, mbx, mby, mvdx, mvdy); }
+  if (lane == 0) { BitWriter h{words, 0, MB_WORDS * 32}; mb_header(h, f, mi, mb, mbx, mby, mvdx, mvdy, two_refs); }
   if (coded) { BitWriter ws{words, my_off, MB_WORDS * 32}; cavlc_block(ws, lv, maxc, nC); }
   __syncwarp();
   int nb = total_bits;
@@ -196,9 +203,28 @@ __device__ __forceinline__ void slice_header(S& s, const FrameCtx& f, int first_
   put_ue(s, 0);
   s.put(8, (uint32_t)(frame_num & 255));
   if (f.idr) put_ue(s, (uint32_t)(f.idr_pic_id & 15));
-  if (!f.idr) { s.put(1, 0); s.put(1, 0); }
-  // dec_ref_pic_marking(), present in reference pictures only
-  if (f.idr) { s.put(1, 0); s.put(1, 0); } else if (f.nal_ref_idc) s.put(1, 0);
+  // B2V_FLAG_LONG_TERM_REF: what k_ltr_mark decided for this picture (nothing without the flag)
+  LtrPic lp{0, 0, 0, 0};
+  if (f.ltr && !f.idr) lp = f.ltr->pic[f.pic & 1];
+  if (!f.idr) {
+    // num_ref_idx_active_override_flag (two references while a long-term picture is one: the previous picture, then the long-term
+    // one, the initial list of 8.2.4.2.1), ref_pic_list_modification_flag_l0
+    if (lp.active) { s.put(1, 1); put_ue(s, 1); } else s.put(1, 0);
+    s.put(1, 0);
+  }
+  // dec_ref_pic_marking(), present in reference pictures only.  A marking picture: adaptive_ref_pic_marking_mode_flag, [MMCO 1 on
+  // the short-term picture two back when no long-term picture was a reference: the DPB holds two frames], MMCO 4 (long-term
+  // indices below 1), MMCO 3 (the previous picture to long-term index 0, replacing the one there), MMCO 0.
+  if (f.idr) { s.put(1, 0); s.put(1, 0); }
+  else if (f.nal_ref_idc) {
+    if (lp.mark) {
+      s.put(1, 1);
+      if (lp.drop_st) { put_ue(s, 1); put_ue(s, 1); }
+      put_ue(s, 4); put_ue(s, 1);
+      put_ue(s, 3); put_ue(s, 0); put_ue(s, 0);
+      put_ue(s, 0);
+    } else s.put(1, 0);
+  }
   put_se(s, qp - 26);
   put_ue(s, 1);
 }

@@ -297,20 +297,29 @@ __device__ __forceinline__ void publish_anchor(const FrameCtx& f, int mb, int sa
 }
 
 // chroma prediction, residual, reconstruction and the macroblock's record; the luma prediction is already in t.pred_y.
-// uv_coloc: this lane's word of the co-located chroma reference.
+// uv_coloc: this lane's word of the co-located chroma reference.  ltr (B2V_FLAG_LONG_TERM_REF): the vector (LTR_MV, LTR_MV), which
+// no macroblock can have, stands for refIdx 1, the zero vector into the long-term picture.  The I_PCM header budget holds for it
+// unchanged: its mvd is -mvp, no longer than the mvd of a vector of the same range, and ref_idx_l0 (te(v), one bit, in every
+// P_L0_16x16 macroblock of a picture with two references) fits: 1 (mb_type) + 2 x 17 (mvd of +-134 quarter samples) + 11
+// (coded_block_pattern) + 1 (mb_qp_delta) = 47 bits without it, 48 with it; with wide-range motion 2 x 23 bits of mvd, 60 of
+// 48 + WM_MVD_BITS.
+constexpr int LTR_MV = -32768;
+constexpr uint32_t LTR_MV_WORD = 0x80008000u;
 template <bool WIDE>
-__device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc) {
+__device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc, bool ltr = false) {
+  const bool ref1 = ltr && mvx == LTR_MV;
   const size_t ysz = (size_t)f.cw * f.ch;
   const uint8_t* __restrict__ ref_uv = f.ref + ysz;
   const int rc4 = lane >> 2, cc4 = (lane & 3) * 4;
   const int mb = p.mb, mbx = p.mbx, mby = p.mby;
   {
     // chroma: mvC = luma mv, in 1/8 chroma samples (8.4.1.4, 8.4.2.2.2)
-    const int xi = mvx >> 3, yi = mvy >> 3, xf = mvx & 7, yf = mvy & 7;
+    const int xi = ref1 ? 0 : mvx >> 3, yi = ref1 ? 0 : mvy >> 3, xf = mvx & 7, yf = mvy & 7;
     const int cwc = f.cw >> 1;
     const int ya = clip3i(ylo >> 1, yhi >> 1, mby * 8 + yi + rc4), yb = clip3i(ylo >> 1, yhi >> 1, mby * 8 + yi + rc4 + 1);
     uint32_t out = 0;
-    if ((mvx | mvy) == 0) out = uv_coloc;      // zero vector: the co-located pairs, loaded with the first batch
+    if (ref1) out = __ldg(reinterpret_cast<const uint32_t*>(f.lt + ysz + (size_t)(mby * 8 + rc4) * f.cw + mbx * 16 + cc4));   // long-term, zero vector
+    else if ((mvx | mvy) == 0) out = uv_coloc;      // zero vector: the co-located pairs, loaded with the first batch
     else if ((xf | yf) == 0) {     // full-sample chroma position (most scrolling content): the (Cb,Cr) pairs are copied
 #pragma unroll
       for (int px = 0; px < 2; px++) {
@@ -336,8 +345,8 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 
   // ---- residual + reconstruction ------------------------------------------------------------------------
   // the vector as MbInfo's first word and the macroblock index are all that stays live across the transform: anything more
-  // spills inside it at k_inter_lean's 64 registers
-  const uint32_t mv = (uint32_t)(mvx & 0xffff) | ((uint32_t)mvy << 16);
+  // spills inside it at k_inter_lean's 64 registers.  So ref_idx 1 travels as a vector no macroblock can have, LTR_MV_WORD.
+  const uint32_t mv = ref1 ? LTR_MV_WORD : (uint32_t)(mvx & 0xffff) | ((uint32_t)mvy << 16);
   int luma_bits, chroma_bits;
   int cbp = transform_mb<false>(t, lane, qp, f.coef + (size_t)mb * COEF_BLOCKS * 16, f.nnz + (size_t)mb * 32, luma_bits, chroma_bits);
   if ((WIDE ? 48 + WM_MVD_BITS : 48) + luma_bits + chroma_bits > MB_BITS_LIMIT) { apply_pcm(t, lane, f.nnz + (size_t)mb * 32); cbp = -1; }   // A.3.1: send raw
@@ -347,6 +356,7 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
     store_recon(f, t, lane, (mb - ry * f.mbw) * 16, ry, ysz);
     if (lane == 0) {
       MbInfo mi; mi.mvx = (int16_t)(mv & 0xffff); mi.mvy = (int16_t)(mv >> 16); mi.type = MB_P16; mi.i16_mode = 0; mi.chroma_mode = 0; mi.cbp = (uint8_t)cbp;
+      if (ltr && mv == LTR_MV_WORD) { mi.mvx = 0; mi.mvy = 0; mi.i16_mode = 1; }
       if (cbp < 0) { mi.mvx = 0; mi.mvy = 0; mi.type = MB_PCM; mi.cbp = 0; }   // too big for CAVLC: I_PCM (transform_mb)
       f.mbinfo[mb] = mi;
     }
@@ -357,20 +367,37 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 // a temporal-predictor hit that needs no refinement are finished here; every other one goes into a queue for k_inter_search —
 // anchors into the anchor queue, the rest into the other.  No search and no 48 x 48 window: the registers and shared memory of
 // the search do not cap the occupancy of the common case.
-template <bool SCALE, bool WIDE>
+// LTR (B2V_FLAG_LONG_TERM_REF): the block counts changed(k) for k_ltr_mark, and while a long-term picture is a reference, a
+// macroblock that both exits fail is tested at the zero vector in it before it is queued (DESIGN.md §5.13).
+template <bool SCALE, bool WIDE, bool LTR>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) {
   __shared__ __align__(16) LeanSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int mbs = f.mbw * f.mbh;
   const int m = blockIdx.x * WARPS_PER_BLOCK + warp;
-  if (m >= mbs) return;
+  if (!LTR && m >= mbs) return;
   const MbPos p = mb_pos(f, m);
   LeanSm& sm = sm_all[warp];
   MbTile& t = sm.t;
   const int qp = frame_qp(f), lambda = me_lambda[qp];
   const int ylo = p.band_r0 * 16, yhi = min(f.mbh, p.band_r0 + f.band_rows) * 16 - 1;
-  const MbStart s = start_mb<SCALE>(f, t, lane, p);
+  MbStart s;
+  if (LTR) {     // every warp of the block reaches the count, those past the last macroblock included
+    if (m < mbs) s = start_mb<SCALE>(f, t, lane, p);
+    const int n = __syncthreads_count(m < mbs && lane == 0 && s.sad0 > ME_EARLY_SAD_PER_LAMBDA * lambda);
+    if (threadIdx.x == 0 && n) atomicAdd(&f.ltr->changed[f.pic & 1], n);
+    if (m >= mbs) return;
+  } else s = start_mb<SCALE>(f, t, lane, p);
   __syncwarp();
+  // B2V_FLAG_LONG_TERM_REF: the zero vector into the long-term picture, while there is one.  Its SAD is taken here, where little
+  // else is live, and used only if both exits below fail.
+  bool lt_hit = false;
+  if (LTR && s.sad0 > ME_EARLY_SAD_PER_LAMBDA * lambda && f.ltr->epoch == f.ltr_epoch) {
+    const int r8 = lane >> 1, c8 = (lane & 1) * 8;
+    const uint2 lz = __ldg(reinterpret_cast<const uint2*>(f.lt + (size_t)(p.mby * 16 + r8) * f.cw + p.mbx * 16 + c8));
+    const uint2 c = *reinterpret_cast<const uint2*>(&t.cur_y[r8][c8]);
+    lt_hit = __reduce_add_sync(FULL, (int)sad4acc(c.x, lz.x, sad4acc(c.y, lz.y, 0u))) <= ME_EARLY_SAD_PER_LAMBDA * lambda;
+  }
 
   // zero-motion early termination: co-located block within the quantisation noise of this QP
   int mvx = 0, mvy = 0, sad_int = 0;
@@ -393,6 +420,14 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
         sad_int = key_sad(best, lambda, mvx, mvy);
       }
     }
+    // the long-term picture at the zero vector, under the zero-motion threshold (tested above): the macroblock is finished from it
+    // (refIdx 1) and leaves the zero vector to its group and to the next picture, as a zero-vector exit does.  k_inter_search never
+    // tries it.
+    if (LTR && !hit && lt_hit) {
+      const int r8 = lane >> 1, c8 = (lane & 1) * 8;
+      *reinterpret_cast<uint2*>(&t.pred_y[r8][c8]) = __ldg(reinterpret_cast<const uint2*>(f.lt + (size_t)(p.mby * 16 + r8) * f.cw + p.mbx * 16 + c8));
+      mvx = mvy = LTR_MV; hit = true;
+    }
     if (!hit) {
       if (lane == 0) {
         const int qi = p.anchor ? 0 : 1;
@@ -401,8 +436,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
       return;
     }
   }
-  if (p.anchor && lane == 0) publish_anchor<WIDE>(f, m, sad_int, mvx, mvy);
-  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
+  if (p.anchor && lane == 0) publish_anchor<WIDE>(f, m, sad_int, LTR && mvx == LTR_MV ? 0 : mvx, LTR && mvy == LTR_MV ? 0 : mvy);   // sad_int 0 for refIdx 1
+  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc, LTR);
 }
 
 // One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
@@ -641,22 +676,32 @@ int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
   const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  if (f.wide) {                             // B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream)
-    if (f.ref_dist == f.prev_ref_dist) {
-      k_inter_lean<false, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+  if (f.ltr) {                              // B2V_FLAG_LONG_TERM_REF (never with B2V_FLAG_DROPPABLE: both distances are 1)
+    if (f.wide) k_inter_lean<false, true, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    else k_inter_lean<false, false, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    if (f.wide) {
       k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
       k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
     } else {
-      k_inter_lean<true, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+      k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+      k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    }
+  } else if (f.wide) {                      // B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream)
+    if (f.ref_dist == f.prev_ref_dist) {
+      k_inter_lean<false, true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    } else {
+      k_inter_lean<true, true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
       k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
       k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
     }
   } else if (f.ref_dist == f.prev_ref_dist) {      // every picture without B2V_FLAG_DROPPABLE
-    k_inter_lean<false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_lean<false, false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
     k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
     k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
   } else {
-    k_inter_lean<true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_lean<true, false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
     k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
     k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
   }
@@ -762,6 +807,39 @@ __global__ void __launch_bounds__(256) k_coarse(FrameCtx f) {
 int launch_coarse(const FrameCtx& f, cudaStream_t st) {
   const dim3 grid((f.mbw + 3) / 4, f.n_bands * ((f.band_rows + 3) / 4));
   k_coarse<<<grid, 256, 0, st>>>(f);
+  return 1;
+}
+
+// ---- k_ltr_mark (B2V_FLAG_LONG_TERM_REF): once per P picture k, on the analysis stream behind the analysis (DESIGN.md §5.13) ----
+// Picture k marks picture k-1 long-term when changed(k) >= max(ceil(mbs / 64), 8 * changed(k-1)): a large change right after a
+// quiet picture (changed of an IDR picture = mbs).  Every block decides from the two counts, which nothing in this launch writes,
+// and copies its share of f.ref (picture k-1's reconstruction) into f.lt when marking; block 0 records the decision for the entropy
+// stage of picture k and, when marking, makes the long-term picture valid for picture k+1.  Picture k itself was analysed against
+// the long-term picture as it stood: the marking takes effect after picture k (8.2.5).  oracle/h264_ltr_ref.c ltr_encode.
+constexpr int LTR_CHANGED_MIN_DIV = 64, LTR_CHANGED_RATIO = 8;
+constexpr int LTR_COPY_THREADS = 256;
+__global__ void __launch_bounds__(LTR_COPY_THREADS) k_ltr_mark(FrameCtx f) {
+  const int mbs = f.mbw * f.mbh;
+  const int changed = f.ltr->changed[f.pic & 1], prev = f.prev_idr ? mbs : f.ltr->changed[(f.pic & 1) ^ 1];
+  const bool mark = changed >= max((mbs + LTR_CHANGED_MIN_DIV - 1) / LTR_CHANGED_MIN_DIV, LTR_CHANGED_RATIO * prev);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const bool active = f.ltr->epoch == f.ltr_epoch;
+    LtrPic r; r.active = active; r.mark = mark; r.drop_st = mark && !active; r.pad = 0;
+    f.ltr->pic[f.pic & 1] = r;
+    if (mark) f.ltr->epoch = f.ltr_epoch;
+  }
+  if (!mark) return;
+  const size_t n16 = (size_t)f.cw * f.ch * 3 / 2 / 16;          // coded width is a multiple of 16
+  const uint4* src = reinterpret_cast<const uint4*>(f.ref);
+  uint4* dst = reinterpret_cast<uint4*>(f.lt);
+  for (size_t i = (size_t)blockIdx.x * LTR_COPY_THREADS + threadIdx.x; i < n16; i += (size_t)gridDim.x * LTR_COPY_THREADS) dst[i] = __ldg(src + i);
+}
+
+int launch_ltr_mark(const FrameCtx& f, cudaStream_t st) {
+  const size_t n16 = (size_t)f.cw * f.ch * 3 / 2 / 16;
+  const size_t want = (n16 + 4 * LTR_COPY_THREADS - 1) / (4 * LTR_COPY_THREADS);   // four 16-byte words per thread, at most 8 blocks per SM
+  const int blocks = (int)(want < 1056 ? want : 1056);
+  k_ltr_mark<<<blocks, LTR_COPY_THREADS, 0, st>>>(f);
   return 1;
 }
 

@@ -78,6 +78,7 @@ class CaptureSettings:
         self.quality_metrics = False             # measure every delivered record on the GPU: results carry `quality` (H.264 only)
         self.h264_droppable_frames = False       # every second P picture a non-reference picture a lagging consumer may drop (full frame only)
         self.h264_wide_motion = False            # motion vectors up to 128 px across and 256 px down/up for fast scrolls and drags (H.264 only)
+        self.h264_long_term_ref = False          # keep one earlier picture as a long-term reference: popups and app switches come back cheaply (full frame only)
 
 
 class StripeCallback:
@@ -262,6 +263,11 @@ class ScreenCapture:
             s.wide_motion = bool(getattr(settings, "h264_wide_motion", False))
             if s.wide_motion and jpeg:
                 raise ValueError("h264_wide_motion needs H.264 (output_mode 1): JPEG has no motion search")
+            s.long_term_ref = bool(getattr(settings, "h264_long_term_ref", False))
+            if s.long_term_ref and (jpeg or not bool(getattr(settings, "h264_fullframe", True)) or s.droppable):
+                raise ValueError("h264_long_term_ref needs full-frame H.264 (output_mode 1, h264_fullframe True) without "
+                                 "h264_droppable_frames: JPEG has no reference pictures, every H.264 stripe is a stream of its own, "
+                                 "and a droppable picture cannot mark a long-term one")
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)

@@ -169,7 +169,8 @@ class Session:
                  device: int = 0, rc_mode: int = N.B2V_RC_CBR, bitrate_kbps: int = 8000, crf: int = 26,
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
-                 collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False):
+                 collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False,
+                 long_term_ref: bool = False):
         self._lib = N.lib()
         if quality:
             flags |= N.B2V_FLAG_QUALITY
@@ -177,9 +178,12 @@ class Session:
             flags |= N.B2V_FLAG_DROPPABLE
         if wide_motion:
             flags |= N.B2V_FLAG_WIDE_MOTION
+        if long_term_ref:
+            flags |= N.B2V_FLAG_LONG_TERM_REF
         self.quality = bool(flags & N.B2V_FLAG_QUALITY)
         self.droppable = bool(flags & N.B2V_FLAG_DROPPABLE)
         self.wide_motion = bool(flags & N.B2V_FLAG_WIDE_MOTION)
+        self.long_term_ref = bool(flags & N.B2V_FLAG_LONG_TERM_REF)   # one earlier picture kept as a long-term reference
         self._hdr_len = 10 if header_mode == N.B2V_HDR_PIXELFLUX else 0
         self.device = device
         self.width, self.height = width, height
