@@ -39,6 +39,8 @@
 #define b2v_ref_wide_create ltr_wide_create_
 #define b2v_ref_wide_destroy ltr_wide_destroy_
 #define b2v_ref_wide_encode ltr_wide_encode_
+#define b2v_ref_wide_coarse ltr_wide_coarse_
+#define b2v_ref_wide_decimated ltr_wide_decimated_
 #include "h264_wide_ref.c"
 
 /* the marking rule: picture k marks picture k-1 long-term when changed(k) >= max(ceil(mbs / LTR_CHANGED_MIN_DIV),

@@ -360,6 +360,7 @@ static int64_t wide_encode(wide_t* w, const uint8_t* cur_nv12, int idr, int rc_m
   /* this picture's decimated luma, then the anchors' coarse vectors against the reference's */
   decimate(e, cur_nv12, dec_plane(w, e->recon[e->cur], 1));
   if (!idr) coarse_search(w, cur_nv12, qp);
+  else for (int i = 0; i < mbs; i++) w->coarse[i] = COARSE_NONE;      /* nothing reads it in an IDR; b2v_ref_wide_coarse reports none */
   /* phase A: analysis + reconstruction.  Intra: macroblocks of a slice are sequential (left/top
    * dependencies), slices are independent.  Inter: every macroblock is independent. */
   if (idr) {
@@ -495,4 +496,14 @@ void b2v_ref_wide_destroy(void* wh) {
 int64_t b2v_ref_wide_encode(void* wh, const uint8_t* cur_nv12, int idr, int rc_mode, int qp_fixed, int64_t target_bits, uint8_t* out) {
   wide_t* w = (wide_t*)wh;
   return w->l ? wide_layers_encode(w, cur_nv12, idr, rc_mode, qp_fixed, target_bits, out) : wide_encode(w, cur_nv12, idr, rc_mode, qp_fixed, target_bits, out);
+}
+/* the last picture's coarse table (mbw x mbh int32: at an anchor its group's dx & 0xffff | dy << 16, else COARSE_NONE) */
+void b2v_ref_wide_coarse(void* wh, int32_t* out) {
+  const wide_t* w = (const wide_t*)wh;
+  memcpy(out, w->coarse, sizeof(int32_t) * w->e->mbw * w->e->mbh);
+}
+/* the last picture's decimated luma ((cw / 4) x (ch / 4)), the plane kept with the reconstruction buffer it was coded into */
+void b2v_ref_wide_decimated(void* wh, uint8_t* out) {
+  wide_t* w = (wide_t*)wh;
+  memcpy(out, dec_plane(w, w->e->recon[w->e->cur], 0), (size_t)(w->e->cw / 4) * (w->e->ch / 4));
 }

@@ -9,6 +9,8 @@ import numpy as np
 from . import _u8p
 from .layers import LayeredRefEncoder
 
+COARSE_NONE = 0x7fffffff         # h264_wide_ref.c: an anchor group without a coarse vector, and every other macroblock
+
 
 class WideRefEncoder(LayeredRefEncoder):
     """LayeredRefEncoder with wide-range motion once set_wide_motion(True) is called (before the first picture; droppable pictures
@@ -52,6 +54,24 @@ class WideRefEncoder(LayeredRefEncoder):
         cur = np.concatenate([y.reshape(-1), uv.reshape(-1)])
         n = self.L.b2v_ref_wide_encode(self._wide, _u8p(cur), int(idr), rc_mode, qp, target_bits, _u8p(self._out))
         return self._out[:n].tobytes()
+
+    def coarse(self) -> list:
+        """The last picture's coarse vectors: coarse()[mby][mbx] is (dx, dy) in decimated samples at an anchor whose group has one,
+        None elsewhere (every macroblock of an IDR picture)."""
+        assert self.wide_motion
+        mbw, mbh = self.cw // 16, self.ch // 16
+        t = np.empty(mbw * mbh, np.int32)
+        self.L.b2v_ref_wide_coarse.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+        self.L.b2v_ref_wide_coarse(self._wide, t.ctypes.data_as(C.POINTER(C.c_int32)))
+        return [[None if v == COARSE_NONE else (int(np.int16(v & 0xffff)), int(v >> 16)) for v in row] for row in t.reshape(mbh, mbw)]
+
+    def decimated(self) -> np.ndarray:
+        """The last picture's decimated luma plane, (ch / 4) x (cw / 4)."""
+        assert self.wide_motion
+        d = np.empty((self.ch // 4, self.cw // 4), np.uint8)
+        self.L.b2v_ref_wide_decimated.argtypes = [C.c_void_p, C.POINTER(C.c_uint8)]
+        self.L.b2v_ref_wide_decimated(self._wide, _u8p(d))
+        return d
 
     def close(self):
         if getattr(self, "_wide", None):

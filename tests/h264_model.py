@@ -1,11 +1,13 @@
-"""A numpy model of the encoder's operations, written from ITU-T H.264 (8.3, 8.4.2.2, 8.5) and DESIGN.md §5.3 / §5.4, in int64.
+"""A numpy model of the encoder's operations, written from ITU-T H.264 (8.3, 8.4.2.2, 8.5) and DESIGN.md §5.3 (wide-range motion
+included) / §5.4, in int64.
 It shares no code with oracle/ or selkies_b200/.  Planes are 2-D uint8 arrays of the coded size (chroma: one array per
 component); coordinates are in samples of the plane."""
 from __future__ import annotations
 
 import numpy as np
+from numpy.lib.stride_tricks import sliding_window_view
 
-from tests.h264_syntax import BLK_IDX, BLK_XY, ZIGZAG_XY
+from tests.h264_syntax import BLK_IDX, BLK_XY, CDC_TOKEN, CDC_TOTAL_ZEROS, COEFF_TOKEN, RUN_BEFORE, TOTAL_ZEROS, ZIGZAG_XY
 
 # 8.5.9 / §5.4: quantisation multipliers MF and dequantisation scales v per qp % 6 for the position classes
 # (both coordinates even, both odd, otherwise)
@@ -136,7 +138,7 @@ def decimation_score(levels_scan):
     return score
 
 
-def decimate(luma_scan):
+def decimate_levels(luma_scan):
     """§5.4 inter-luma decimation of (16 blkIdx, 16 scan) levels: an 8x8 quadrant scoring < 4 is zeroed, all of it when the
     macroblock scores < 6."""
     out = luma_scan.copy()
@@ -150,6 +152,76 @@ def decimate(luma_scan):
 
 def raster_to_scan(r):
     return np.array([r[y, x] for x, y in ZIGZAG_XY], np.int64)
+
+
+# ------------------------------------------------------------------------------------------------ the I_PCM rule (§5.7)
+def _lengths(table):
+    return {v: len(code) for code, v in table.items()}
+
+
+_TOKEN, _CDC_TOKEN = [_lengths(t) for t in COEFF_TOKEN], _lengths(CDC_TOKEN)
+_TZ, _CDC_TZ, _RUN = [_lengths(t) for t in TOTAL_ZEROS], [_lengths(t) for t in CDC_TOTAL_ZEROS], [_lengths(t) for t in RUN_BEFORE]
+HEADER_BITS = 48                 # §5.7: the header budget of a macroblock; 96 for Intra4x4 (its prediction modes)
+WM_MVD_BITS = 48                 # §5.3: 48 more for a P macroblock of a wide-motion picture (two mvd of up to ±2046)
+
+
+def cavlc_bits(scan, chroma_dc=False):
+    """9.2: the length of residual_block_cavlc() for the levels `scan` (scan order, maxNumCoeff = len(scan)), with the longest
+    coeff_token of the four nC tables (§5.7: a size taken before the neighbours' counts are known), the chroma DC table for
+    chroma_dc."""
+    nz = [k for k, v in enumerate(scan) if v]
+    total = len(nz)
+    lv = [int(scan[k]) for k in reversed(nz)]            # highest frequency first
+    t1 = 0
+    while t1 < min(3, total) and abs(lv[t1]) == 1:
+        t1 += 1
+    bits = _CDC_TOKEN[(total, t1)] if chroma_dc else max(t.get((total, t1), 0) for t in _TOKEN)
+    if not total:
+        return bits
+    suffix_len = 1 if total > 10 and t1 < 3 else 0
+    for i, v in enumerate(lv):
+        if i < t1:
+            bits += 1                                    # trailing_ones_sign_flag
+            continue
+        code = 2 * v - 2 if v > 0 else -2 * v - 1        # 9.2.2.1 levelCode
+        if i == t1 and t1 < 3:
+            code -= 2
+        if suffix_len == 0:
+            bits += code + 1 if code < 14 else 19 if code < 30 else 28      # level_prefix 14 + 4 suffix bits; 15 + 12
+        else:
+            bits += (code >> suffix_len) + 1 + suffix_len if code < 15 << suffix_len else 28
+        if suffix_len == 0:
+            suffix_len = 1
+        if abs(v) > 3 << (suffix_len - 1) and suffix_len < 6:
+            suffix_len += 1
+    zeros = nz[-1] + 1 - total
+    if total < len(scan):
+        bits += (_CDC_TZ if chroma_dc else _TZ)[total - 1][zeros]
+    for i in range(total - 1):                           # run_before, highest frequency first, while zeros are left
+        if zeros <= 0:
+            break
+        run = nz[-1 - i] - nz[-2 - i] - 1
+        bits += _RUN[min(zeros, 7) - 1][run]
+        zeros -= run
+    return bits
+
+
+def mb_size_estimate(m, wide=False):
+    """§5.7 / §5.3: the size the encoders give a parsed macroblock `m` (not I_PCM, not P_Skip) when they decide whether to send it
+    raw: its coded blocks by cavlc_bits, plus the header budget — 48 bits, 96 for Intra4x4, 48 more for a P macroblock of a
+    wide-motion picture.  Above 3200 the macroblock is I_PCM."""
+    bits = HEADER_BITS + (HEADER_BITS if m.kind == "I_NxN" else 0) + (WM_MVD_BITS if wide and not m.intra else 0)
+    i16 = m.kind == "I_16x16"
+    if i16:
+        bits += cavlc_bits(m.luma_dc)
+    for blk in range(16):
+        if m.cbp >> (blk >> 2) & 1:
+            bits += cavlc_bits(m.luma[blk][1:] if i16 else m.luma[blk])
+    if m.cbp >> 4:
+        bits += sum(cavlc_bits(m.chroma_dc[c], chroma_dc=True) for c in range(2))
+    if m.cbp >> 4 & 2:
+        bits += sum(cavlc_bits(m.chroma_ac[c][blk][1:]) for c in range(2) for blk in range(4))
+    return bits
 
 
 # ------------------------------------------------------------------------------------------------ intra prediction (8.3)
@@ -386,13 +458,32 @@ def sad(a, b):
     return int(np.abs(np.asarray(a, np.int64) - np.asarray(b, np.int64)).sum())
 
 
-def full_search(src_blk, ref, x0, y0, qp, rows=None):
-    """Brute force over dx in [-16, 15], dy in [-16, 16] with clamped coordinates: {(dx, dy): (SAD, cost)}."""
+MV_MAX_FULL = 255                # §5.3 vector range, full samples per component (wide-range motion)
+
+
+def mv_ok(vx, vy):
+    """§5.3: a full-sample vector is usable when both components lie in [-255, 255]."""
+    return -MV_MAX_FULL <= vx <= MV_MAX_FULL and -MV_MAX_FULL <= vy <= MV_MAX_FULL
+
+
+def full_search(src_blk, ref, x0, y0, qp, rows=None, centre=(0, 0)):
+    """Brute force over the window centred on the full-sample vector `centre` — dx in [-16, 15], dy in [-16, 16] around it —
+    with clamped coordinates (8.4.2.2.1: a full-sample prediction is the reference sample at the clamped position), the vectors
+    outside mv_ok left out: {(vx, vy) full samples: (SAD, cost)}."""
+    h, w = ref.shape
+    r0, r1 = rows if rows is not None else (0, h - 1)
+    cx, cy = centre
+    ys = np.clip(np.arange(y0 + cy - 16, y0 + cy + 16 + 16), r0, r1)
+    xs = np.clip(np.arange(x0 + cx - 16, x0 + cx + 15 + 16), 0, w - 1)
+    win = sliding_window_view(ref[np.ix_(ys, xs)].astype(np.int64), (16, 16))      # win[16 + dy, 16 + dx] = the prediction
+    sads = np.abs(win - np.asarray(src_blk, np.int64)).sum(axis=(2, 3))
     out = {}
     for dy in range(-16, 17):
         for dx in range(-16, 16):
-            s = sad(src_blk, luma_inter(ref, x0, y0, (4 * dx, 4 * dy), rows=rows))
-            out[(dx, dy)] = (s, motion_cost(s, (4 * dx, 4 * dy), qp))
+            v = (cx + dx, cy + dy)
+            if mv_ok(*v):
+                s = int(sads[16 + dy, 16 + dx])
+                out[v] = (s, motion_cost(s, (4 * v[0], 4 * v[1]), qp))
     return out
 
 
@@ -400,3 +491,46 @@ def anchor_of(mbx, mby, mbw, band_r0, band_r1):
     """§5.3: the anchor of a macroblock is offset (1, 1) of its 4x4 group, rows counted inside the band [band_r0, band_r1),
     clamped into the band and the picture for partial groups."""
     return min(4 * (mbx // 4) + 1, mbw - 1), min(band_r0 + 4 * ((mby - band_r0) // 4) + 1, band_r1 - 1)
+
+
+# ------------------------------------------------------------------------------------------------ wide-range motion (§5.3)
+COARSE_DX, COARSE_DY = 32, 64    # the coarse search: dx in [-32, 31], dy in [-64, 63] decimated samples
+
+
+def decimate(y):
+    """The decimated luma of a coded luma plane: each sample the rounded mean (s + 8) >> 4 of the sum s of a 4x4 block."""
+    y = np.asarray(y, np.int64)
+    h, w = y.shape
+    return (y.reshape(h // 4, 4, w // 4, 4).sum(axis=(1, 3)) + 8) >> 4
+
+
+def coarse_search(dec_cur, dec_ref, mbx, mby, mbw, band_r0, band_r1, sad0, qp):
+    """The coarse vector (dx, dy) in decimated samples of the anchor group of macroblock (mbx, mby), or None.  Only an anchor whose
+    co-located full-resolution SAD `sad0` exceeds 96·λ searches.  The group (4x4 macroblocks, rows counted inside the band
+    [band_r0, band_r1), partial at the picture's right edge and the band's bottom) is a decimated block of up to 16x16 samples,
+    compared with dec_ref at every dx in [-32, 31], dy in [-64, 63] that keeps it inside the plane and the band's decimated rows;
+    the winner is the lexicographic minimum of (SAD, |dx| + |dy|, dy, dx).  The planes are decimate() of whole coded pictures."""
+    if anchor_of(mbx, mby, mbw, band_r0, band_r1) != (mbx, mby) or sad0 <= EARLY_SAD_PER_LAMBDA * LAMBDA[qp]:
+        return None
+    gx0, gy0 = 4 * (mbx // 4), band_r0 + 4 * ((mby - band_r0) // 4)
+    X0, Y0, W, H = 4 * gx0, 4 * gy0, 4 * (min(gx0 + 4, mbw) - gx0), 4 * (min(gy0 + 4, band_r1) - gy0)
+    blk = np.asarray(dec_cur, np.int64)[Y0:Y0 + H, X0:X0 + W]
+    lo, hi, dw = 4 * band_r0, 4 * band_r1, dec_ref.shape[1]
+    dxs = [dx for dx in range(-COARSE_DX, COARSE_DX) if 0 <= X0 + dx and X0 + dx + W <= dw]
+    dys = [dy for dy in range(-COARSE_DY, COARSE_DY) if lo <= Y0 + dy and Y0 + dy + H <= hi]
+    if not dxs or not dys:
+        return None
+    win = sliding_window_view(np.asarray(dec_ref, np.int64), (H, W))                # win[y, x] = the block at (x, y)
+    sads = np.abs(win[Y0 + dys[0]:Y0 + dys[-1] + 1, X0 + dxs[0]:X0 + dxs[-1] + 1] - blk).sum(axis=(2, 3))
+    DY, DX = (a.ravel() for a in np.meshgrid(dys, dxs, indexing="ij"))
+    i = np.lexsort((DX, DY, np.abs(DX) + np.abs(DY), sads.ravel()))[0]
+    return int(DX[i]), int(DY[i])
+
+
+def second_window(coarse):
+    """§5.3: the full-sample centre (coarse × 4) of an anchor's second ±16 search, or None — no coarse vector, or one the co-located
+    search covers with the 4 samples either way a decimated sample spans (x in [-12, 11] and y in [-12, 12])."""
+    if coarse is None:
+        return None
+    cx, cy = 4 * coarse[0], 4 * coarse[1]
+    return None if -12 <= cx <= 11 and -12 <= cy <= 12 else (cx, cy)

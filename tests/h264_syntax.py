@@ -258,6 +258,7 @@ class Picture:
     idr: bool
     frame_num: int
     qp: int                      # slice QP of the first slice
+    nal_ref_idc: int = 1         # of the first slice: 0 for a non-reference picture
     mbs: list = field(default_factory=list)
     slice_first_mb: list = field(default_factory=list)
     headers: list = field(default_factory=list)      # the parsed header fields of every slice, in order
@@ -595,7 +596,7 @@ class StreamParser:
                     state = _PicState(self.sps)
                 hdr = parse_slice(rbsp, t, ref_idc, self.sps, self.pps, state, len(pic.slice_first_mb) if pic else 0)
                 if pic is None:
-                    pic = Picture(self.sps, t == 5, hdr["frame_num"], hdr["qp"])
+                    pic = Picture(self.sps, t == 5, hdr["frame_num"], hdr["qp"], ref_idc)
                 elif hdr["first_mb"] != pic.headers[-1]["end_mb"]:
                     raise SyntaxError_("slices are not contiguous")
                 pic.slice_first_mb.append(hdr["first_mb"])

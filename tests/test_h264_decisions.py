@@ -21,9 +21,12 @@ import pytest
 import oracle
 from oracle import avdec
 from tests import h264_model as M
+from tests import layered_scenario as LS
 from tests import scenario as S
 from tests import synth
-from tests.h264_syntax import BLK_XY, Mb, parse_stream, scan_to_raster
+from tests import wide_content as WC
+from tests import wide_scenario as WS
+from tests.h264_syntax import BLK_XY, Mb, StreamParser, parse_stream, scan_to_raster, split_annexb
 
 MAX_MB_BITS = 3200                       # A.3.1
 # Table A-1: level_idc -> MaxFS (macroblocks), levels 3.1 .. 6.2
@@ -55,6 +58,7 @@ class Encoded:
         self.bands = {}
         self.sources = []
         self.recon = None                # the encoder's reconstruction after the last picture
+        self.wide = False                # coded with wide-range motion (B2V_FLAG_WIDE_MOTION)
 
     def add(self, index, y_start, au):
         self.bands.setdefault(y_start, []).append((index, au))
@@ -66,11 +70,20 @@ def source_nv12(frame, cw, ch):
     return y, uv[:, 0::2], uv[:, 1::2]
 
 
-def encode_oracle(cfg: S.Config, frames, idr_at=(0,), qps=None) -> Encoded:
-    """The oracle encoder over `frames` (IDR at the indices in idr_at, QP per picture from qps when given)."""
-    side = S.OracleSide(cfg)
+def oracle_side(cfg: S.Config) -> S.OracleSide:
+    """The oracle side for cfg.flags: wide-range motion (droppable or not), droppable pictures, or neither."""
+    if cfg.flags & WS.FLAG_WIDE_MOTION:
+        return WS.WideOracleSide(cfg)
+    return LS.LayeredOracleSide(cfg) if cfg.flags & LS.FLAG_DROPPABLE else S.OracleSide(cfg)
+
+
+def encode_oracle(cfg: S.Config, frames, idr_at=(0,), qps=None, each=None) -> Encoded:
+    """The oracle encoder over `frames` (IDR at the indices in idr_at, QP per picture from qps when given); each(i, encoder, bands)
+    after picture i when given."""
+    side = oracle_side(cfg)
     enc = side.enc
     out = Encoded(cfg.width, cfg.height, enc.cw, enc.ch)
+    out.wide = bool(cfg.flags & WS.FLAG_WIDE_MOTION)
     for i, f in enumerate(frames):
         if i in idr_at:
             side.control(S.request_idr())
@@ -80,6 +93,8 @@ def encode_oracle(cfg: S.Config, frames, idr_at=(0,), qps=None) -> Encoded:
         out.sources.append(source_nv12(f, enc.cw, enc.ch))
         for y0, au in x.bands:
             out.add(i, y0, au)
+        if each is not None:
+            each(i, enc, x.bands)
     out.recon = enc.recon()
     return out
 
@@ -125,10 +140,10 @@ def _avail(pic, addr, mbw):
     return M.Avail(ok(-1, 0), ok(0, -1), ok(1, -1), ok(-1, -1))
 
 
-def check_picture(pic, prev, src, where, stats):
-    """Reconstructs `pic` from its syntax with the model (prev = the model's previous picture of this stream) and checks every
-    macroblock's levels against the model's levels for the source `src` (Y, U, V of the stream's coded size).  Returns the
-    reconstruction (Y, U, V)."""
+def check_picture(pic, prev, src, where, stats, wide=False):
+    """Reconstructs `pic` from its syntax with the model (prev = the model's reference picture of this stream) and checks every
+    macroblock's levels against the model's levels for the source `src` (Y, U, V of the stream's coded size), and that every
+    macroblock sent coded fits the I_PCM rule's budget (wide: a wide-motion stream).  Returns the reconstruction (Y, U, V)."""
     mbw, mbh = pic.sps.mbw, pic.sps.mbh
     rec = [np.zeros((mbh * 16, mbw * 16), np.uint8), np.zeros((mbh * 8, mbw * 8), np.uint8), np.zeros((mbh * 8, mbw * 8), np.uint8)]
     sy, su, sv = (p.astype(np.int64) for p in src)
@@ -144,6 +159,9 @@ def check_picture(pic, prev, src, where, stats):
             continue
         if m.kind != "P_Skip":
             assert m.bits <= MAX_MB_BITS, f"{at}: macroblock_layer() of {m.bits} bits (A.3.1 limit 3200)"
+            est = M.mb_size_estimate(m, wide)
+            assert m.bits <= est, f"{at}: {m.bits} bits coded, more than the {est} of the size rule"     # the rule only overstates
+            assert est <= MAX_MB_BITS, f"{at}: sized {est} bits by the rule of §5.7 (wide {wide}), coded instead of I_PCM"
             stats.max_bits = max(stats.max_bits, m.bits)
         if m.kind == "P_L0_16x16":
             assert not (m.cbp == 0 and m.mv == m.skip_mv), f"{at}: cbp 0 and the P_Skip vector {m.mv}, coded as P_L0_16x16"
@@ -179,7 +197,7 @@ def check_picture(pic, prev, src, where, stats):
                 assert np.array_equal(M.raster_to_scan(dc), m.luma_dc), f"{at}: Intra16x16 DC levels {m.luma_dc} != model {M.raster_to_scan(dc)}"
                 dcy = M.luma_dc_dequant(scan_to_raster(m.luma_dc), qp)
             else:
-                model = M.decimate(model)
+                model = M.decimate_levels(model)
             for blk in range(16):
                 assert np.array_equal(model[blk], parsed[blk]), f"{at}: luma block {blk} levels {parsed[blk]} != model {model[blk]}"
             for blk in range(16):
@@ -220,7 +238,8 @@ def check_picture(pic, prev, src, where, stats):
 
 
 def check_encoded(e: Encoded, stripe_rows=0):
-    """All per-picture checks over every band stream of `e`; returns Stats."""
+    """All per-picture checks over every band stream of `e`; returns Stats.  A P picture predicts from the model's reconstruction
+    of the last picture with nal_ref_idc != 0 (two back after a droppable picture)."""
     stats = Stats()
     mbw, mbh = e.cw // 16, e.ch // 16
     for y_start, items in sorted(e.bands.items()):
@@ -236,14 +255,15 @@ def check_encoded(e: Encoded, stripe_rows=0):
                 check_sps(pic.sps, e.width, e.height, y_start, band_h, mbw, band_mbh, stats)
             assert pic.sps.mbh == band_mbh
             src = [p[y_start // k: y_start // k + band_mbh * 16 // k] for p, k in zip(e.sources[index], (1, 2, 2))]
-            rec = check_picture(pic, prev, src, where, stats)
+            rec = check_picture(pic, prev, src, where, stats, e.wide)
             vh, vw = pic.sps.height, pic.sps.width
             for k, (r, d) in enumerate(zip(rec, dec)):
                 s = 1 if k == 0 else 2
                 assert np.array_equal(r[: vh // s, : vw // s], d), f"{where}: model reconstruction of plane {k} != libavcodec's decode"
-            prev = rec
+            if pic.nal_ref_idc:
+                prev = rec
             stats.pictures += 1
-        stats.last[y_start] = prev
+        stats.last[y_start] = rec
     return stats
 
 
@@ -298,6 +318,62 @@ def cases():
     out.append(("predictor_paths", S.Config(130, 70, qp=30), synth.predictor_paths(130, 70), (0,), None, 0))
     still = synth.desktop(96, 64, 0)
     out.append(("paintover_burst", S.Config(96, 64, qp=40, paint=(2, 20, 3)), [still] * 8, (0,), None, 0))
+    return out + wide_cases()
+
+
+WIDE = WS.FLAG_WIDE_MOTION
+
+
+def blocky_noise(w, h, x0, y0, seed=11):
+    """The window at (x0, y0) of one large plane of 2x2-blocky mid-range grey noise, as a BGRA picture."""
+    rng = np.random.default_rng(seed)
+    luma = rng.integers(48, 208, (h // 2 + 160, w // 2 + 160)).repeat(2, 0).repeat(2, 1)
+    return grey(w, h, grey_table(), luma[y0:y0 + h, x0:x0 + w])
+
+
+def band_bottom_scroll(w, h, rows, seed=13):
+    """Two BGRA pictures of 2x2-blocky grey noise, the second scrolled up by 4 px, with the last 4 luma rows of every band of `rows`
+    macroblock rows dark in the second (the first 4 of the next band in the first): the bottom group of each band matches the
+    reference exactly one decimated row below the band, where the coarse search must not look."""
+    rng = np.random.default_rng(seed)
+    luma = rng.integers(48, 208, ((h + 4) // 2 + 1, w // 2)).repeat(2, 0).repeat(2, 1)[:h + 4]
+    for y in range(16 * rows, h, 16 * rows):
+        luma[y:y + 4] = 16
+    inv = grey_table()
+    return [grey(w, h, inv, luma[:h]), grey(w, h, inv, luma[4:4 + h])]
+
+
+def moving_noise(w, h, n, v, seed=3):
+    """n BGRA pictures of 2x2-blocky grey noise moving by v px per picture (content at (x, y) was at (x, y) + v one picture earlier:
+    true vector v) with fresh noise on top, its amplitude rising from 0 at the left edge to 64 at the right edge: residuals from
+    none to beyond the limit of A.3.1."""
+    rng = np.random.default_rng(seed)
+    pw, ph = w + abs(v[0]) * n, h + abs(v[1]) * n
+    base = rng.integers(40, 216, (ph // 2 + 1, pw // 2 + 1)).repeat(2, 0).repeat(2, 1)
+    inv = grey_table()
+    amp = np.linspace(0, 64, w)[None, :]
+    out = []
+    for t in range(n):
+        x0, y0 = (t * c + (n - 1) * max(0, -c) for c in v)
+        fresh = np.rint(amp * rng.uniform(-1, 1, (h, w))).astype(np.int64)
+        out.append(grey(w, h, inv, np.clip(base[y0:y0 + h, x0:x0 + w] + fresh, 16, 235)))
+    return out
+
+
+def wide_cases():
+    """Wide-range motion (B2V_FLAG_WIDE_MOTION, §5.3): the configurations of both files with the flag on."""
+    out = [("wide_scroll40", S.Config(640, 368, qp=26, flags=WIDE), [WC.desktop_scroll(640, 368, t, 40) for t in range(3)], (0,), None, 0),
+           ("wide_scroll250_tall", S.Config(96, 640, qp=26, flags=WIDE), [WC.desktop_scroll(96, 640, t, 250) for t in range(3)], (0,), None, 0),
+           # mbw = 21: a group of one macroblock column at the right edge; the window leaves through the top-left corner
+           ("wide_drag_corner", S.Config(336, 208, qp=26, flags=WIDE),
+            [WC.drag(336, 208, t, (-37, -29), (150, 100), 160, 112) for t in range(6)], (0,), None, 0),
+           # bands of 3 macroblock rows (and one of 2): every group is partial, the coarse search stops at each band's edges
+           ("wide_drag_striped3", S.Config(320, 176, qp=27, slice_rows=1, stripe_rows=3, flags=WIDE),
+            [WC.drag(320, 176, t, (-70, 6), (220, 30), 96, 112) for t in range(3)], (0,), None, 3),
+           # droppable: pictures 1 and 3 are non-reference, pictures 2 and 4 predict from two back (256 px, beyond the range)
+           ("wide_scroll128_droppable", S.Config(160, 480, qp=26, flags=WIDE | LS.FLAG_DROPPABLE),
+            [WC.desktop_scroll(160, 480, t, 128) for t in range(5)], (0,), None, 0),
+           ("wide_pcm_noise_qp0_4", S.Config(224, 128, qp=0, flags=WIDE), moving_noise(224, 128, 3, (-100, 60)), (0,), [0, 2, 4], 0)]
     return out
 
 
@@ -316,10 +392,62 @@ def test_oracle_decisions(case):
     e, st = run_case(encode_oracle, case)
     check_recon(e, st)
     assert st.pictures >= len(case[2])
-    if case[0] == "pcm_noise_qp0_4":
+    if case[0] in ("pcm_noise_qp0_4", "wide_pcm_noise_qp0_4"):
         assert st.kinds.get("I_PCM", 0) > 0, st.kinds
     if case[0] == "paintover_burst":
         assert st.kinds.get("P_L0_16x16", 0) > 0        # the burst re-codes the still at the paint-over QP
+
+
+def nal_ref_idc(au):
+    """nal_ref_idc of the first slice of an access unit."""
+    return next(n[0] >> 5 & 3 for n in split_annexb(au) if n[0] & 31 in (1, 5))
+
+
+# The decisions' wide-motion cases, and three more for the coarse search alone: mbw % 4 = 2 in bands of 5 rows at QP 51 (the
+# largest λ: most groups stay below the early exit), mbw % 4 = 3 at QP 0 (λ = 1: nearly every group searches), 2x2-blocky
+# noise moved 124 px left and 256 px down, whose only match is the coarse window's corner (dx = 31, dy = -64), and noise
+# scrolled in bands of 5 rows whose bottom groups match best one decimated row past the band.
+COARSE_CASES = [c for c in CASES if c[1].flags & WIDE] + [
+    ("coarse_drag_stripes5_qp51", S.Config(160, 144, qp=51, stripe_rows=5, flags=WIDE),
+     [WC.drag(160, 144, t, (-30, 22), (90, 10), 64, 64) for t in range(4)], (0,), None, 5),
+    ("coarse_scroll_qp0", S.Config(240, 208, qp=0, flags=WIDE), [WC.desktop_scroll(240, 208, t, 60) for t in range(3)], (0,), None, 0),
+    ("coarse_noise_corner", S.Config(192, 448, qp=26, flags=WIDE), [blocky_noise(192, 448, 0, 256), blocky_noise(192, 448, 124, 0)],
+     (0,), None, 0),
+    ("coarse_band_bottoms", S.Config(128, 208, qp=26, stripe_rows=5, flags=WIDE), band_bottom_scroll(128, 208, 5), (0,), None, 5)]
+
+
+@pytest.mark.parametrize("case", COARSE_CASES, ids=[c[0] for c in COARSE_CASES])
+def test_oracle_coarse_search(case):
+    """The decimated plane of every picture equals the model's decimation of its source, and at every macroblock the coarse table
+    equals the model's coarse search (None included: non-anchors, still groups, IDR pictures) between the decimated sources of the
+    picture and of its reference (the last reference picture: two back after a droppable one)."""
+    _, cfg, frames, idr_at, qps, stripe_rows = case
+    seen = []
+    e = encode_oracle(cfg, frames, idr_at, qps,
+                      each=lambda i, enc, bands: seen.append((enc.decimated(), enc.coarse(), enc.recon()[0].copy(),
+                                                              nal_ref_idc(bands[0][1]) if bands else 1)))
+    mbw, mbh = e.cw // 16, e.ch // 16
+    rows = stripe_rows or mbh
+    ref, searched = None, 0
+    for i, (dec, coarse, recon, ref_idc) in enumerate(seen):
+        y = e.sources[i][0]
+        assert np.array_equal(dec, M.decimate(y)), f"picture {i}: decimated plane"
+        if i in idr_at:
+            assert all(v is None for row in coarse for v in row), f"picture {i}: an IDR picture with coarse vectors"
+        else:
+            dref, yref = M.decimate(e.sources[ref][0]), seen[ref][2].astype(np.int64)
+            dcur = M.decimate(y)
+            for mby in range(mbh):
+                r0 = mby // rows * rows
+                for mbx in range(mbw):
+                    x0, y0 = 16 * mbx, 16 * mby
+                    sad0 = M.sad(y[y0:y0 + 16, x0:x0 + 16], yref[y0:y0 + 16, x0:x0 + 16])
+                    want = M.coarse_search(dcur, dref, mbx, mby, mbw, r0, min(r0 + rows, mbh), sad0, cfg.qp if qps is None else qps[i])
+                    assert coarse[mby][mbx] == want, f"picture {i} mb ({mbx},{mby}): coarse vector {coarse[mby][mbx]}, model {want}"
+                    searched += want is not None
+        if ref_idc:
+            ref = i
+    assert searched > 0
 
 
 def test_oracle_decisions_720p_idr():
@@ -335,10 +463,12 @@ def test_oracle_decisions_720p_idr():
 class OracleEnc:
     """One CQP oracle encoder, picture by picture: encode() returns {band y_start: access unit} of the coded bands."""
 
-    def __init__(self, w, h, qp, slice_rows=0, stripe_rows=0):
-        self.e = oracle.RefEncoder(w, h, slice_rows)
+    def __init__(self, w, h, qp, slice_rows=0, stripe_rows=0, wide=False):
+        self.e = (WS.WideRefEncoder if wide else oracle.RefEncoder)(w, h, slice_rows)
         if stripe_rows:
             self.e.set_stripes(stripe_rows)
+        if wide:
+            self.e.set_wide_motion(True)
         self.qp, self.stripe_rows = qp, stripe_rows
 
     def encode(self, frame, idr):
@@ -367,46 +497,77 @@ def shifted(y, mv):
 
 # Full-sample extremes of the window, interior full-sample shifts, and half- and quarter-sample shifts with |d| <= 13.
 RECOVERY_SHIFTS = [(-64, 0), (60, 0), (0, -64), (0, 64), (-64, 64), (20, -12), (10, -6), (-26, 18), (5, -3), (-51, 45), (47, -1)]
+# Wide-range motion (quarter samples) on a wide, short picture: 16 and -17 px, just past the co-located window (16 px needs the
+# second search: the co-located one ends at 15); the coarse window's edges -128 and +124 px across; (37, -53) px, not a multiple
+# of 4; (-90.5, 20.25) px, fractional, its refinement gate open.  On a tall, narrow one: 252 px down, the coarse window's last row,
+# and 255 px up, the end of the vector range.
+WIDE_SHIFTS_ACROSS = [(64, 0), (-68, 0), (-512, 0), (496, 0), (148, -212), (-362, 81)]
+WIDE_SHIFTS_DOWN = [(0, 1008), (0, -1020)]
 
 
-def motion_recovery(make_enc, qp=26, w=256, h=160):
+def _interior(mbx, mby, mv, w, h, wide):
+    """The macroblocks a search must resolve to exactly the shift mv.  The 48x48 window of §5.3 spans x0-16 .. x0+31 and y0-16 ..
+    y0+31 around its centre; where it lies inside the picture nothing is clamped, and the refinement runs only for |d| <= 13,
+    whose 6-tap support (-15 .. +31) stays inside the window.  Without wide motion the window is centred on the macroblock; with
+    it, on the shift's full-sample vector (its x rounded down to a multiple of 4, as §5.3 stages a far candidate's window), and the
+    macroblock's group, moved by the shift / 4 either way rounded, stays inside the decimated plane: the coarse search sees it."""
+    fx, fy = ((mv[0] + 2) >> 2, (mv[1] + 2) >> 2) if wide else (0, 0)
+    cx = fx & ~3
+    if not (16 <= 16 * mbx + cx and 16 * mbx + cx + 32 <= w and 16 <= 16 * mby + fy and 16 * mby + fy + 32 <= h):
+        return False
+    if not wide:
+        return True
+    gx0, gy0 = 4 * (mbx // 4), 4 * (mby // 4)
+    gx1, gy1 = min(gx0 + 4, w // 16), min(gy0 + 4, h // 16)
+    return (16 * gx0 + 4 * (fx // 4) >= 0 and 16 * gx1 + 4 * -(-fx // 4) <= w and 16 * gy0 + 4 * (fy // 4) >= 0
+            and 16 * gy1 + 4 * -(-fy // 4) <= h)
+
+
+def motion_recovery(make_enc, qp=26, w=256, h=160, wide=False, shifts=RECOVERY_SHIFTS, gate_at=(3, 2)):
     """An IDR of 2x2-blocky mid-range luma noise, then for each shift a P picture built from the encoder's own reconstruction
-    moved by the shift: every macroblock must come out with cbp 0, and every macroblock whose window and interpolation support
-    stay inside the picture must carry exactly the shift."""
+    moved by the shift: every macroblock must come out with cbp 0, and every macroblock _interior() names must carry exactly the
+    shift.  wide: with wide-range motion, where cbp 0 is asserted on those macroblocks only (a group whose block the shift moves
+    out of the decimated plane has no coarse match, and its macroblocks may code a residual); and for a fractional shift on the
+    anchors only: the others reach a far vector only through their anchor's, whose test accepts a full-sample SAD of at most
+    4·96·λ, and an open refinement gate puts it above that.  A fractional shift's refinement gate is checked open at macroblock
+    gate_at."""
     rng = np.random.default_rng(11)
     luma = rng.integers(96, 160, (h // 2, w // 2)).repeat(2, 0).repeat(2, 1)
     inv = grey_table()
     f0 = grey(w, h, inv, luma)
-    enc = make_enc(w, h, qp)
+    enc = make_enc(w, h, qp, wide=wide)
     try:
         aus0 = enc.encode(f0, True)
+        parser = StreamParser()
+        parser.picture(aus0[0])
         ry, ruv = enc.recon()
         assert (ruv == 128).all()
         lam = M.LAMBDA[qp]
         mbw, mbh = w // 16, h // 16
-        for mv in RECOVERY_SHIFTS:
+        for mv in shifts:
             y1 = shifted(ry, mv)
             assert 16 <= y1.min() and y1.max() <= 235                   # no sample of the target is clipped by the CSC
             # the refinement gate of §5.3 is open for a fractional shift: full-sample SAD above 96·λ and below 8192
             if (mv[0] | mv[1]) & 3:
-                fs = (mv[0] + 2) >> 2, (mv[1] + 2) >> 2
-                s = M.sad(y1[32:48, 48:64], M.luma_inter(ry, 48, 32, (4 * fs[0], 4 * fs[1])))
+                fs, (x0, y0) = ((mv[0] + 2) >> 2, (mv[1] + 2) >> 2), (16 * gate_at[0], 16 * gate_at[1])
+                assert _interior(*gate_at, mv, w, h, wide)
+                s = M.sad(y1[y0:y0 + 16, x0:x0 + 16], M.luma_inter(ry, x0, y0, (4 * fs[0], 4 * fs[1])))
                 assert M.EARLY_SAD_PER_LAMBDA * lam < s < M.REFINE_MAX_SAD, (mv, s)
             f1 = grey(w, h, inv, y1)
-            enc.encode(f0, True)
-            aus = enc.encode(f1, False)
-            pics = parse_stream([aus0[0], aus[0]])
-            p = pics[1]
-            # The 48x48 window of §5.3 spans x0-16 .. x0+31 and y0-16 .. y0+31.  Where it lies inside the picture nothing is
-            # clamped; the refinement runs only for |d| <= 13, whose 6-tap support (-15 .. +31) stays inside the window.
+            enc.encode(f0, True)                                        # the same parameter sets: parsed once
+            p = parser.picture(enc.encode(f1, False)[0])
             interior = 0
             for m in p.mbs:
                 mbx, mby = m.addr % mbw, m.addr // mbw
-                assert m.kind in ("P_Skip", "P_L0_16x16") and m.cbp == 0, (mv, mbx, mby, m.kind, m.cbp, m.mv)
-                if 16 <= 16 * mbx and 16 * mbx + 32 <= w and 16 <= 16 * mby and 16 * mby + 32 <= h:
+                inside = _interior(mbx, mby, mv, w, h, wide)
+                if wide and (mv[0] | mv[1]) & 3 and M.anchor_of(mbx, mby, mbw, 0, mbh) != (mbx, mby):
+                    inside = False          # a far fractional vector is the anchors' alone: see the docstring
+                if inside or not wide:
+                    assert m.kind in ("P_Skip", "P_L0_16x16") and m.cbp == 0, (mv, mbx, mby, m.kind, m.cbp, m.mv)
+                if inside:
                     assert m.mv == mv, (mv, mbx, mby, m.mv)
                     interior += 1
-            assert interior == (mbw - 2) * (mbh - 2)
+            assert interior == (mbw - 2) * (mbh - 2) if not wide else interior >= 4, (mv, interior)
     finally:
         enc.close()
 
@@ -415,19 +576,32 @@ def test_oracle_motion_recovery():
     motion_recovery(OracleEnc)
 
 
-def search_optimality(make_enc, w, h, stripe_rows=0, qp=28):
-    """A cut to new structured content (a gradient with noise, still for one picture, then translated by a known vector plus
-    mild noise).  On the translated picture the anchors search (§5.3).  For every anchor the model shows did search —
-    SAD(0,0) above 96·λ and the temporal predictor (its previous vector) more than 4·96·λ off — the documented cost of the coded
-    vector is at most the brute-force minimum over the window, and equal to it when the vector is full-sample."""
+@pytest.mark.parametrize("w,h,shifts,gate_at", [(448, 128, WIDE_SHIFTS_ACROSS, (13, 1)), (96, 640, WIDE_SHIFTS_DOWN, None)],
+                         ids=["across", "down"])
+def test_oracle_wide_motion_recovery(w, h, shifts, gate_at):
+    motion_recovery(OracleEnc, w=w, h=h, wide=True, shifts=shifts, gate_at=gate_at)
+
+
+def search_optimality(make_enc, w, h, stripe_rows=0, qp=28, wide=False, shift=(-5, 7), blocky=False):
+    """A cut to new structured content (a gradient with noise, or 2x2-blocky noise, still for one picture, then translated by
+    `shift` px plus mild noise).  On the translated picture the anchors search (§5.3).  For every anchor the model shows did
+    search — SAD(0,0) above 96·λ and the temporal predictor (its previous vector) more than 4·96·λ off — the documented cost of
+    the coded vector is at most the brute-force minimum over the window, and equal to it when the vector is full-sample.
+    wide: with wide-range motion, over the co-located window and the window around the model's coarse vector × 4 (when §5.3
+    searches it), vectors outside the range left out; and the coded vector's full-sample part lies in one of them."""
     rng = np.random.default_rng(5)
-    yy, xx = np.mgrid[0:h + 64, 0:w + 64]
-    base = 40 + (xx * 3 + yy * 2) % 150 + rng.integers(0, 30, xx.shape)
+    sx, sy = shift
+    ox, oy = max(24, -sx), max(20, -sy)                                  # the still picture's corner in the content
+    yy, xx = np.mgrid[0:oy + max(sy, 44) + h, 0:ox + max(sx, 40) + w]
+    if blocky:
+        base = rng.integers(40, 200, ((yy.shape[0] + 1) // 2, (xx.shape[1] + 1) // 2)).repeat(2, 0).repeat(2, 1)[:yy.shape[0], :xx.shape[1]]
+    else:
+        base = 40 + (xx * 3 + yy * 2) % 150 + rng.integers(0, 30, xx.shape)
     mild = lambda: rng.integers(-2, 3, (h, w))
     inv = grey_table()
-    still = grey(w, h, inv, np.clip(base[20:20 + h, 24:24 + w], 16, 235))
-    moved = grey(w, h, inv, np.clip(base[20 + 7:27 + h, 24 - 5:19 + w] + mild(), 16, 235))
-    enc = make_enc(w, h, qp, stripe_rows=stripe_rows)
+    still = grey(w, h, inv, np.clip(base[oy:oy + h, ox:ox + w], 16, 235))
+    moved = grey(w, h, inv, np.clip(base[oy + sy:oy + sy + h, ox + sx:ox + sx + w] + mild(), 16, 235))
+    enc = make_enc(w, h, qp, stripe_rows=stripe_rows, wide=wide)
     try:
         streams = {}
         for i, f in enumerate([still, still, moved]):
@@ -435,7 +609,7 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28):
                 streams.setdefault(y0, []).append(au)
     finally:
         enc.close()
-    lam, checked, anchors = M.LAMBDA[qp], 0, 0
+    lam, checked, anchors, far = M.LAMBDA[qp], 0, 0, 0
     cw, ch = (w + 15) // 16 * 16, (h + 15) // 16 * 16
     sources = [source_nv12(f, cw, ch) for f in (still, still, moved)]
     for y0, aus in streams.items():
@@ -448,20 +622,31 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28):
         prev_mbs = pics[1].mbs if len(pics) == 3 else [Mb(a, 0, "P_Skip", qp) for a in range(mbw * mbh)]
         # the coded-size reference of the band (or picture): a band's stream clamps at the band's own edges
         ref = rec[0]
-        sy = band[2][0].astype(np.int64)
+        cur = band[2][0].astype(np.int64)
+        dec_cur, dec_ref = M.decimate(band[2][0]), M.decimate(band[1][0])      # the reference is picture 1, still
         early = M.EARLY_SAD_PER_LAMBDA * lam
         for m in pics[-1].mbs:
             mbx, mby = m.addr % mbw, m.addr // mbw
             if M.anchor_of(mbx, mby, mbw, 0, mbh) != (mbx, mby) or m.kind == "I_PCM":
                 continue
             anchors += 1
-            blk = sy[16 * mby:16 * mby + 16, 16 * mbx:16 * mbx + 16]
+            blk = cur[16 * mby:16 * mby + 16, 16 * mbx:16 * mbx + 16]
             costs = M.full_search(blk, ref, 16 * mbx, 16 * mby, qp)
             prev = prev_mbs[m.addr]
             pv = ((prev.mv[0] + 2) >> 2, (prev.mv[1] + 2) >> 2) if not prev.intra else None
             if costs[(0, 0)][0] <= early or (pv in costs and costs[pv][0] <= 4 * early):
                 continue
             checked += 1
+            if wide:
+                coarse = M.coarse_search(dec_cur, dec_ref, mbx, mby, mbw, 0, mbh, costs[(0, 0)][0], qp)
+                centre = M.second_window(coarse)
+                if centre is not None:
+                    costs.update(M.full_search(blk, ref, 16 * mbx, 16 * mby, qp, centre=centre))
+                    far += 1
+                # the full-sample position the refinement started from: within 3 quarter samples of the coded vector
+                near = [(fx, fy) for fx in {m.mv[0] >> 2, -(-m.mv[0] // 4)} for fy in {m.mv[1] >> 2, -(-m.mv[1] // 4)}
+                        if abs(m.mv[0] - 4 * fx) <= 3 and abs(m.mv[1] - 4 * fy) <= 3]
+                assert any(v in costs for v in near), (y0, mbx, mby, m.mv, coarse)
             best = min(c for _, c in costs.values())
             pred = M.luma_inter(ref, 16 * mbx, 16 * mby, m.mv)
             cost = M.motion_cost(M.sad(blk, pred), m.mv, qp)
@@ -470,11 +655,23 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28):
             else:
                 assert cost == best, (y0, mbx, mby, m.mv, cost, best)
     assert anchors and checked >= 0.75 * anchors, (checked, anchors)
+    assert far or not wide
 
 
 @pytest.mark.parametrize("w,h,stripe_rows", [(130, 70, 0), (200, 112, 3)])
 def test_oracle_search_optimality(w, h, stripe_rows):
     search_optimality(OracleEnc, w, h, stripe_rows)
+
+
+# The cut translated by large vectors (px); in bands of 3 rows, whose edges clamp the coarse search; and 2x2-blocky noise moved 256 px
+# down, one row past the vector range: the coarse window's first row (dy = -64) is its only decimated match.
+WIDE_OPTIMALITY = [(192, 176, 0, (-45, 70), False), (256, 96, 0, (90, -30), False), (256, 144, 3, (-70, 21), False),
+                   (64, 448, 0, (0, -256), True)]
+
+
+@pytest.mark.parametrize("w,h,stripe_rows,shift,blocky", WIDE_OPTIMALITY)
+def test_oracle_wide_search_optimality(w, h, stripe_rows, shift, blocky):
+    search_optimality(OracleEnc, w, h, stripe_rows, wide=True, shift=shift, blocky=blocky)
 
 
 # ------------------------------------------------------------------------------------------------ level_idc (Table A-1)

@@ -15,13 +15,14 @@ def _session(cfg: S.Config) -> Session:
     p = cfg.paint
     return Session(cfg.width, cfg.height, fps=cfg.fps, rc_mode=cfg.rc_mode, bitrate_kbps=cfg.kbps, crf=cfg.qp,
                    slice_rows=cfg.slice_rows, idr_slice_mbs=cfg.idr_slice_mbs, stripe_rows=cfg.stripe_rows,
-                   paintover_trigger_frames=p[0], paintover_crf=p[1], paintover_burst_frames=p[2])
+                   paintover_trigger_frames=p[0], paintover_crf=p[1], paintover_burst_frames=p[2], flags=cfg.flags)
 
 
 def encode_gpu(cfg: S.Config, frames, idr_at=(0,), qps=None) -> D.Encoded:
     with _session(cfg) as s:
         cw, ch = s.coded_size()
         out = D.Encoded(cfg.width, cfg.height, cw, ch)
+        out.wide = s.wide_motion
         for i, f in enumerate(frames):
             if i in idr_at and i > 0:
                 s.flush()
@@ -42,8 +43,8 @@ def encode_gpu(cfg: S.Config, frames, idr_at=(0,), qps=None) -> D.Encoded:
 class GpuEnc:
     """One CQP session, picture by picture (the D.OracleEnc interface)."""
 
-    def __init__(self, w, h, qp, slice_rows=0, stripe_rows=0):
-        self.s = Session(w, h, rc_mode=N.B2V_RC_CQP, crf=qp, slice_rows=slice_rows, stripe_rows=stripe_rows)
+    def __init__(self, w, h, qp, slice_rows=0, stripe_rows=0, wide=False):
+        self.s = Session(w, h, rc_mode=N.B2V_RC_CQP, crf=qp, slice_rows=slice_rows, stripe_rows=stripe_rows, wide_motion=wide)
         self.first = True
 
     def encode(self, frame, idr):
@@ -66,7 +67,7 @@ def test_gpu_decisions(case):
     e, st = D.run_case(encode_gpu, case)
     D.check_recon(e, st)
     assert st.pictures >= len(case[2])
-    if case[0] == "pcm_noise_qp0_4":
+    if case[0] in ("pcm_noise_qp0_4", "wide_pcm_noise_qp0_4"):
         assert st.kinds.get("I_PCM", 0) > 0, st.kinds
     if case[0] == "paintover_burst":
         assert st.kinds.get("P_L0_16x16", 0) > 0        # the burst re-codes the still at the paint-over QP
@@ -76,9 +77,20 @@ def test_gpu_motion_recovery():
     D.motion_recovery(GpuEnc)
 
 
+@pytest.mark.parametrize("w,h,shifts,gate_at", [(448, 128, D.WIDE_SHIFTS_ACROSS, (13, 1)), (96, 640, D.WIDE_SHIFTS_DOWN, None)],
+                         ids=["across", "down"])
+def test_gpu_wide_motion_recovery(w, h, shifts, gate_at):
+    D.motion_recovery(GpuEnc, w=w, h=h, wide=True, shifts=shifts, gate_at=gate_at)
+
+
 @pytest.mark.parametrize("w,h,stripe_rows", [(130, 70, 0), (200, 112, 3)])
 def test_gpu_search_optimality(w, h, stripe_rows):
     D.search_optimality(GpuEnc, w, h, stripe_rows)
+
+
+@pytest.mark.parametrize("w,h,stripe_rows,shift,blocky", D.WIDE_OPTIMALITY)
+def test_gpu_wide_search_optimality(w, h, stripe_rows, shift, blocky):
+    D.search_optimality(GpuEnc, w, h, stripe_rows, wide=True, shift=shift, blocky=blocky)
 
 
 @pytest.mark.parametrize("w,h,stripe_rows", [(3840, 64, 0), (3840, 2160, 8)])
