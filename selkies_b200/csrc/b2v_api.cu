@@ -96,7 +96,7 @@ struct Session {
   b2v_settings cfg{};
   int device = 0;
   int src_w = 0, src_h = 0, dst_w = 0, dst_h = 0, coded_w = 0, coded_h = 0;
-  bool encode = true, timing = false, timing_csc_only = false, quality = false, droppable = false, wide_motion = false, long_term_ref = false;
+  bool encode = true, timing = false, timing_csc_only = false;
   cudaStream_t st_copy = nullptr, st_enc = nullptr, st_out = nullptr, st_pack = nullptr;
 
   // ingest ring
@@ -159,6 +159,37 @@ bool size_ok(int w, int h) { return w >= 16 && h >= 16 && w <= 7680 && h <= 4320
 // H.264 striped mode at an encoded height of dst_h rows (the encoder's rule: stripe_rows > 0 and less than the macroblock rows)
 bool stripes_active(int stripe_rows, int dst_h) { return stripe_rows > 0 && stripe_rows < round16(dst_h) / 16; }
 
+// The opt-in H.264 flags and what each combines with (include/b2video.h).  Only check_coding_flags reads this table.
+struct CodingFlagRule {
+  int flag; const char* name;
+  const char* h264;        // null, or why the flag needs H.264 coding (neither B2V_FLAG_JPEG nor B2V_FLAG_NO_ENCODE)
+  bool full_frame;         // refused where stripe_rows stripes the picture: every stripe is a stream of its own
+  int excludes;            // B2V_FLAG_* it never comes with, and why
+  const char* why_excluded;
+};
+constexpr CodingFlagRule kCodingFlags[] = {
+  {B2V_FLAG_QUALITY, "B2V_FLAG_QUALITY", "measures the H.264 reconstruction", false, 0, nullptr},
+  {B2V_FLAG_DROPPABLE, "B2V_FLAG_DROPPABLE", "layers H.264 pictures", true, 0, nullptr},
+  {B2V_FLAG_WIDE_MOTION, "B2V_FLAG_WIDE_MOTION", "searches H.264 P pictures", false, 0, nullptr},
+  {B2V_FLAG_LONG_TERM_REF, "B2V_FLAG_LONG_TERM_REF", "keeps an H.264 reference picture", true, B2V_FLAG_DROPPABLE,
+   "a non-reference picture cannot mark a long-term picture, and its reference is two pictures back"},
+};
+
+// `flags` against the table for a picture of dst_h rows: 0, or B2V_EINVAL naming the flag.  No CUDA call.
+int check_coding_flags(int flags, int stripe_rows, int dst_h) {
+  for (const CodingFlagRule& r : kCodingFlags) {
+    if (!(flags & r.flag)) continue;
+    if (r.h264 && (flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
+      return fail(B2V_EINVAL, "%s %s: %s codes none", r.name, r.h264, (flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
+    for (const CodingFlagRule& o : kCodingFlags)
+      if (flags & r.excludes & o.flag) return fail(B2V_EINVAL, "%s with %s: %s", r.name, o.name, r.why_excluded);
+    if (r.full_frame && stripes_active(stripe_rows, dst_h))
+      return fail(B2V_EINVAL, "%s is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows (every stripe is a "
+                  "stream of its own)", r.name, stripe_rows, round16(dst_h) / 16);
+  }
+  return 0;
+}
+
 int alloc_geometry(Session* s) {
   // (re)allocate everything that depends on the frame size
   s->coded_w = s->encode ? round16(s->dst_w) : s->dst_w;
@@ -194,10 +225,7 @@ int alloc_geometry(Session* s) {
     ec.slice_rows = s->cfg.slice_rows;          // <= 0: the encoder's default rule
     ec.stripe_rows = s->cfg.stripe_rows > 0 ? s->cfg.stripe_rows : 0;
     ec.idr_slice_mbs = s->cfg.idr_slice_mbs;
-    ec.quality = s->quality;
-    ec.droppable = s->droppable;
-    ec.wide_motion = s->wide_motion;
-    ec.long_term_ref = s->long_term_ref;
+    ec.flags = s->cfg.flags;
     int rc = encoder_create(&ec, &s->enc);
     if (rc) return fail(rc, "encoder_create failed: %s", encoder_last_error());
     s->lay = encoder_layout(s->enc);
@@ -695,27 +723,8 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   if (!size_ok(sw, sh)) return fail(B2V_EINVAL, "source size %dx%d unsupported (even, 16..7680 x 16..4320)", sw, sh);
   if (!size_ok(dw, dh)) return fail(B2V_EINVAL, "encoded size %dx%d unsupported", dw, dh);
   if (cfg->idr_slice_mbs < 0) return fail(B2V_EINVAL, "idr_slice_mbs %d out of range (0 = default, n > 0 macroblocks per slice)", cfg->idr_slice_mbs);
-  if ((cfg->flags & B2V_FLAG_QUALITY) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
-    return fail(B2V_EINVAL, "B2V_FLAG_QUALITY measures the H.264 reconstruction: %s has none",
-                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
-  if ((cfg->flags & B2V_FLAG_DROPPABLE) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
-    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE layers H.264 pictures: %s codes none",
-                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
-  if ((cfg->flags & B2V_FLAG_WIDE_MOTION) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
-    return fail(B2V_EINVAL, "B2V_FLAG_WIDE_MOTION searches H.264 P pictures: %s codes none",
-                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
-  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && (cfg->flags & (B2V_FLAG_JPEG | B2V_FLAG_NO_ENCODE)))
-    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF keeps an H.264 reference picture: %s codes none",
-                (cfg->flags & B2V_FLAG_JPEG) ? "B2V_FLAG_JPEG" : "B2V_FLAG_NO_ENCODE");
-  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && (cfg->flags & B2V_FLAG_DROPPABLE))
-    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF with B2V_FLAG_DROPPABLE: a non-reference picture cannot mark a long-term "
-                "picture, and its reference is two pictures back");
-  if ((cfg->flags & B2V_FLAG_LONG_TERM_REF) && stripes_active(cfg->stripe_rows, dh))
-    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
-                "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
-  if ((cfg->flags & B2V_FLAG_DROPPABLE) && stripes_active(cfg->stripe_rows, dh))
-    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d stripes a picture of %d macroblock rows "
-                "(every stripe is a stream of its own)", cfg->stripe_rows, round16(dh) / 16);
+  int rc = check_coding_flags(cfg->flags, cfg->stripe_rows, dh);
+  if (rc) return rc;
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(B2V_EINVAL, "device %d out of range (%d devices)", cfg->device, ndev);
@@ -725,10 +734,6 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->src_w = sw; s->src_h = sh; s->dst_w = dw; s->dst_h = dh;
   s->encode = !(cfg->flags & B2V_FLAG_NO_ENCODE);
   s->jpeg = (cfg->flags & B2V_FLAG_JPEG) != 0;
-  s->quality = (cfg->flags & B2V_FLAG_QUALITY) != 0;
-  s->droppable = (cfg->flags & B2V_FLAG_DROPPABLE) != 0;
-  s->wide_motion = (cfg->flags & B2V_FLAG_WIDE_MOTION) != 0;
-  s->long_term_ref = (cfg->flags & B2V_FLAG_LONG_TERM_REF) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;
@@ -755,7 +760,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   cudaEventCreateWithFlags(&s->ev_dev_in, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&s->ev_dev_done, cudaEventDisableTiming);
   if (s->timing && (cfg->flags & B2V_FLAG_DEVICE_TIMER)) cudaMalloc((void**)&s->d_csc_ts, sizeof(unsigned long long) * 2 * kMaxSlots);
-  int rc = alloc_geometry(s);
+  rc = alloc_geometry(s);
   if (rc) { release_session(s); return rc; }
   s->out_thread = std::thread(output_loop, s);
   *out = s;
@@ -927,12 +932,8 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   if (dw <= 0) dw = sw;
   if (dh <= 0) dh = sh;
   if (!size_ok(sw, sh) || !size_ok(dw, dh)) return fail(B2V_EINVAL, "size unsupported");
-  if (s->droppable && stripes_active(s->cfg.stripe_rows, dh))
-    return fail(B2V_EINVAL, "B2V_FLAG_DROPPABLE is full-frame only: stripe_rows %d would stripe a picture of %d macroblock rows",
-                s->cfg.stripe_rows, round16(dh) / 16);
-  if (s->long_term_ref && stripes_active(s->cfg.stripe_rows, dh))
-    return fail(B2V_EINVAL, "B2V_FLAG_LONG_TERM_REF is full-frame only: stripe_rows %d would stripe a picture of %d macroblock rows",
-                s->cfg.stripe_rows, round16(dh) / 16);
+  int rc = check_coding_flags(s->cfg.flags, s->cfg.stripe_rows, dh);
+  if (rc) return rc;
   // Submitters are locked out FIRST; then everything in flight drains (the output thread needs `mu`, not `submit_mu`, so it
   // keeps delivering); a producer still holding an acquired slot would be writing into memory about to be freed: refuse.
   std::lock_guard<std::mutex> sub(s->submit_mu);
@@ -948,7 +949,7 @@ int b2v_set_resolution(void* h, int32_t sw, int32_t sh, int32_t dw, int32_t dh) 
   CK(cudaDeviceSynchronize());
   free_geometry(s);
   s->src_w = sw; s->src_h = sh; s->dst_w = dw; s->dst_h = dh;
-  const int rc = alloc_geometry(s);
+  rc = alloc_geometry(s);
   std::lock_guard<std::mutex> lk(s->mu);
   if (rc) {                      // half-allocated buffers: the session cannot run any more, every later call says why
     s->failed = true;

@@ -123,7 +123,7 @@ std::vector<uint8_t> make_param_sets(const EncoderConfig& c, int mbw, int mbh, i
   b.ue(0);                 // seq_parameter_set_id
   b.ue(4);                 // log2_max_frame_num_minus4
   b.ue(2);                 // pic_order_cnt_type
-  b.ue(c.long_term_ref ? 2 : 1);   // max_num_ref_frames: the previous picture, and with B2V_FLAG_LONG_TERM_REF a long-term one
+  b.ue((c.flags & B2V_FLAG_LONG_TERM_REF) ? 2 : 1);   // max_num_ref_frames: the previous picture, and the long-term one
   b.put(1, 0);             // gaps_in_frame_num_value_allowed_flag
   b.ue(mbw - 1); b.ue(mbh - 1);
   b.put(1, 1);             // frame_mbs_only_flag
@@ -142,7 +142,7 @@ std::vector<uint8_t> make_param_sets(const EncoderConfig& c, int mbw, int mbh, i
   b.ue(0); b.ue(0);        // max_bytes_per_pic_denom, max_bits_per_mb_denom
   b.ue(10); b.ue(10);      // log2_max_mv_length_horizontal / vertical
   b.ue(0);                 // max_num_reorder_frames
-  b.ue(c.long_term_ref ? 2 : 1);   // max_dec_frame_buffering
+  b.ue((c.flags & B2V_FLAG_LONG_TERM_REF) ? 2 : 1);   // max_dec_frame_buffering
   b.trailing();
   append_nal(out, 3, 7, b.buf);
   HostBits p;
@@ -192,19 +192,19 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     e->idr_grid = slice_grid(e->mbw, e->mbh, 1, cols);
   }
   const size_t mbs = (size_t)e->mbw * e->mbh, fb = (size_t)cfg->coded_w * cfg->coded_h * 3 / 2;
-  e->n_recon = cfg->droppable ? 3 : 2;
+  e->n_recon = (cfg->flags & B2V_FLAG_DROPPABLE) ? 3 : 2;
   for (int b = 0; b < e->n_recon; b++) {
     ECK(cudaMalloc((void**)&e->recon[b], fb));
     ECK(cudaMemset(e->recon[b], 0, fb));
   }
-  if (cfg->wide_motion) {
+  if (cfg->flags & B2V_FLAG_WIDE_MOTION) {
     for (int b = 0; b < e->n_recon; b++) {
       ECK(cudaMalloc((void**)&e->dec[b], fb / 24));      // fb / 24 = (coded_w / 4) x (coded_h / 4)
       ECK(cudaMemset(e->dec[b], 0, fb / 24));
     }
     ECK(cudaMalloc((void**)&e->coarse, mbs * sizeof(int)));
   }
-  if (cfg->long_term_ref) {
+  if (cfg->flags & B2V_FLAG_LONG_TERM_REF) {
     ECK(cudaMalloc((void**)&e->lt, fb));
     ECK(cudaMemset(e->lt, 0, fb));
     ECK(cudaMalloc((void**)&e->ltr, sizeof(LtrState)));
@@ -249,11 +249,6 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
   // bands: full-frame coding is one band of mbh rows; striped mode gives every band its own SPS (height = the band's)
   const int crop_b = (cfg->coded_h - cfg->height) / 2;
   e->striped = cfg->stripe_rows > 0 && cfg->stripe_rows < e->mbh;
-  if (e->striped && cfg->droppable) { snprintf(g_enc_err, sizeof g_enc_err, "non-reference pictures are not coded in striped mode"); encoder_destroy(e); return -1; }
-  if (cfg->long_term_ref && (e->striped || cfg->droppable)) {
-    snprintf(g_enc_err, sizeof g_enc_err, "a long-term reference is not kept in striped mode or with non-reference pictures");
-    encoder_destroy(e); return -1;
-  }
   if (e->striped && cfg->stripe_rows % cfg->slice_rows) { snprintf(g_enc_err, sizeof g_enc_err, "stripe_rows must be a multiple of slice_rows"); encoder_destroy(e); return -1; }
   e->band_rows = e->striped ? cfg->stripe_rows : e->mbh;
   e->n_bands = (e->mbh + e->band_rows - 1) / e->band_rows;
@@ -265,7 +260,7 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     ps.insert(ps.end(), last.begin(), last.end());
     e->au_data_off = (int)sizeof(AuHeader) + ((e->n_bands * (int)sizeof(BandEntry) + 16 + 63) & ~63);
   }
-  if (cfg->quality) {     // the quality table sits between the band table (if any) and the first data byte
+  if (cfg->flags & B2V_FLAG_QUALITY) {     // the quality table sits between the band table (if any) and the first data byte
     e->quality_off = e->au_data_off;
     e->au_data_off += (e->n_bands * (int)sizeof(QualityEntry) + 63) & ~63;
     ECK(cudaMalloc((void**)&e->q_acc, e->n_bands * sizeof(QualityEntry)));
@@ -313,7 +308,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   if (idr) { e->frame_num = 0; e->since_idr = 0; }
   // B2V_FLAG_DROPPABLE: counted from the IDR, every P picture at an odd count is a non-reference picture.  Every P picture predicts
   // from the last reference picture: the one just before it, or two before it when that one was a non-reference picture.
-  const bool is_ref = !e->cfg.droppable || idr || (e->since_idr & 1) == 0;
+  const bool is_ref = !(e->cfg.flags & B2V_FLAG_DROPPABLE) || idr || (e->since_idr & 1) == 0;
   const int ref_dist = e->last_was_ref ? 1 : 2;
   // the buffer this picture writes: neither the last picture's reconstruction nor this picture's reference (see the schedule below)
   int wb = 0;
@@ -335,8 +330,8 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.band_rows = e->band_rows; f.n_bands = e->n_bands; f.striped = e->striped; f.param_len_last = e->param_len_last;
   f.band_fn = e->band_fn; f.band_coded = e->band_coded; f.au_data_off = e->au_data_off;
   f.param_sets = e->param_sets; f.param_len = e->param_len; f.csc_ts = p->csc_ts; f.au = p->au; f.overflow = e->overflow;
-  if (e->cfg.wide_motion) { f.wide = 1; f.dec_cur = e->dec[wb]; f.dec_ref = e->dec[e->ref_buf]; f.coarse = e->coarse; }
-  if (e->cfg.long_term_ref) { f.ltr = e->ltr; f.lt = e->lt; f.ltr_epoch = e->idr_count; f.prev_idr = e->since_idr == 1; }
+  if (e->cfg.flags & B2V_FLAG_WIDE_MOTION) { f.wide = 1; f.dec_cur = e->dec[wb]; f.dec_ref = e->dec[e->ref_buf]; f.coarse = e->coarse; }
+  if (e->cfg.flags & B2V_FLAG_LONG_TERM_REF) { f.ltr = e->ltr; f.lt = e->lt; f.ltr_epoch = e->idr_count; f.prev_idr = e->since_idr == 1; }
   int n = 0;
   // Two-stream schedule (no per-stage events requested): ANALYSIS of picture k on `st` (CSC before it, by the caller), ENTROPY
   // coding of picture k (CAVLC, slice build with the rate-control step, pack) on `st_pack`, overlapping

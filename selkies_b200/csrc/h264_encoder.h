@@ -17,10 +17,11 @@ struct EncoderConfig {
   int slice_rows;          // macroblock rows per slice
   int stripe_rows;         // macroblock rows per band (multiple of slice_rows); 0 = full-frame
   int idr_slice_mbs;       // IDR pictures, whatever slice_rows is: macroblocks per slice inside a row; 0 = default rule (>= 0)
-  bool quality;            // B2V_FLAG_QUALITY: k_quality measures every band into the access unit's quality table
-  bool droppable;          // B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture (full frame only)
-  bool wide_motion;        // B2V_FLAG_WIDE_MOTION: coarse vectors per anchor group (k_coarse) and windows centred on far candidates
-  bool long_term_ref;      // B2V_FLAG_LONG_TERM_REF: one long-term reference picture, marked on the GPU (k_ltr_mark; full frame only)
+  int flags;               // the session's B2V_FLAG_*, a combination check_coding_flags (b2v_api.cu) allows.  The encoder reads:
+                           //   B2V_FLAG_QUALITY: k_quality measures every band into the access unit's quality table
+                           //   B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture
+                           //   B2V_FLAG_WIDE_MOTION: coarse vectors per anchor group (k_coarse) and windows centred on far candidates
+                           //   B2V_FLAG_LONG_TERM_REF: one long-term reference picture, marked on the GPU (k_ltr_mark)
 };
 
 struct EncodeFrameParams {

@@ -672,39 +672,25 @@ cudaError_t inter_search_grid(int* blocks) {
   return e;
 }
 
+// The three passes of a P picture: SCALE, the previous picture's vectors span another reference distance than this picture's
+// (B2V_FLAG_DROPPABLE); WIDE, B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream); LTR, B2V_FLAG_LONG_TERM_REF.
+template <bool SCALE, bool WIDE, bool LTR>
+void launch_passes(const FrameCtx& f, int lean_blocks, cudaStream_t st) {
+  k_inter_lean<SCALE, WIDE, LTR><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+  k_inter_search<SCALE, WIDE><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
+  k_inter_search<SCALE, WIDE><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+}
+
 int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
   const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  if (f.ltr) {                              // B2V_FLAG_LONG_TERM_REF (never with B2V_FLAG_DROPPABLE: both distances are 1)
-    if (f.wide) k_inter_lean<false, true, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    else k_inter_lean<false, false, true><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    if (f.wide) {
-      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
-    } else {
-      k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-      k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
-    }
-  } else if (f.wide) {                      // B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream)
-    if (f.ref_dist == f.prev_ref_dist) {
-      k_inter_lean<false, true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-      k_inter_search<false, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
-    } else {
-      k_inter_lean<true, true, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-      k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-      k_inter_search<true, true><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
-    }
-  } else if (f.ref_dist == f.prev_ref_dist) {      // every picture without B2V_FLAG_DROPPABLE
-    k_inter_lean<false, false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
-    k_inter_search<false, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
-  } else {
-    k_inter_lean<true, false, false><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-    k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
-    k_inter_search<true, false><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
-  }
+  // The long-term reference never comes with droppable pictures (check_coding_flags), so with it both distances are 1: LTR
+  // implies !SCALE, and no <true, *, true> variant is compiled.
+  const bool scale = f.ref_dist != f.prev_ref_dist;
+  if (f.ltr) f.wide ? launch_passes<false, true, true>(f, lean_blocks, st) : launch_passes<false, false, true>(f, lean_blocks, st);
+  else if (scale) f.wide ? launch_passes<true, true, false>(f, lean_blocks, st) : launch_passes<true, false, false>(f, lean_blocks, st);
+  else f.wide ? launch_passes<false, true, false>(f, lean_blocks, st) : launch_passes<false, false, false>(f, lean_blocks, st);
   return 3;
 }
 

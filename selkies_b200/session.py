@@ -164,6 +164,11 @@ def tensor_frame_args(frame, width: int, height: int, device: int, *, channels: 
     return t, _producer_stream(frame, cai, torch, stream)
 
 
+# the opt-in H.264 flags: Session keyword and attribute -> B2V_FLAG_* bit
+_OPT_IN_FLAGS = {"quality": N.B2V_FLAG_QUALITY, "droppable": N.B2V_FLAG_DROPPABLE, "wide_motion": N.B2V_FLAG_WIDE_MOTION,
+                 "long_term_ref": N.B2V_FLAG_LONG_TERM_REF}
+
+
 class Session:
     def __init__(self, width: int, height: int, *, dst_width: int = 0, dst_height: int = 0, fps: float = 60.0,
                  device: int = 0, rc_mode: int = N.B2V_RC_CBR, bitrate_kbps: int = 8000, crf: int = 26,
@@ -172,18 +177,10 @@ class Session:
                  collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False,
                  long_term_ref: bool = False):
         self._lib = N.lib()
-        if quality:
-            flags |= N.B2V_FLAG_QUALITY
-        if droppable:
-            flags |= N.B2V_FLAG_DROPPABLE
-        if wide_motion:
-            flags |= N.B2V_FLAG_WIDE_MOTION
-        if long_term_ref:
-            flags |= N.B2V_FLAG_LONG_TERM_REF
-        self.quality = bool(flags & N.B2V_FLAG_QUALITY)
-        self.droppable = bool(flags & N.B2V_FLAG_DROPPABLE)
-        self.wide_motion = bool(flags & N.B2V_FLAG_WIDE_MOTION)
-        self.long_term_ref = bool(flags & N.B2V_FLAG_LONG_TERM_REF)   # one earlier picture kept as a long-term reference
+        asked = dict(quality=quality, droppable=droppable, wide_motion=wide_motion, long_term_ref=long_term_ref)
+        for name, bit in _OPT_IN_FLAGS.items():      # the attribute reports the bit, whether the keyword or `flags` set it
+            flags |= bit if asked[name] else 0
+            setattr(self, name, bool(flags & bit))
         self._hdr_len = 10 if header_mode == N.B2V_HDR_PIXELFLUX else 0
         self.device = device
         self.width, self.height = width, height
