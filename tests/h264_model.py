@@ -206,11 +206,17 @@ def cavlc_bits(scan, chroma_dc=False):
     return bits
 
 
+def header_budget(m, wide=False):
+    """§5.7 / §5.3 / §5.13: the bits budgeted for everything of macroblock `m` before its residual — mb_type, ref_idx_l0 (one bit in a
+    picture with two references), mvd, coded_block_pattern and mb_qp_delta: 48, 96 for Intra4x4 (its prediction modes), 48 more for
+    a P macroblock of a wide-motion picture."""
+    return HEADER_BITS + (HEADER_BITS if m.kind == "I_NxN" else 0) + (WM_MVD_BITS if wide and not m.intra else 0)
+
+
 def mb_size_estimate(m, wide=False):
     """§5.7 / §5.3: the size the encoders give a parsed macroblock `m` (not I_PCM, not P_Skip) when they decide whether to send it
-    raw: its coded blocks by cavlc_bits, plus the header budget — 48 bits, 96 for Intra4x4, 48 more for a P macroblock of a
-    wide-motion picture.  Above 3200 the macroblock is I_PCM."""
-    bits = HEADER_BITS + (HEADER_BITS if m.kind == "I_NxN" else 0) + (WM_MVD_BITS if wide and not m.intra else 0)
+    raw: its coded blocks by cavlc_bits, plus header_budget().  Above 3200 the macroblock is I_PCM."""
+    bits = header_budget(m, wide)
     i16 = m.kind == "I_16x16"
     if i16:
         bits += cavlc_bits(m.luma_dc)
@@ -534,3 +540,135 @@ def second_window(coarse):
         return None
     cx, cy = 4 * coarse[0], 4 * coarse[1]
     return None if -12 <= cx <= 11 and -12 <= cy <= 12 else (cx, cy)
+
+
+# ------------------------------------------------------------------------------------------------ the lean pass's exits (§5.3, §5.12, §5.13)
+PRED_SAD_FACTOR = 4              # §5.3: a temporal predictor is taken with a SAD of at most 4·96·λ
+LTR_CHANGED_MIN_DIV, LTR_CHANGED_RATIO = 64, 8      # §5.13: the marking rule
+
+
+def scale_mv(v, num, den):
+    """§5.12: one component of the previous picture's vector, which spanned `den` pictures, as a predictor for a reference `num`
+    pictures back: unchanged, doubled, or halved rounding half away from zero."""
+    if num == den:
+        return v
+    if num > den:
+        return 2 * v
+    return -((-v + 1) >> 1) if v < 0 else (v + 1) >> 1
+
+
+def full_pred(ref, x0, y0, v):
+    """The 16x16 full-sample prediction at (x0, y0) for vector v (full samples), coordinates clamped to the plane (8.4.2.2.1)."""
+    h, w = ref.shape
+    ys, xs = np.clip(np.arange(y0 + v[1], y0 + v[1] + 16), 0, h - 1), np.clip(np.arange(x0 + v[0], x0 + v[0] + 16), 0, w - 1)
+    return ref[np.ix_(ys, xs)].astype(np.int64)
+
+
+def predictor_candidate(mv, wide):
+    """§5.3: the previous vector `mv` (quarter samples, already scaled) rounded to the full-sample candidate k = ((mv + 2) >> 2), and
+    the centre of the window its test runs in: (0, 0) when k lies in the co-located window's test range (x in [-15, 14], y in
+    [-15, 15], so that its 8 neighbours are in the window too); with wide motion, outside that range and within the vector range,
+    the window re-centred on (kx & ~3, ky).  None: the predictor is not tested."""
+    k = ((mv[0] + 2) >> 2, (mv[1] + 2) >> 2)
+    if -15 <= k[0] <= 14 and -15 <= k[1] <= 15:
+        return k, (0, 0)
+    if wide and mv_ok(*k):
+        return k, (k[0] & ~3, k[1])
+    return None
+
+
+def predictor_test(src_blk, ref, x0, y0, k, centre, sad0, qp):
+    """§5.3: the 3x3 test of full-sample candidate k (real vector) in the window centred on `centre`.  Every position's key is
+    cost << 11 | index, cost = SAD + λ·(bits(4x) + bits(4y)) of the real vector and index = (y − cy + 16)·32 + (x − cx + 16) relative
+    to the window, so equal costs go to the lower row, then the lower column.  Taken when the candidate's SAD ≤ 4·96·λ, its key is
+    below all 8 neighbours' (a strict local minimum) and at most the zero vector's key0 = (sad0 + 2λ) << 11 | 528."""
+    lam = LAMBDA[qp]
+    keys = {}
+    for j in (-1, 0, 1):
+        for i in (-1, 0, 1):
+            v = (k[0] + i, k[1] + j)
+            s = sad(src_blk, full_pred(ref, x0, y0, v))
+            keys[(i, j)] = (s, (s + lam * (se_bits(4 * v[0]) + se_bits(4 * v[1]))) << 11 | (v[1] - centre[1] + 16) * 32 + (v[0] - centre[0] + 16))
+    sadc, kc = keys.pop((0, 0))
+    key0 = (sad0 + 2 * lam) << 11 | (16 * 32 + 16)
+    return sadc <= PRED_SAD_FACTOR * EARLY_SAD_PER_LAMBDA * lam and all(kc < kk for _, kk in keys.values()) and kc <= key0
+
+
+class Exit:
+    """The lean pass's class of one macroblock (lean_exit) and what it allows the coded macroblock to be.  cls: "zero", "predictor",
+    "long-term" or "searched".  k: the predictor's full-sample candidate (or None); frac: the previous vector was fractional;
+    lean: the lean pass took the predictor (otherwise the search pass did, on the clamped window, with its refinement)."""
+
+    def __init__(self, cls, k=None, frac=False, lean=False, search_pred=False):
+        self.cls, self.k, self.frac, self.lean = cls, k, frac, lean
+        self.search_pred = search_pred          # "long-term": the search pass's predictor test would have hit
+
+    def allows(self, kind, ref_idx, mv):
+        """True when a coded macroblock (parsed kind, refIdx, vector in quarter samples) is what this class allows.  I_PCM overrides
+        every class."""
+        if kind == "I_PCM":
+            return True
+        if self.cls == "long-term":
+            return kind == "P_L0_16x16" and ref_idx == 1 and mv == (0, 0)
+        if ref_idx != 0:
+            return False
+        if self.cls == "zero":
+            return mv == (0, 0)
+        if self.cls == "predictor":
+            if not self.frac:
+                return mv == (4 * self.k[0], 4 * self.k[1])
+            return abs(mv[0] - 4 * self.k[0]) <= 3 and abs(mv[1] - 4 * self.k[1]) <= 3
+        return True
+
+
+def lean_exit(src_blk, ref, lt, prev, x0, y0, qp, wide=False, dist=(1, 1)):
+    """§5.3 / §5.12 / §5.13: the class of the macroblock at (x0, y0) with source luma `src_blk`.  ref: the model's reconstruction of
+    refIdx 0 (luma); lt: the long-term picture's (None while there is none); prev: the previous picture's parsed record at this
+    address (None after nothing); dist: (ref_dist, prev_ref_dist) of §5.12.
+      1. zero: SAD(0,0) ≤ 96·λ.
+      2. the temporal predictor: only a P macroblock record (P_Skip included; intra and I_PCM give none) gives one, its vector scaled
+         by dist and rounded (predictor_candidate), tested by predictor_test.  The lean pass takes a hit only when the window's 48
+         columns lie inside the picture (x0 − 16 + cx ≥ 0, x0 + 32 + cx ≤ width) and the previous vector was full-sample; a hit of
+         a picture-edge macroblock or of a fractional previous vector is the search pass's, on the clamped window (the same test).
+      3. long-term: while there is a long-term picture, its SAD at the zero vector ≤ 96·λ — tried in the lean pass only, so only
+         when 1 and the lean pass's part of 2 failed: an edge or fractional-vector macroblock whose search-pass predictor would hit
+         takes the long-term picture, an inside one whose lean predictor hits never tries it.
+      4. searched: the search passes, with the search pass's predictor hit when there is one."""
+    lam = LAMBDA[qp]
+    thr = EARLY_SAD_PER_LAMBDA * lam
+    sad0 = sad(src_blk, full_pred(ref, x0, y0, (0, 0)))
+    if sad0 <= thr:
+        return Exit("zero")
+    hit = None
+    if prev is not None and prev.kind in ("P_L0_16x16", "P_Skip"):
+        mv = tuple(scale_mv(c, *dist) for c in prev.mv)
+        cand = predictor_candidate(mv, wide)
+        if cand is not None and predictor_test(src_blk, ref, x0, y0, cand[0], cand[1], sad0, qp):
+            inside = x0 - 16 + cand[1][0] >= 0 and x0 + 32 + cand[1][0] <= ref.shape[1]
+            hit = cand[0], bool((mv[0] | mv[1]) & 3), inside
+    if hit is not None and hit[2] and not hit[1]:
+        return Exit("predictor", hit[0], False, lean=True)
+    if lt is not None and sad(src_blk, full_pred(lt, x0, y0, (0, 0))) <= thr:
+        return Exit("long-term", search_pred=hit is not None)
+    if hit is not None:
+        return Exit("predictor", hit[0], hit[1], lean=False)
+    return Exit("searched")
+
+
+def changed_count(src_y, ref_y, qp):
+    """§5.13 changed(k): the macroblocks of a P picture whose co-located SAD against its short-term reference fails the zero-motion
+    exit (> 96·λ), counted from the source luma and the model's reconstruction of the reference."""
+    h, w = src_y.shape
+    d = np.abs(np.asarray(src_y, np.int64) - np.asarray(ref_y, np.int64)).reshape(h // 16, 16, w // 16, 16).sum(axis=(1, 3))
+    return int((d > EARLY_SAD_PER_LAMBDA * LAMBDA[qp]).sum())
+
+
+def marks(changed, changed_prev, mbs):
+    """§5.13: picture k marks picture k − 1 long-term when changed(k) ≥ max(⌈mbs/64⌉, 8·changed(k−1)) (an IDR counts every macroblock)."""
+    return changed >= max(-(-mbs // LTR_CHANGED_MIN_DIV), LTR_CHANGED_RATIO * changed_prev)
+
+
+def marking_ops(long_term_exists):
+    """§5.13: the operations of a marking picture — MMCO 1 on the picture two back only while there is no long-term picture (the
+    sliding window holds two short-term frames then), MMCO 4 (one long-term index), MMCO 3 (the previous picture to index 0)."""
+    return ([] if long_term_exists else [(1, 1)]) + [(4, 1), (3, 0, 0)]

@@ -7,7 +7,8 @@ or selkies_b200/.
 
 `parse_stream(aus)` returns what h264_syntax.parse_stream does, and besides: every P picture carries its RefPicList0
 (`Picture.ref_list`: decoding-order indices) and the long-term frames after its marking (`Picture.long_term`), every inter
-macroblock its `ref_idx` and the picture it predicts from (`Mb.ref_pic`), and a slice header its override (`num_ref_idx_active`)
+macroblock its `ref_idx` and the picture it predicts from (`Mb.ref_pic`), every coded macroblock the bits of its header
+(`Mb.header_bits`: everything before the residual), and a slice header its override (`num_ref_idx_active`)
 and its marking operations (`mmco`: (op, args...) tuples) when it has them.  The DPB raises when a stream marks more reference
 frames than max_num_ref_frames or names a picture it does not hold."""
 from __future__ import annotations
@@ -24,6 +25,7 @@ from tests.h264_syntax import SyntaxError_
 class Mb(HS.Mb):
     ref_idx: int = 0             # ref_idx_l0 of an inter macroblock (0 for P_Skip)
     ref_pic: int = -1            # inter macroblock: decoding-order index of the picture RefPicList0[ref_idx] names
+    header_bits: int = 0         # macroblock_layer() bits before the residual: mb_type .. mb_qp_delta (0 for P_Skip and I_PCM)
 
 
 @dataclass
@@ -131,6 +133,7 @@ def _macroblock_layer(b, state, m: Mb, slice_p: bool, qp: int):
     if m.cbp or m.kind == "I_16x16":
         qp = (qp + b.se() + 52) % 52                     # 7.4.5 mb_qp_delta
     m.qp = qp
+    m.header_bits = b.pos - start
     HS._residual(b, state, m, m.kind == "I_16x16")
     m.bits = b.pos - start
     return qp
@@ -297,7 +300,7 @@ class StreamParser:
                     state = HS._PicState(self.sps)
                 hdr = parse_slice(rbsp, t, ref_idc, self.sps, self.pps, state, len(pic.slice_first_mb) if pic else 0)
                 if pic is None:
-                    pic = Picture(self.sps, t == 5, hdr["frame_num"], hdr["qp"])
+                    pic = Picture(self.sps, t == 5, hdr["frame_num"], hdr["qp"], ref_idc)
                 elif hdr["first_mb"] != pic.headers[-1]["end_mb"]:
                     raise SyntaxError_("slices are not contiguous")
                 pic.slice_first_mb.append(hdr["first_mb"])

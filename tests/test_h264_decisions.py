@@ -1,14 +1,20 @@
 """The encoder's decisions, macroblock by macroblock, against a second statement of DESIGN.md §5 that shares no code with either
-encoder: tests/h264_syntax.py parses the bytes, tests/h264_model.py restates prediction, quantisation, decimation and motion
-cost.  Byte parity with the oracle and libavcodec's decode pin conformance; these checks pin what is coded.
+encoder: tests/h264_syntax_refs.py (on tests/h264_syntax.py) parses the bytes and follows the decoded picture buffer,
+tests/h264_model.py restates prediction, quantisation, decimation, motion cost, the lean pass's exits and the long-term marking rule.
+Byte parity with the oracle and libavcodec's decode pin conformance; these checks pin what is coded.
 
 Per stream (one per band in striped mode) and picture:
   - parser self-check: the model's reconstruction from the parsed syntax equals libavcodec's decode of the same bytes;
   - quantisation: every block's parsed levels equal the model's levels for source − prediction (after decimation in P
-    macroblocks), blocks absent from cbp and P_Skip macroblocks included;
-  - A.3.1: every non-PCM macroblock_layer() is at most 3200 bits, every I_PCM sample equals the source;
-  - no P_L0_16x16 macroblock has cbp 0 and its P_Skip vector;
-  - the SPS: profile, constraint flags, level against Table A-1, cropping and the VUI of §5.1.
+    macroblocks), blocks absent from cbp and P_Skip macroblocks included, each inter macroblock predicted from the model's
+    reconstruction of the picture its refIdx names;
+  - A.3.1: every non-PCM macroblock_layer() is at most 3200 bits, its header within the budget of §5.7, every I_PCM sample equals
+    the source;
+  - no refIdx-0 P_L0_16x16 macroblock has cbp 0 and its P_Skip vector;
+  - the lean pass's exits (§5.3, §5.13): every P macroblock's coded refIdx and vector are what its class allows;
+  - the long-term reference (§5.13): the marks, their operations, the override and the picture the DPB names follow the model's
+    rule on the model's own changed(k);
+  - the SPS: profile, constraint flags, level against Table A-1, reference frames, cropping and the VUI of §5.1.
 This file runs them on the oracle's streams; tests/test_h264_decisions_gpu.py on the GPU's."""
 from __future__ import annotations
 
@@ -21,12 +27,15 @@ import pytest
 import oracle
 from oracle import avdec
 from tests import h264_model as M
+from tests import h264_syntax_refs as HSR
 from tests import layered_scenario as LS
+from tests import ltr_content as LC
+from tests import ltr_scenario as LTS
 from tests import scenario as S
 from tests import synth
 from tests import wide_content as WC
 from tests import wide_scenario as WS
-from tests.h264_syntax import BLK_XY, Mb, StreamParser, parse_stream, scan_to_raster, split_annexb
+from tests.h264_syntax import BLK_XY, Mb, StreamParser, scan_to_raster, split_annexb
 
 MAX_MB_BITS = 3200                       # A.3.1
 # Table A-1: level_idc -> MaxFS (macroblocks), levels 3.1 .. 6.2
@@ -58,7 +67,15 @@ class Encoded:
         self.bands = {}
         self.sources = []
         self.recon = None                # the encoder's reconstruction after the last picture
-        self.wide = False                # coded with wide-range motion (B2V_FLAG_WIDE_MOTION)
+        self.flags = 0                   # the session's B2V_FLAG_* word
+
+    @property
+    def wide(self):
+        return bool(self.flags & WS.FLAG_WIDE_MOTION)
+
+    @property
+    def ltr(self):
+        return bool(self.flags & LTS.FLAG_LONG_TERM_REF)
 
     def add(self, index, y_start, au):
         self.bands.setdefault(y_start, []).append((index, au))
@@ -71,7 +88,10 @@ def source_nv12(frame, cw, ch):
 
 
 def oracle_side(cfg: S.Config) -> S.OracleSide:
-    """The oracle side for cfg.flags: wide-range motion (droppable or not), droppable pictures, or neither."""
+    """The oracle side for cfg.flags: the long-term reference (wide motion or not), wide-range motion (droppable or not), droppable
+    pictures, or none of them."""
+    if cfg.flags & LTS.FLAG_LONG_TERM_REF:
+        return LTS.LtrOracleSide(cfg)
     if cfg.flags & WS.FLAG_WIDE_MOTION:
         return WS.WideOracleSide(cfg)
     return LS.LayeredOracleSide(cfg) if cfg.flags & LS.FLAG_DROPPABLE else S.OracleSide(cfg)
@@ -83,7 +103,7 @@ def encode_oracle(cfg: S.Config, frames, idr_at=(0,), qps=None, each=None) -> En
     side = oracle_side(cfg)
     enc = side.enc
     out = Encoded(cfg.width, cfg.height, enc.cw, enc.ch)
-    out.wide = bool(cfg.flags & WS.FLAG_WIDE_MOTION)
+    out.flags = cfg.flags
     for i, f in enumerate(frames):
         if i in idr_at:
             side.control(S.request_idr())
@@ -107,25 +127,37 @@ class Stats:
         self.pictures = 0
         self.levels = []                  # SPS level_idc seen
         self.last = {}                    # band y_start -> the model's last reconstruction (Y, U, V)
+        self.exits = {}                   # lean-pass class (and "predictor lean" / "predictor search" / "long-term over predictor") -> count
+        self.marks = []                   # (band y_start, decoding index) of the pictures that mark a long-term picture
+        self.mmco1_wrap = 0               # marking pictures whose MMCO 1 names a frame across the frame_num wrap
+        self.mark_at_fn0 = 0              # marking pictures with frame_num 0 (MMCO 3 names PicNum -1)
+        self.lt_age = 0                   # the largest distance (pictures) from a long-term picture to a picture predicting from it
+        self.lt_fn_twin = 0               # refIdx-1 macroblocks in pictures whose short-term reference has the long-term frame_num
+        self.skip_next_to_lt = 0          # refIdx-0 P_Skip macroblocks with a refIdx-1 neighbour left or above
+        self.scaled = 0                   # predictor-class macroblocks of pictures whose reference distances differ, previous vector fractional
+        self.pcm_two_refs = 0             # I_PCM macroblocks in pictures with two references
 
-    def count(self, kind):
-        self.kinds[kind] = self.kinds.get(kind, 0) + 1
+    def count(self, kind, d=None):
+        d = self.kinds if d is None else d
+        d[kind] = d.get(kind, 0) + 1
 
 
-def check_sps(sps, width, height, y_start, band_h, mbw, mbh_band, stats):
+def check_sps(sps, width, height, y_start, band_h, mbw, mbh_band, stats, flags=0):
+    """§5.1 (and §5.13 with B2V_FLAG_LONG_TERM_REF: two reference frames, two frames of decoded picture buffer)."""
     stats.levels.append(sps.level_idc)
+    refs = 2 if flags & LTS.FLAG_LONG_TERM_REF else 1
     assert sps.profile_idc == 66 and sps.constraint_flags & 0xC0 == 0xC0, "Constrained Baseline (set0 | set1)"
     assert (sps.mbw, sps.mbh) == (mbw, mbh_band)
     assert sps.width == width and sps.height == band_h, (sps.width, sps.height, width, band_h, y_start)
     assert sps.crop[0] == 0 and sps.crop[2] == 0
-    assert sps.poc_type == 2 and sps.max_num_ref_frames == 1
+    assert sps.poc_type == 2 and sps.max_num_ref_frames == refs
     assert level_ok(sps.level_idc, sps.mbw, sps.mbh), f"level_idc {sps.level_idc} does not hold {sps.mbw}x{sps.mbh} macroblocks"
     assert sps.level_idc == smallest_level(sps.mbw, sps.mbh)
     v = sps.vui
     assert (v.get("video_format"), v.get("video_full_range_flag")) == (5, 0)
     assert (v.get("colour_primaries"), v.get("transfer_characteristics"), v.get("matrix_coefficients")) == (1, 1, 1)
     assert (v.get("chroma_sample_loc_type_top"), v.get("chroma_sample_loc_type_bottom")) == (1, 1)
-    assert (v.get("max_num_reorder_frames"), v.get("max_dec_frame_buffering")) == (0, 1)
+    assert (v.get("max_num_reorder_frames"), v.get("max_dec_frame_buffering")) == (0, refs)
     assert v["timing_info_present_flag"] == 0 and v["nal_hrd"] == 0 and v["vcl_hrd"] == 0
 
 
@@ -140,10 +172,11 @@ def _avail(pic, addr, mbw):
     return M.Avail(ok(-1, 0), ok(0, -1), ok(1, -1), ok(-1, -1))
 
 
-def check_picture(pic, prev, src, where, stats, wide=False):
-    """Reconstructs `pic` from its syntax with the model (prev = the model's reference picture of this stream) and checks every
-    macroblock's levels against the model's levels for the source `src` (Y, U, V of the stream's coded size), and that every
-    macroblock sent coded fits the I_PCM rule's budget (wide: a wide-motion stream).  Returns the reconstruction (Y, U, V)."""
+def check_picture(pic, recs, src, where, stats, wide=False):
+    """Reconstructs `pic` from its syntax with the model (recs: the model's reconstructions of this stream by decoding index; an
+    inter macroblock predicts from recs[m.ref_pic], the picture its refIdx names) and checks every macroblock's levels against the
+    model's levels for the source `src` (Y, U, V of the stream's coded size), and that every macroblock sent coded fits the I_PCM
+    rule's budget, its header included (wide: a wide-motion stream).  Returns the reconstruction (Y, U, V)."""
     mbw, mbh = pic.sps.mbw, pic.sps.mbh
     rec = [np.zeros((mbh * 16, mbw * 16), np.uint8), np.zeros((mbh * 8, mbw * 8), np.uint8), np.zeros((mbh * 8, mbw * 8), np.uint8)]
     sy, su, sv = (p.astype(np.int64) for p in src)
@@ -159,15 +192,18 @@ def check_picture(pic, prev, src, where, stats, wide=False):
             continue
         if m.kind != "P_Skip":
             assert m.bits <= MAX_MB_BITS, f"{at}: macroblock_layer() of {m.bits} bits (A.3.1 limit 3200)"
+            budget = M.header_budget(m, wide)
+            assert m.header_bits <= budget, f"{at}: a header of {m.header_bits} bits (ref_idx {m.ref_idx}, mvd {m.mvd}), budget {budget}"
             est = M.mb_size_estimate(m, wide)
             assert m.bits <= est, f"{at}: {m.bits} bits coded, more than the {est} of the size rule"     # the rule only overstates
             assert est <= MAX_MB_BITS, f"{at}: sized {est} bits by the rule of §5.7 (wide {wide}), coded instead of I_PCM"
             stats.max_bits = max(stats.max_bits, m.bits)
-        if m.kind == "P_L0_16x16":
+        if m.kind == "P_L0_16x16" and m.ref_idx == 0:
             assert not (m.cbp == 0 and m.mv == m.skip_mv), f"{at}: cbp 0 and the P_Skip vector {m.mv}, coded as P_L0_16x16"
         qp, intra = m.qp, m.intra
         av = _avail(pic, m.addr, mbw)
         sblk = sy[y0:y0 + 16, x0:x0 + 16]
+        ref = None if intra else recs[m.ref_pic]
         # ---- luma
         if m.kind == "I_NxN":
             for blk in range(16):
@@ -183,7 +219,7 @@ def check_picture(pic, prev, src, where, stats, wide=False):
             if m.kind == "I_16x16":
                 pred = M.intra16_pred(m.i16_mode, *M.mb_edges(rec[0], x0, y0, 16, av))
             else:
-                pred = M.luma_inter(prev[0], x0, y0, m.mv)
+                pred = M.luma_inter(ref[0], x0, y0, m.mv)
             model = np.zeros((16, 16), np.int64)
             w_dc = np.zeros((4, 4), np.int64)
             for blk in range(16):
@@ -213,7 +249,7 @@ def check_picture(pic, prev, src, where, stats, wide=False):
             if intra:
                 pc = M.chroma_pred(m.chroma_mode, *M.mb_edges(rec[1 + c], xc, yc, 8, av))
             else:
-                pc = M.chroma_inter(prev[1 + c], xc, yc, m.mv)
+                pc = M.chroma_inter(ref[1 + c], xc, yc, m.mv)
             scb = sc[yc:yc + 8, xc:xc + 8]
             w_dc = np.zeros((2, 2), np.int64)
             ac = np.zeros((4, 16), np.int64)
@@ -237,31 +273,102 @@ def check_picture(pic, prev, src, where, stats, wide=False):
     return rec
 
 
+def check_exits(pic, prev, recs, src_y, where, stats, wide=False):
+    """Every macroblock of P picture `pic` against the lean pass's class (M.lean_exit) from the source luma `src_y`, the model's
+    reconstructions of refIdx 0 and of the long-term picture (refIdx 1, while the picture has two references) and the previous
+    picture's parsed records `prev` (the picture just before in decoding order, reference or not): its coded refIdx and vector must
+    be what the class allows."""
+    mbw = pic.sps.mbw
+    ref = recs[pic.ref_list[0]][0]
+    lt = recs[pic.ref_list[1]][0] if len(pic.ref_list) > 1 else None
+    dist = (pic.index - pic.ref_list[0], prev.index - prev.ref_list[0] if prev.ref_list else 1)
+    y = src_y.astype(np.int64)
+    for m in pic.mbs:
+        mbx, mby = m.addr % mbw, m.addr // mbw
+        x0, y0 = 16 * mbx, 16 * mby
+        pm = prev.mbs[m.addr]
+        ex = M.lean_exit(y[y0:y0 + 16, x0:x0 + 16], ref, lt, pm, x0, y0, pic.qp, wide, dist)
+        assert ex.allows(m.kind, m.ref_idx, m.mv), \
+            f"{where} mb ({mbx},{mby}): class {ex.cls} (k {ex.k}, fractional {ex.frac}, lean {ex.lean}) but coded {m.kind} refIdx {m.ref_idx} mv {m.mv}"
+        stats.count(ex.cls, stats.exits)
+        if ex.cls == "predictor":
+            stats.count("predictor lean" if ex.lean else "predictor search", stats.exits)
+            if dist[0] != dist[1] and (pm.mv[0] | pm.mv[1]) & 3:
+                stats.scaled += 1
+        if ex.cls == "long-term" and ex.search_pred:
+            inside = 16 <= x0 and x0 + 32 <= ref.shape[1]
+            stats.count("long-term over edge predictor" if not inside else "long-term over fractional predictor", stats.exits)
+        if m.ref_idx == 1 and pic.ref_frame_nums[0] == pic.ref_frame_nums[1]:
+            stats.lt_fn_twin += 1
+        stats.pcm_two_refs += m.kind == "I_PCM" and lt is not None
+        if m.kind == "P_Skip" and lt is not None:
+            if (mbx > 0 and pic.mbs[m.addr - 1].ref_idx == 1) or (mby > 0 and pic.mbs[m.addr - mbw].ref_idx == 1):
+                stats.skip_next_to_lt += 1
+
+
+class LtrModel:
+    """The long-term reference of §5.13 restated on one stream: the model's changed(k) from the source and the model's reconstruction
+    of picture k − 1, the marking rule, whether a long-term picture exists and which."""
+
+    def __init__(self, mbs):
+        self.mbs, self.prev_changed, self.lt = mbs, mbs, None
+
+    def picture(self, pic, recs, src_y, stats, y_start):
+        """Checks picture `pic`'s marking, operations, override and long-term reference against the rule, then advances."""
+        where = f"picture {pic.index} band {y_start}"
+        if pic.idr:
+            assert all("mmco" not in h and not h.get("long_term_reference_flag") for h in pic.headers), where
+            self.prev_changed, self.lt = self.mbs, None
+            return
+        changed = M.changed_count(src_y, recs[pic.index - 1][0], pic.qp)
+        mark = M.marks(changed, self.prev_changed, self.mbs)
+        for h in pic.headers:
+            assert h.get("mmco") == (M.marking_ops(self.lt is not None) if mark else None), \
+                f"{where}: operations {h.get('mmco')}, the rule says mark {mark} (changed {changed}, before {self.prev_changed})"
+            assert h.get("num_ref_idx_active", 1) == (2 if self.lt is not None else 1), f"{where}: override {h.get('num_ref_idx_active')}"
+        assert pic.ref_list == ([pic.index - 1] + ([self.lt] if self.lt is not None else [])), (where, pic.ref_list, self.lt)
+        if self.lt is not None:
+            stats.lt_age = max(stats.lt_age, pic.index - self.lt)
+        if mark:
+            stats.marks.append((y_start, pic.index))
+            stats.mark_at_fn0 += pic.frame_num == 0
+            if self.lt is None:
+                stats.mmco1_wrap += pic.frame_num < 2
+            self.lt = pic.index - 1
+        assert pic.long_term == ([self.lt] if self.lt is not None else []), (where, pic.long_term, self.lt)
+        self.prev_changed = changed
+
+
 def check_encoded(e: Encoded, stripe_rows=0):
-    """All per-picture checks over every band stream of `e`; returns Stats.  A P picture predicts from the model's reconstruction
-    of the last picture with nal_ref_idc != 0 (two back after a droppable picture)."""
+    """All per-picture checks over every band stream of `e`; returns Stats.  The reader's DPB names the picture each inter
+    macroblock predicts from; the model keeps its reconstructions by decoding index."""
     stats = Stats()
     mbw, mbh = e.cw // 16, e.ch // 16
     for y_start, items in sorted(e.bands.items()):
         band_mbh = min(mbh - y_start // 16, stripe_rows or mbh)
         band_h = min(e.height - y_start, band_mbh * 16)
-        pics = parse_stream([au for _, au in items])
+        pics = HSR.parse_stream([au for _, au in items])
         decoded = avdec.decode_stream([au for _, au in items], quiet=True)
         assert len(decoded) == len(pics)
-        prev = None
-        for (index, _), pic, dec in zip(items, pics, decoded):
+        recs, ltr = [], LtrModel(mbw * band_mbh) if e.ltr else None
+        for k, ((index, _), pic, dec) in enumerate(zip(items, pics, decoded)):
             where = f"picture {index} band {y_start}"
             if pic.idr:
-                check_sps(pic.sps, e.width, e.height, y_start, band_h, mbw, band_mbh, stats)
+                check_sps(pic.sps, e.width, e.height, y_start, band_h, mbw, band_mbh, stats, e.flags)
             assert pic.sps.mbh == band_mbh
-            src = [p[y_start // k: y_start // k + band_mbh * 16 // k] for p, k in zip(e.sources[index], (1, 2, 2))]
-            rec = check_picture(pic, prev, src, where, stats, e.wide)
+            src = [p[y_start // k_: y_start // k_ + band_mbh * 16 // k_] for p, k_ in zip(e.sources[index], (1, 2, 2))]
+            pic.ref_frame_nums = [pics[i].frame_num for i in pic.ref_list]
+            rec = check_picture(pic, recs, src, where, stats, e.wide)
             vh, vw = pic.sps.height, pic.sps.width
-            for k, (r, d) in enumerate(zip(rec, dec)):
-                s = 1 if k == 0 else 2
-                assert np.array_equal(r[: vh // s, : vw // s], d), f"{where}: model reconstruction of plane {k} != libavcodec's decode"
-            if pic.nal_ref_idc:
-                prev = rec
+            for c, (r, d) in enumerate(zip(rec, dec)):
+                s = 1 if c == 0 else 2
+                assert np.array_equal(r[: vh // s, : vw // s], d), f"{where}: model reconstruction of plane {c} != libavcodec's decode"
+            # the exits need the previous picture's records: a band left unsent (all skipped) in between hides them
+            if not pic.idr and k > 0 and items[k - 1][0] == index - 1:
+                check_exits(pic, pics[k - 1], recs, src[0], where, stats, e.wide)
+            if ltr is not None:
+                ltr.picture(pic, recs, src[0], stats, y_start)
+            recs.append(rec)
             stats.pictures += 1
         stats.last[y_start] = rec
     return stats
@@ -318,10 +425,11 @@ def cases():
     out.append(("predictor_paths", S.Config(130, 70, qp=30), synth.predictor_paths(130, 70), (0,), None, 0))
     still = synth.desktop(96, 64, 0)
     out.append(("paintover_burst", S.Config(96, 64, qp=40, paint=(2, 20, 3)), [still] * 8, (0,), None, 0))
-    return out + wide_cases()
+    return out + wide_cases() + ltr_cases()
 
 
 WIDE = WS.FLAG_WIDE_MOTION
+LTR = LTS.FLAG_LONG_TERM_REF
 
 
 def blocky_noise(w, h, x0, y0, seed=11):
@@ -377,6 +485,71 @@ def wide_cases():
     return out
 
 
+def waves(w, h, t, parts, amp=40):
+    """BGRA picture t of grey content whose rows [y0, y1) hold a vertical-bar cosine of `period` px moving left by `step` px per
+    picture, for (y0, y1, period, step) in parts (exact at every t: a step of half a period repeats the content two pictures on)."""
+    inv = grey_table()
+    x = np.arange(w)[None, :]
+    luma = np.full((h, w), 128.0)
+    for y0, y1, period, step in parts:
+        luma[y0:y1] = 128 + amp * np.cos(2 * np.pi * (x + step * t) / period)
+    return grey(w, h, inv, np.rint(luma).astype(np.int64))
+
+
+def wrap_content(w, h):
+    """513 pictures of flat grey for frame_num's wrap (8 bits): content A still for pictures 0..255, B from 256 on (picture 256 marks picture 255,
+    frame_num 255, with MMCO 1 on frame_num 254 across the wrap and MMCO 3 on PicNum -1), still to 511 (no picture marks: changed
+    stays 0), A again at 512, which predicts from the long-term picture 257 pictures later while picture 511, its short-term
+    reference, has frame_num 255 too."""
+    inv, yy = grey_table(), np.arange(h)[:, None] + np.zeros(w, np.int64)
+    a, b = grey(w, h, inv, np.where(yy < h // 2, 60, 180)), grey(w, h, inv, np.where(yy < h // 2, 200, 40))
+    return [a] * 256 + [b] * 256 + [a]
+
+
+def ltr_cases():
+    """The long-term reference (B2V_FLAG_LONG_TERM_REF, §5.13): the configurations of both files with the flag on.  Each reaches
+    what LTR_TARGETS names for it."""
+    w, h = 320, 192
+    pan = [waves(128, 64, t, [(0, 64, 24, 1.25)], amp=30) for t in range(6)]
+    return [("ltr_popup", S.Config(w, h, qp=26, flags=LTR), LC.popup(w, h)[0], (0,), None, 0),
+            ("ltr_alt_tab_wide", S.Config(w, h, qp=26, flags=LTR | WIDE), LC.alt_tab(w, h)[0], (0,), None, 0),
+            # two short popups, an IDR requested at 6 and a gop of 5 (an IDR at 11): no override after an IDR, the rule starting again
+            ("ltr_cbr_idr_gop", S.Config(w, h, rc_mode=S.CBR, kbps=2000, fps=30.0, gop=5, flags=LTR),
+             LC.popup(w, h, 2, 2, 2)[0] * 2, (0, 6), None, 0),
+            # still, then bars of period 16 moving 8 px per picture (and of period 16.5 moving 8.25): picture 2 marks picture 1, and
+            # picture 3 repeats picture 1, its vectors from picture 2 (the bars' half period either way)
+            ("ltr_both_exits", S.Config(160, 96, qp=40, flags=LTR),
+             [waves(160, 96, t, [(0, 48, 16, 8), (48, 96, 16.5, 8.25)], amp=20) for t in (0, 0, 1, 2, 3)], (0,), None, 0),
+            ("ltr_pcm_noise_qp0_4", S.Config(64, 48, qp=0, flags=LTR), [synth.noise(64, 48, s) for s in (5, 5, 6, 7, 8)], (0,),
+             [0, 0, 2, 4, 4], 0),
+            ("ltr_frame_num_wrap", S.Config(48, 32, qp=26, flags=LTR), wrap_content(48, 32), (0,), None, 0),
+            ("droppable_fractional_pan", S.Config(128, 64, qp=22, flags=LS.FLAG_DROPPABLE), pan, (0,), None, 0)]
+
+
+def assert_targets(name, st):
+    """What each case is there for, from the parsed streams and the model: a case that drifts away from its target fails."""
+    ex = st.exits
+    if name in ("pcm_noise_qp0_4", "wide_pcm_noise_qp0_4"):
+        assert st.kinds.get("I_PCM", 0) > 0, st.kinds
+    if name == "paintover_burst":
+        assert st.kinds.get("P_L0_16x16", 0) > 0        # the burst re-codes the still at the paint-over QP
+    if name in ("ltr_popup", "ltr_alt_tab_wide"):
+        assert st.marks and ex.get("long-term", 0) > 0, (st.marks, ex)
+    if name == "ltr_popup":
+        assert st.skip_next_to_lt > 0, ex
+    if name == "ltr_cbr_idr_gop":
+        assert any(k > 6 for _, k in st.marks) and any(k < 6 for _, k in st.marks), st.marks
+    if name == "ltr_both_exits":
+        assert ex.get("predictor lean", 0) > 0 and ex.get("long-term over edge predictor", 0) > 0, ex
+    if name == "ltr_pcm_noise_qp0_4":
+        assert st.pcm_two_refs > 0, (st.kinds, st.marks)
+    if name == "ltr_frame_num_wrap":
+        assert st.mark_at_fn0 and st.mmco1_wrap and st.lt_age > 256 and st.lt_fn_twin > 0, \
+            (st.marks, st.mark_at_fn0, st.mmco1_wrap, st.lt_age, st.lt_fn_twin)
+    if name == "droppable_fractional_pan":
+        assert st.scaled > 0, ex
+
+
 CASES = cases()
 
 
@@ -392,10 +565,7 @@ def test_oracle_decisions(case):
     e, st = run_case(encode_oracle, case)
     check_recon(e, st)
     assert st.pictures >= len(case[2])
-    if case[0] in ("pcm_noise_qp0_4", "wide_pcm_noise_qp0_4"):
-        assert st.kinds.get("I_PCM", 0) > 0, st.kinds
-    if case[0] == "paintover_burst":
-        assert st.kinds.get("P_L0_16x16", 0) > 0        # the burst re-codes the still at the paint-over QP
+    assert_targets(case[0], st)
 
 
 def nal_ref_idc(au):
@@ -403,11 +573,11 @@ def nal_ref_idc(au):
     return next(n[0] >> 5 & 3 for n in split_annexb(au) if n[0] & 31 in (1, 5))
 
 
-# The decisions' wide-motion cases, and three more for the coarse search alone: mbw % 4 = 2 in bands of 5 rows at QP 51 (the
+# The decisions' wide-motion cases (the long-term reference's left out: its coarse search is the wide oracle's), and three more for the coarse search alone: mbw % 4 = 2 in bands of 5 rows at QP 51 (the
 # largest λ: most groups stay below the early exit), mbw % 4 = 3 at QP 0 (λ = 1: nearly every group searches), 2x2-blocky
 # noise moved 124 px left and 256 px down, whose only match is the coarse window's corner (dx = 31, dy = -64), and noise
 # scrolled in bands of 5 rows whose bottom groups match best one decimated row past the band.
-COARSE_CASES = [c for c in CASES if c[1].flags & WIDE] + [
+COARSE_CASES = [c for c in CASES if c[1].flags & WIDE and not c[1].flags & LTR] + [
     ("coarse_drag_stripes5_qp51", S.Config(160, 144, qp=51, stripe_rows=5, flags=WIDE),
      [WC.drag(160, 144, t, (-30, 22), (90, 10), 64, 64) for t in range(4)], (0,), None, 5),
     ("coarse_scroll_qp0", S.Config(240, 208, qp=0, flags=WIDE), [WC.desktop_scroll(240, 208, t, 60) for t in range(3)], (0,), None, 0),
@@ -613,12 +783,13 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28, wide=False, shift=(-
     cw, ch = (w + 15) // 16 * 16, (h + 15) // 16 * 16
     sources = [source_nv12(f, cw, ch) for f in (still, still, moved)]
     for y0, aus in streams.items():
-        pics = parse_stream(aus)                 # a band whose still picture was all skipped is not sent: 2 pictures
+        pics = HSR.parse_stream(aus)             # a band whose still picture was all skipped is not sent: 2 pictures
         mbw, mbh = pics[-1].sps.mbw, pics[-1].sps.mbh
         band = [[p[y0 // k:(y0 + 16 * mbh) // k] for p, k in zip(s, (1, 2, 2))] for s in sources]
-        st, rec = Stats(), None
+        st, recs = Stats(), []
         for i in range(len(pics) - 1):
-            rec = check_picture(pics[i], rec, band[i], f"band {y0} picture {i}", st)
+            recs.append(check_picture(pics[i], recs, band[i], f"band {y0} picture {i}", st))
+        rec = recs[-1]
         prev_mbs = pics[1].mbs if len(pics) == 3 else [Mb(a, 0, "P_Skip", qp) for a in range(mbw * mbh)]
         # the coded-size reference of the band (or picture): a band's stream clamps at the band's own edges
         ref = rec[0]

@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 def _session(cfg: S.Config) -> Session:
     p = cfg.paint
-    return Session(cfg.width, cfg.height, fps=cfg.fps, rc_mode=cfg.rc_mode, bitrate_kbps=cfg.kbps, crf=cfg.qp,
+    return Session(cfg.width, cfg.height, fps=cfg.fps, rc_mode=cfg.rc_mode, bitrate_kbps=cfg.kbps, crf=cfg.qp, gop=cfg.gop,
                    slice_rows=cfg.slice_rows, idr_slice_mbs=cfg.idr_slice_mbs, stripe_rows=cfg.stripe_rows,
                    paintover_trigger_frames=p[0], paintover_crf=p[1], paintover_burst_frames=p[2], flags=cfg.flags)
 
@@ -22,7 +22,7 @@ def encode_gpu(cfg: S.Config, frames, idr_at=(0,), qps=None) -> D.Encoded:
     with _session(cfg) as s:
         cw, ch = s.coded_size()
         out = D.Encoded(cfg.width, cfg.height, cw, ch)
-        out.wide = s.wide_motion
+        out.flags = cfg.flags
         for i, f in enumerate(frames):
             if i in idr_at and i > 0:
                 s.flush()
@@ -67,10 +67,7 @@ def test_gpu_decisions(case):
     e, st = D.run_case(encode_gpu, case)
     D.check_recon(e, st)
     assert st.pictures >= len(case[2])
-    if case[0] in ("pcm_noise_qp0_4", "wide_pcm_noise_qp0_4"):
-        assert st.kinds.get("I_PCM", 0) > 0, st.kinds
-    if case[0] == "paintover_burst":
-        assert st.kinds.get("P_L0_16x16", 0) > 0        # the burst re-codes the still at the paint-over QP
+    D.assert_targets(case[0], st)
 
 
 def test_gpu_motion_recovery():

@@ -1,7 +1,7 @@
 """The long-term reference picture (B2V_FLAG_LONG_TERM_REF) in the oracle.  Every stream decodes with libavcodec to the oracle's
 reconstructions, over CQP and CBR, wide motion on and off, paint-over, IDR requests and a gop, a resize, an odd cropped size and
 scaling.  The independent syntax model (tests/h264_syntax_refs.py, on tests/h264_syntax.py) finds the SPS values, the marking operations in exactly the pictures
-the rule names, the override exactly while a long-term picture exists, and refIdx-1 macroblocks only with the zero vector, never as
+the rule of tests/h264_model.py names (on its own changed(k)), the override exactly while a long-term picture exists, and refIdx-1 macroblocks only with the zero vector, never as
 P_Skip, within the zero-motion threshold of the long-term picture its DPB names.  max_num_ref_frames 2 fits MaxDpbFrames at every
 level the encoder writes.  The flag cuts the bytes of the pictures on which content comes back and costs the existing contents at
 most 2 %."""
@@ -11,6 +11,7 @@ import pytest
 import oracle
 from oracle import avdec
 from oracle.ltr import LongTermRefEncoder
+from tests import h264_model as M
 from tests import h264_syntax as HS
 from tests import h264_syntax_refs as HSR
 from tests import ltr_content as LC
@@ -47,41 +48,34 @@ def _assert_decodes(aus, recs, w, h):
         assert np.array_equal(U, ruv[:h // 2, 0:w:2]) and np.array_equal(V, ruv[:h // 2, 1:w:2]), f"picture {k}: chroma"
 
 
-def _changed_rule(states, idrs, mbs):
-    """the pictures the marking rule names, from the oracle's changed(k) (an IDR counts every macroblock)"""
+def _model_marks(frames, recs, pics, idrs):
+    """the pictures the marking rule of tests/h264_model.py names, on its changed(k) from the source and picture k-1's reconstruction
+    (an IDR counts every macroblock)"""
+    h, w = recs[0][0].shape
+    mbs = (w // 16) * (h // 16)
     out, prev = [], mbs
-    for k, st in enumerate(states):
+    for k, f in enumerate(frames):
         if k in idrs:
             prev = mbs
             continue
-        if st["changed"] >= max(-(-mbs // 64), 8 * prev):
+        y, _ = oracle.csc_nv12(f, coded_w=w, coded_h=h)
+        changed = M.changed_count(y, recs[k - 1][0], pics[k].qp)
+        if M.marks(changed, prev, mbs):
             out.append(k)
-        prev = st["changed"]
+        prev = changed
     return out
 
 
-def _threshold(qp):
-    """the zero-motion threshold ME_EARLY_SAD_PER_LAMBDA x me_lambda[qp] (oracle/h264_ref.c, oracle/h264_tables_ref.h)"""
-    import os
-    import re
-    d = os.path.dirname(oracle.__file__)
-    tab = re.search(r"me_lambda\[52\]\s*=\s*\{([^}]*)\}", open(os.path.join(d, "h264_tables_ref.h")).read()).group(1)
-    per = int(re.search(r"#define ME_EARLY_SAD_PER_LAMBDA (\d+)", open(os.path.join(d, "h264_ref.c")).read()).group(1))
-    return per * [int(v) for v in tab.split(",")][qp]
-
-
-def _check_syntax(aus, recs, states, lts, idrs):
+def _check_syntax(frames, aus, recs, states, lts, idrs):
     pics = HSR.parse_stream(aus)
-    mbs = len(pics[0].mbs)
     marks = [k for k, p in enumerate(pics) if "mmco" in p.headers[0]]
-    assert marks == [k for k, s in enumerate(states) if s["mark"]] == _changed_rule(states, set(idrs) | {0}, mbs)
+    assert marks == [k for k, s in enumerate(states) if s["mark"]] == _model_marks(frames, recs, pics, set(idrs) | {0})
     for k, p in enumerate(pics):
         assert p.sps.max_num_ref_frames == 2 and p.sps.vui["max_dec_frame_buffering"] == 2
         for hd in p.headers:
             assert ("mmco" in hd) == (k in marks)
             if k in marks:
-                drop = [(1, 1)] if not states[k]["active"] else []
-                assert hd["mmco"] == drop + [(4, 1), (3, 0, 0)], (k, hd["mmco"])
+                assert hd["mmco"] == M.marking_ops(states[k]["active"]), (k, hd["mmco"])
             # the override exactly while a long-term picture exists
             assert hd.get("num_ref_idx_active", 1) == (2 if lts[k] is not None and not p.idr else 1), k
         if lts[k] is not None and not p.idr:
@@ -96,7 +90,7 @@ def _check_syntax(aus, recs, states, lts, idrs):
 
 def _sad_checks(frames, pics, lts, qp, w, h):
     """every refIdx-1 macroblock's source block lies within the zero-motion threshold of the long-term picture at the zero vector"""
-    thr = _threshold(qp)
+    thr = M.EARLY_SAD_PER_LAMBDA * M.LAMBDA[qp]
     cw, ch = (w + 15) & ~15, (h + 15) & ~15
     mbw = cw // 16
     n = 0
@@ -121,7 +115,7 @@ def test_contents_decode_and_syntax(name, wide):
     frames, _ = LC.CONTENTS[name](w, h)
     aus, recs, states, lts = _encode(frames, wide=wide, qp=26)
     _assert_decodes(aus, recs, w, h)
-    pics, marks = _check_syntax(aus, recs, states, lts, ())
+    pics, marks = _check_syntax(frames, aus, recs, states, lts, ())
     n = _sad_checks(frames, pics, lts, 26, w, h)
     if name in ("popup", "alt_tab"):
         assert marks and n > 0, (marks, n)
@@ -136,7 +130,7 @@ def test_cbr_idr_request_gop_and_paintover():
     idrs = [8] + [k for k in range(12, len(frames)) if (k - 12) % 5 == 0]
     aus, recs, states, lts = _encode(frames, idr_at=idrs, paint=(3, 18, 2), rc_mode=0, target_bits=120000)
     _assert_decodes(aus, recs, w, h)
-    _check_syntax(aus, recs, states, lts, idrs)
+    _check_syntax(frames, aus, recs, states, lts, idrs)
     for k in idrs:
         assert lts[k + 1] is None if k + 1 < len(frames) else True      # an IDR retires the long-term picture
 
