@@ -133,7 +133,7 @@ enum {
                                    scaling, B2V_FLAG_DROPPABLE and B2V_FLAG_QUALITY.  H.264 only: b2v_create rejects it
                                    (B2V_EINVAL) with B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE.  It costs one kernel launch per picture
                                    (kernel_launches) and coded width x height / 16 bytes per reconstruction buffer. */
-  B2V_FLAG_LONG_TERM_REF = 512  /* keep one earlier picture as a long-term reference, so that content that comes back (a popup or
+  B2V_FLAG_LONG_TERM_REF = 512, /* keep one earlier picture as a long-term reference, so that content that comes back (a popup or
                                    menu closing, a switch back to an application, a window dragged off the desktop) is predicted
                                    from it instead of coded as new.  The SPS says max_num_ref_frames 2 and max_dec_frame_buffering 2.
                                    P picture k marks picture k-1 long-term (adaptive dec_ref_pic_marking: MMCO 4, MMCO 3 with
@@ -150,7 +150,20 @@ enum {
                                    b2v_set_resolution rejects a size at which stripe_rows would stripe.  It costs one kernel launch
                                    per P picture (kernel_launches), a copy of one picture on the pictures that mark, and coded
                                    width x height x 1.5 bytes. */
+  B2V_FLAG_DAMAGE        = 1024 /* damage rectangles (an ingest flag, not a coding flag: it works with H.264 full-frame and striped,
+                                   B2V_FLAG_JPEG, B2V_FLAG_NO_ENCODE and every coding flag).  The b2v_*_damage submits take the
+                                   regions of the source that changed since the previous picture; only those are copied and
+                                   colour-converted.  The contract: when the rectangles cover every pixel that changed since the
+                                   previous picture of the session, the access units, the reconstructions and the NV12 pictures are
+                                   exactly those of a whole-frame submit of the same picture.  The ring then copies into one
+                                   persistent device frame (the mirror, src_w x src_h x 4 bytes) instead of one device buffer per
+                                   ring slot: at 4K that is 33 MB of HBM instead of ring_slots x 33 MB. */
 };
+
+/* B2V_FLAG_DAMAGE: one changed region of the source, in source pixels of the frame (or the device window) the submit names.
+ * Rectangles are clipped to the frame; w == 0 or h == 0 is an empty rectangle. */
+typedef struct b2v_rect { int32_t x, y, w, h; } b2v_rect;
+#define B2V_MAX_DAMAGE_RECTS 64    /* most rectangles of one submit (each ring rectangle is one copy); merge beyond it */
 
 /* One encoded frame, the native image of the pixelflux callback result
  * (`result.data / result.size / result.frame_id`, media_pipeline.py:284-292).
@@ -278,6 +291,27 @@ typedef struct b2v_tensor {
  * aligned to the element size; memory that is not device or managed memory of the session's device; a last byte read,
  * data + 2 * stride_c + (src_h - 1) * stride_y + (src_w - 1) * stride_x + element size - 1, outside the allocation holding `data`. */
 int   b2v_submit_tensor(void* h, const b2v_tensor* t, void* cuda_stream, int64_t capture_ns);
+
+/* ---- damage submits (B2V_FLAG_DAMAGE).  b2v_ring_submit, b2v_submit_device and b2v_submit_tensor are these with rects = NULL.
+ *   rects == NULL: the whole frame.  n_rects == 0 with rects != NULL: nothing changed; the picture is still coded and delivered.
+ *   Rejections (B2V_EINVAL, before any CUDA call; a ring slot stays acquired): rects without B2V_FLAG_DAMAGE, a negative w or h,
+ *   n_rects < 0 or above B2V_MAX_DAMAGE_RECTS, a null handle.
+ * Ring: copies exactly the given rectangles of the slot into the mirror, one 2-D copy each, so the producer only has to write
+ *   those rectangles into the slot.  A damage submit needs the previous picture of the session to be a ring picture at the
+ *   current geometry: otherwise (the first picture after b2v_create or b2v_set_resolution, a ring picture after a device,
+ *   tensor or resident picture) it fails with B2V_ESTATE and the slot stays acquired, so the producer can fill it whole and
+ *   submit it again.  A whole-frame ring submit of a flagged session copies the whole slot into the mirror.  The copy of a
+ *   picture waits for the colour conversion of the one before to have read the mirror.
+ * Device and tensor: the frame is read in place, so there is no copy to save; only the tiles the rectangles touch are converted.
+ *   With no previous picture at this geometry the whole frame is converted.
+ * The conversion: the rectangles are mapped to 16 x 16 tiles of the coded picture (b2v_damage_tiles); when the dirty tiles cover
+ *   more than a quarter of the picture (DESIGN.md §4, damage rectangles), and for whole-frame submits, the whole frame is converted as without the
+ *   flag.  Either way one CSC kernel per picture (kernel_launches).  stats.h2d_bytes counts the pixel bytes actually copied:
+ *   4 x the clipped rectangle area of a ring damage submit, src_w x src_h x 4 of a whole one. */
+int   b2v_ring_submit_damage(void* h, int32_t slot, int32_t stride_bytes, const b2v_rect* rects, int32_t n_rects, int64_t capture_ns);
+int   b2v_submit_device_damage(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, const b2v_rect* rects,
+                               int32_t n_rects, void* cuda_stream, int64_t capture_ns);
+int   b2v_submit_tensor_damage(void* h, const b2v_tensor* t, const b2v_rect* rects, int32_t n_rects, void* cuda_stream, int64_t capture_ns);
 int   b2v_flush(void* h);                               /* wait until every submitted frame was delivered */
 
 /* ---- live control: ScreenCapture.update_framerate (media_pipeline.py:236),
@@ -310,6 +344,12 @@ int  b2v_reset_stats(void* h);
 int  b2v_coded_size(void* h, int32_t* coded_w, int32_t* coded_h);
 /* synchronous fused CSC(+scale) of one host BGRA frame to host NV12 (dst_w*dst_h*3/2 bytes) */
 int  b2v_csc_nv12(void* h, const void* bgra_host, int32_t stride_bytes, void* nv12_host);
+/* B2V_FLAG_DAMAGE's map of rectangles (source pixels, clipped to src_w x src_h) to the 16 x 16 tiles of a dst_w x dst_h output:
+ * map[ty * ceil(dst_w / 16) + tx] = 1 when tile (tx, ty) must be converted again, else 0.  At 1:1 a tile is dirty when it meets a
+ * rectangle; when scaling, when the source footprint of its bilinear taps meets one.  Padding rows and columns of the coded
+ * picture lie in the tile of the last visible row or column.  Returns the count of dirty tiles, or B2V_EINVAL (sizes as
+ * b2v_create takes them, rectangles as the damage submits take them, null map).  Host code, no CUDA call; the submits use it. */
+int  b2v_damage_tiles(int32_t src_w, int32_t src_h, int32_t dst_w, int32_t dst_h, const b2v_rect* rects, int32_t n_rects, uint8_t* map);
 /* the same of one device tensor, read in place after the work enqueued on `cuda_stream` (checked as b2v_submit_tensor checks it) */
 int  b2v_csc_nv12_tensor(void* h, const b2v_tensor* t, void* cuda_stream, void* nv12_host);
 /* reconstruction of the last encoded frame: NV12, coded_w*coded_h*3/2 bytes */

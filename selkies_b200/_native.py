@@ -21,6 +21,8 @@ B2V_FLAG_QUALITY = 64
 B2V_FLAG_DROPPABLE = 128
 B2V_FLAG_WIDE_MOTION = 256
 B2V_FLAG_LONG_TERM_REF = 512
+B2V_FLAG_DAMAGE = 1024
+B2V_MAX_DAMAGE_RECTS = 64
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
 B2V_DT_U8, B2V_DT_F16, B2V_DT_BF16, B2V_DT_F32 = 0, 1, 2, 3
 
@@ -70,6 +72,10 @@ class B2VTensor(C.Structure):
     ]
 
 
+class B2VRect(C.Structure):
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32)]
+
+
 class B2VQuality(C.Structure):
     _fields_ = [
         ("sse_y", C.c_int64), ("sse_cb", C.c_int64), ("sse_cr", C.c_int64),
@@ -93,6 +99,10 @@ SYMBOLS = [
     ("b2v_submit_resident", C.c_int, [C.c_void_p, C.c_int32, C.c_int64]),
     ("b2v_submit_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64]),
     ("b2v_submit_tensor", C.c_int, [C.c_void_p, C.POINTER(B2VTensor), C.c_void_p, C.c_int64]),
+    ("b2v_ring_submit_damage", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(B2VRect), C.c_int32, C.c_int64]),
+    ("b2v_submit_device_damage", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(B2VRect), C.c_int32, C.c_void_p,
+                                           C.c_int64]),
+    ("b2v_submit_tensor_damage", C.c_int, [C.c_void_p, C.POINTER(B2VTensor), C.POINTER(B2VRect), C.c_int32, C.c_void_p, C.c_int64]),
     ("b2v_flush", C.c_int, [C.c_void_p]),
     ("b2v_set_framerate", C.c_int, [C.c_void_p, C.c_double]),
     ("b2v_set_bitrate_kbps", C.c_int, [C.c_void_p, C.c_int32]),
@@ -105,6 +115,7 @@ SYMBOLS = [
     ("b2v_reset_stats", C.c_int, [C.c_void_p]),
     ("b2v_coded_size", C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("b2v_csc_nv12", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    ("b2v_damage_tiles", C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(B2VRect), C.c_int32, C.c_void_p]),
     ("b2v_csc_nv12_tensor", C.c_int, [C.c_void_p, C.POINTER(B2VTensor), C.c_void_p, C.c_void_p]),
     ("b2v_get_recon", C.c_int, [C.c_void_p, C.c_void_p]),
     ("b2v_bench_csc", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
@@ -145,6 +156,16 @@ def lib():
                 raise ImportError("libb2video ABI version mismatch")
             _lib = l
     return _lib
+
+
+def rect_array(rects):
+    """(pointer, count) of a list of (x, y, w, h) for the damage entry points: (None, 0) for None (the whole frame); a valid
+    pointer with count 0 for an empty list (nothing changed)."""
+    if rects is None:
+        return None, 0
+    rects = [tuple(int(v) for v in r) for r in rects]
+    arr = (B2VRect * max(1, len(rects)))(*rects)
+    return arr, len(rects)
 
 
 def check(rc):

@@ -15,6 +15,7 @@
 //   st_out  : cudaMemcpyAsync  AU head (size + first chunk) -> pinned output slot
 //   output thread: waits the D2H event, fetches the tail of oversized AUs, runs the callback in order: one call per band
 //   that carries data (striped H.264, JPEG stripes); a full frame is delivered as the one band of the picture.
+#include <algorithm>
 #include <condition_variable>
 #include <cstdarg>
 #include <cstdio>
@@ -91,6 +92,10 @@ inline cudaError_t wait_event_polling(cudaEvent_t ev, bool* slept) {
 
 // ingest-ring slot states
 enum : uint8_t { SLOT_FREE = 0, SLOT_ACQUIRED = 1, SLOT_IN_FLIGHT = 2 };
+// where a picture came from (B2V_FLAG_DAMAGE: a ring damage submit stands on a ring picture, any other on any picture)
+enum { SRC_NONE = 0, SRC_RING = 1, SRC_OTHER = 2 };
+// B2V_FLAG_DAMAGE: above this fraction of dirty tiles the whole-frame kernel converts the picture (DESIGN.md §4, damage rectangles)
+constexpr double kDamageFullFraction = 0.25;
 
 struct Session {
   b2v_settings cfg{};
@@ -108,8 +113,19 @@ struct Session {
   size_t frame_bytes = 0;
   // resident frames (bench `value` leg)
   std::vector<uint8_t*> resident;
-  // scaling taps
+  // scaling taps (the host copies map damage rectangles to tiles)
   Tap *d_tx = nullptr, *d_ty = nullptr;
+  std::vector<Tap> h_tx, h_ty;
+  // B2V_FLAG_DAMAGE: the ring's one device frame (pitch src_w * 4; replaces dev_slot[]), the event behind the latest CSC (the next
+  // copy into the mirror waits for it), per-output-slot tile lists (pinned staging, device copy), the tile map, and what the
+  // previous picture at this geometry came from (guarded by submit_mu; alloc_geometry resets it)
+  bool damage = false;
+  uint8_t* d_mirror = nullptr;
+  cudaEvent_t ev_csc_read = nullptr;
+  int* h_tiles[kMaxSlots] = {};
+  int* d_tiles[kMaxSlots] = {};
+  std::vector<uint8_t> tile_map;
+  int prev_src = 0;              // SRC_*
   // current-frame NV12 (coded size)
   uint8_t* d_cur = nullptr;
   // encoder: H.264 (enc) or, with B2V_FLAG_JPEG, JPEG stripes (jenc)
@@ -197,18 +213,28 @@ int alloc_geometry(Session* s) {
   s->frame_bytes = (size_t)s->src_w * s->src_h * 4;
   for (int i = 0; i < s->n_slots; i++) {
     CK(cudaHostAlloc((void**)&s->host_slot[i], s->frame_bytes, cudaHostAllocDefault));
-    CK(cudaMalloc((void**)&s->dev_slot[i], s->frame_bytes));
+    if (!s->damage) CK(cudaMalloc((void**)&s->dev_slot[i], s->frame_bytes));
     s->slot_state[i] = SLOT_FREE;
   }
   CK(cudaMalloc((void**)&s->d_cur, (size_t)s->coded_w * s->coded_h * 3 / 2));
+  s->h_tx.clear(); s->h_ty.clear();
   if (s->dst_w != s->src_w || s->dst_h != s->src_h) {
-    std::vector<Tap> tx(s->dst_w), ty(s->dst_h);
-    make_taps_host(tx.data(), s->dst_w, s->src_w);
-    make_taps_host(ty.data(), s->dst_h, s->src_h);
+    s->h_tx.resize(s->dst_w); s->h_ty.resize(s->dst_h);
+    make_taps_host(s->h_tx.data(), s->dst_w, s->src_w);
+    make_taps_host(s->h_ty.data(), s->dst_h, s->src_h);
     CK(cudaMalloc((void**)&s->d_tx, sizeof(Tap) * s->dst_w));
     CK(cudaMalloc((void**)&s->d_ty, sizeof(Tap) * s->dst_h));
-    CK(cudaMemcpy(s->d_tx, tx.data(), sizeof(Tap) * s->dst_w, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(s->d_ty, ty.data(), sizeof(Tap) * s->dst_h, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(s->d_tx, s->h_tx.data(), sizeof(Tap) * s->dst_w, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(s->d_ty, s->h_ty.data(), sizeof(Tap) * s->dst_h, cudaMemcpyHostToDevice));
+  }
+  s->prev_src = SRC_NONE;
+  if (s->damage) {
+    CK(cudaMalloc((void**)&s->d_mirror, s->frame_bytes));
+    s->tile_map.assign((size_t)((s->dst_w + 15) / 16) * ((s->dst_h + 15) / 16), 0);
+    for (int i = 0; i < s->n_slots; i++) {
+      CK(cudaHostAlloc((void**)&s->h_tiles[i], sizeof(int) * s->tile_map.size(), cudaHostAllocDefault));
+      CK(cudaMalloc((void**)&s->d_tiles[i], sizeof(int) * s->tile_map.size()));
+    }
   }
   if (s->encode && s->jpeg) {
     JpegConfig jc{};
@@ -246,8 +272,13 @@ void free_geometry(Session* s) {
     if (s->dev_slot[i]) cudaFree(s->dev_slot[i]);
     if (s->d_au[i]) cudaFree(s->d_au[i]);
     if (s->h_out[i]) cudaFreeHost(s->h_out[i]);
+    if (s->h_tiles[i]) cudaFreeHost(s->h_tiles[i]);
+    if (s->d_tiles[i]) cudaFree(s->d_tiles[i]);
     s->host_slot[i] = s->dev_slot[i] = s->d_au[i] = s->h_out[i] = nullptr;
+    s->h_tiles[i] = s->d_tiles[i] = nullptr;
   }
+  if (s->d_mirror) cudaFree(s->d_mirror);
+  s->d_mirror = nullptr;
   for (auto p : s->resident) if (p) cudaFree(p);
   s->resident.clear();
   if (s->d_cur) cudaFree(s->d_cur);
@@ -455,10 +486,12 @@ int submit_failed(Session* s, int out_idx, int in_slot, cudaError_t e, const cha
 #define CKS(call)                                                                              \
   do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return submit_failed(s, out_idx, in_slot, e_, #call); } while (0)
 
-// common tail of b2v_ring_submit / b2v_submit_device / b2v_submit_tensor / b2v_submit_resident: CSC + encode + D2H + job.
+// common tail of the ring, device, tensor and resident submits: CSC + encode + D2H + job.  Caller holds submit_mu.
 // `producer` (device frames of the caller) is the stream the CSC is ordered after, and that is ordered after the CSC in turn;
-// null: no such stream.
-int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStream_t* producer, int64_t capture_ns) {
+// null: no such stream.  `rects` (B2V_FLAG_DAMAGE, checked): null = the whole frame; else only the tiles they touch are
+// converted, when there is a previous picture at this geometry and they are few enough.  `kind`: SRC_RING or SRC_OTHER.
+int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStream_t* producer, int64_t capture_ns,
+                  const b2v_rect* rects, int n_rects, int kind) {
   int out_idx = 0;
   Job j{};
   EncodeFrameParams fp{};
@@ -502,6 +535,17 @@ int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStrea
   }
   CscSource cp = csc_params(s, src, s->d_cur);
   cudaEvent_t* ev = j.timing ? s->ev_t[out_idx] : nullptr;
+  int n_tiles = -1;                     // -1: the whole-frame kernel
+  if (rects && s->prev_src != SRC_NONE) {
+    n_tiles = damage_tiles(s->h_tx.empty() ? nullptr : s->h_tx.data(), s->h_ty.empty() ? nullptr : s->h_ty.data(), s->src_w, s->src_h,
+                           s->dst_w, s->dst_h, rects, n_rects, s->tile_map.data());
+    if (n_tiles > kDamageFullFraction * (double)s->tile_map.size()) n_tiles = -1;
+    else {                              // the staging buffer of this output slot is free: its last picture was delivered
+      int* list = s->h_tiles[out_idx];
+      for (int t = 0, k = 0; k < n_tiles; t++) if (s->tile_map[t]) list[k++] = t;
+      if (n_tiles > 0) CKS(cudaMemcpyAsync(s->d_tiles[out_idx], list, sizeof(int) * n_tiles, cudaMemcpyHostToDevice, s->st_enc));
+    }
+  }
   if (producer) {
     CKS(cudaEventRecord(s->ev_dev_in, *producer));
     CKS(cudaStreamWaitEvent(s->st_enc, s->ev_dev_in, 0));
@@ -512,8 +556,9 @@ int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStrea
     cudaMemsetAsync(cp.ts + 1, 0, sizeof(unsigned long long), s->st_enc);
   }
   if (ev) cudaEventRecord(ev[0], s->st_enc);
-  int nl = launch_csc(cp, s->st_enc);
+  int nl = n_tiles >= 0 ? launch_csc_tiles(cp, s->d_tiles[out_idx], n_tiles, s->st_enc) : launch_csc(cp, s->st_enc);
   if (ev) cudaEventRecord(ev[1], s->st_enc);
+  if (s->damage) CKS(cudaEventRecord(s->ev_csc_read, s->st_enc));     // the next copy into the mirror waits for this
   if (producer) {                       // the caller may reuse the frame in stream order once the CSC has read it
     CKS(cudaEventRecord(s->ev_dev_done, s->st_enc));
     CKS(cudaStreamWaitEvent(*producer, s->ev_dev_done, 0));
@@ -543,6 +588,7 @@ int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStrea
     s->stats.ns_submit += now_ns() - t_enter - t_slot;
     s->jobs.push_back(j);
   }
+  s->prev_src = kind;
   s->cv_job.notify_one();
   return 0;
 }
@@ -562,6 +608,7 @@ void release_session(Session* s) {
   if (s->ev_timer[1]) cudaEventDestroy(s->ev_timer[1]);
   if (s->ev_dev_in) cudaEventDestroy(s->ev_dev_in);
   if (s->ev_dev_done) cudaEventDestroy(s->ev_dev_done);
+  if (s->ev_csc_read) cudaEventDestroy(s->ev_csc_read);
   if (s->d_csc_ts) cudaFree(s->d_csc_ts);
   if (s->st_copy) cudaStreamDestroy(s->st_copy);
   if (s->st_enc) cudaStreamDestroy(s->st_enc);
@@ -703,6 +750,19 @@ int bench_csc(Session* s, int32_t n_resident, int32_t iters, float* ms_per_launc
   return 0;
 }
 
+// The rectangles of a damage submit (include/b2video.h), with no CUDA call: their count and sizes first, then the handle, then
+// the flag.  rects == NULL (the whole frame) needs neither.
+int check_damage_args(const Session* s, const b2v_rect* rects, int n) {
+  if (rects) {
+    if (n < 0 || n > B2V_MAX_DAMAGE_RECTS) return fail(B2V_EINVAL, "%d damage rectangles: 0 .. B2V_MAX_DAMAGE_RECTS (%d)", n, B2V_MAX_DAMAGE_RECTS);
+    for (int i = 0; i < n; i++)
+      if (rects[i].w < 0 || rects[i].h < 0) return fail(B2V_EINVAL, "damage rectangle %d has a negative size (%d x %d)", i, rects[i].w, rects[i].h);
+  }
+  if (!s) return fail(B2V_EINVAL, "null handle");
+  if (rects && !(s->cfg.flags & B2V_FLAG_DAMAGE)) return fail(B2V_EINVAL, "damage rectangles need a session created with B2V_FLAG_DAMAGE");
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -734,6 +794,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   s->src_w = sw; s->src_h = sh; s->dst_w = dw; s->dst_h = dh;
   s->encode = !(cfg->flags & B2V_FLAG_NO_ENCODE);
   s->jpeg = (cfg->flags & B2V_FLAG_JPEG) != 0;
+  s->damage = (cfg->flags & B2V_FLAG_DAMAGE) != 0;
   s->timing = (cfg->flags & (B2V_FLAG_TIMING | B2V_FLAG_TIMING_CSC)) != 0;
   s->timing_csc_only = s->timing && !(cfg->flags & B2V_FLAG_TIMING);
   s->n_slots = cfg->ring_slots > 0 ? cfg->ring_slots : 4;
@@ -759,6 +820,7 @@ int b2v_create(const b2v_settings* cfg, b2v_cb cb, void* user, void** out) {
   cudaEventCreate(&s->ev_timer[0]); cudaEventCreate(&s->ev_timer[1]);
   cudaEventCreateWithFlags(&s->ev_dev_in, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&s->ev_dev_done, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&s->ev_csc_read, cudaEventDisableTiming);
   if (s->timing && (cfg->flags & B2V_FLAG_DEVICE_TIMER)) cudaMalloc((void**)&s->d_csc_ts, sizeof(unsigned long long) * 2 * kMaxSlots);
   rc = alloc_geometry(s);
   if (rc) { release_session(s); return rc; }
@@ -813,28 +875,61 @@ int b2v_ring_release(void* h, int32_t slot) {
 }
 
 int b2v_ring_submit(void* h, int32_t slot, int32_t stride, int64_t capture_ns) {
+  return b2v_ring_submit_damage(h, slot, stride, nullptr, 0, capture_ns);
+}
+
+int b2v_ring_submit_damage(void* h, int32_t slot, int32_t stride, const b2v_rect* rects, int32_t n_rects, int64_t capture_ns) {
   Session* s = (Session*)h;
-  if (!s || slot < 0 || slot >= s->n_slots) return fail(B2V_EINVAL, "bad slot");
+  int rc = check_damage_args(s, rects, n_rects);
+  if (rc) return rc;
+  if (slot < 0 || slot >= s->n_slots) return fail(B2V_EINVAL, "bad slot");
   if (stride <= 0) stride = s->src_w * 4;
   if (stride < s->src_w * 4 || (size_t)stride * s->src_h > s->frame_bytes) return fail(B2V_EINVAL, "stride %d does not fit the slot", stride);
   std::lock_guard<std::mutex> sub(s->submit_mu);
   {
     std::lock_guard<std::mutex> lk(s->mu);
     if (s->slot_state[slot] != SLOT_ACQUIRED) return fail(B2V_ESTATE, "slot %d was not acquired (double submit?)", slot);
+    if (rects && s->prev_src != SRC_RING)
+      return fail(B2V_ESTATE, "a ring damage submit needs a ring picture before it at this size (%s): submit slot %d whole",
+                  s->prev_src == SRC_NONE ? "this is the first picture since the session was created or resized" : "the previous picture was not a ring picture", slot);
     s->slot_state[slot] = SLOT_IN_FLIGHT;
   }
   const int64_t t0 = now_ns();
   const int out_idx = -1, in_slot = slot;             // for CKS: no output slot reserved yet
   CKS(cudaSetDevice(s->device));
-  CKS(cudaMemcpyAsync(s->dev_slot[slot], s->host_slot[slot], (size_t)stride * s->src_h, cudaMemcpyHostToDevice, s->st_copy));
+  const uint8_t* host = s->host_slot[slot];
+  int64_t bytes = (int64_t)stride * s->src_h;
+  CscSource src = packed_src(s->dev_slot[slot], stride, B2V_PIX_BGRA);
+  if (!s->damage) {
+    CKS(cudaMemcpyAsync(s->dev_slot[slot], host, (size_t)bytes, cudaMemcpyHostToDevice, s->st_copy));
+  } else {                                            // into the mirror, once the previous picture's CSC has read it
+    const size_t pitch = (size_t)s->src_w * 4;
+    src = packed_src(s->d_mirror, (int)pitch, B2V_PIX_BGRA);
+    CKS(cudaStreamWaitEvent(s->st_copy, s->ev_csc_read, 0));
+    if (!rects) {
+      CKS(cudaMemcpy2DAsync(s->d_mirror, pitch, host, stride, pitch, s->src_h, cudaMemcpyHostToDevice, s->st_copy));
+      bytes = (int64_t)pitch * s->src_h;
+    } else {
+      bytes = 0;
+      for (int i = 0; i < n_rects; i++) {             // clipped to the frame
+        const int x0 = rects[i].x > 0 ? rects[i].x : 0, y0 = rects[i].y > 0 ? rects[i].y : 0;
+        const int64_t x1 = std::min<int64_t>((int64_t)rects[i].x + rects[i].w, s->src_w), y1 = std::min<int64_t>((int64_t)rects[i].y + rects[i].h, s->src_h);
+        if (x1 <= x0 || y1 <= y0) continue;
+        const size_t w = (size_t)(x1 - x0) * 4, rows = (size_t)(y1 - y0);
+        CKS(cudaMemcpy2DAsync(s->d_mirror + y0 * pitch + (size_t)x0 * 4, pitch, host + (size_t)y0 * stride + (size_t)x0 * 4, stride, w, rows,
+                              cudaMemcpyHostToDevice, s->st_copy));
+        bytes += (int64_t)(w * rows);
+      }
+    }
+  }
   CKS(cudaEventRecord(s->ev_h2d[slot], s->st_copy));
   CKS(cudaStreamWaitEvent(s->st_enc, s->ev_h2d[slot], 0));
   {
     std::lock_guard<std::mutex> lk(s->mu);
-    s->stats.h2d_bytes += (int64_t)stride * s->src_h;
+    s->stats.h2d_bytes += bytes;
     s->stats.ns_submit += now_ns() - t0;
   }
-  return submit_common(s, packed_src(s->dev_slot[slot], stride, B2V_PIX_BGRA), slot, nullptr, capture_ns);
+  return submit_common(s, src, slot, nullptr, capture_ns, rects, n_rects, SRC_RING);
 }
 
 int b2v_resident_upload(void* h, int32_t index, const void* bgra, int32_t stride) {
@@ -854,31 +949,43 @@ int b2v_submit_resident(void* h, int32_t index, int64_t capture_ns) {
   if (!s || index < 0 || index >= (int)s->resident.size() || !s->resident[index]) return fail(B2V_EINVAL, "resident frame %d not uploaded", index);
   std::lock_guard<std::mutex> sub(s->submit_mu);
   CK(cudaSetDevice(s->device));
-  return submit_common(s, packed_src(s->resident[index], s->src_w * 4, B2V_PIX_BGRA), -1, nullptr, capture_ns);
+  return submit_common(s, packed_src(s->resident[index], s->src_w * 4, B2V_PIX_BGRA), -1, nullptr, capture_ns, nullptr, 0, SRC_OTHER);
 }
 
 int b2v_submit_device(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, void* cuda_stream, int64_t capture_ns) {
+  return b2v_submit_device_damage(h, frame, pitch_bytes, pixel_format, nullptr, 0, cuda_stream, capture_ns);
+}
+
+int b2v_submit_device_damage(void* h, const void* frame, int32_t pitch_bytes, int32_t pixel_format, const b2v_rect* rects, int32_t n_rects,
+                             void* cuda_stream, int64_t capture_ns) {
   Session* s = (Session*)h;
   if (pixel_format < B2V_PIX_BGRA || pixel_format > B2V_PIX_RGB) return fail(B2V_EINVAL, "unknown pixel format %d", pixel_format);
-  if (!s || !frame) return fail(B2V_EINVAL, "null argument");
+  int rc = check_damage_args(s, rects, n_rects);
+  if (rc) return rc;
+  if (!frame) return fail(B2V_EINVAL, "null argument");
   std::lock_guard<std::mutex> sub(s->submit_mu);         // the source size is stable from here on (b2v_set_resolution takes it too)
-  int rc = check_device_frame(s, (const uint8_t*)frame, pitch_bytes, pixel_format);
+  rc = check_device_frame(s, (const uint8_t*)frame, pitch_bytes, pixel_format);
   if (rc) return rc;
   const cudaStream_t producer = (cudaStream_t)cuda_stream;
-  return submit_common(s, packed_src((const uint8_t*)frame, pitch_bytes, pixel_format), -1, &producer, capture_ns);
+  return submit_common(s, packed_src((const uint8_t*)frame, pitch_bytes, pixel_format), -1, &producer, capture_ns, rects, n_rects, SRC_OTHER);
 }
 
 int b2v_submit_tensor(void* h, const b2v_tensor* t, void* cuda_stream, int64_t capture_ns) {
+  return b2v_submit_tensor_damage(h, t, nullptr, 0, cuda_stream, capture_ns);
+}
+
+int b2v_submit_tensor_damage(void* h, const b2v_tensor* t, const b2v_rect* rects, int32_t n_rects, void* cuda_stream, int64_t capture_ns) {
   Session* s = (Session*)h;
   int rc = check_tensor_args(t);
   if (rc) return rc;
-  if (!s) return fail(B2V_EINVAL, "null handle");
+  rc = check_damage_args(s, rects, n_rects);
+  if (rc) return rc;
   std::lock_guard<std::mutex> sub(s->submit_mu);         // the source size is stable from here on
   CscSource src;
   rc = tensor_source(s, t, &src);
   if (rc) return rc;
   const cudaStream_t producer = (cudaStream_t)cuda_stream;
-  return submit_common(s, src, -1, &producer, capture_ns);
+  return submit_common(s, src, -1, &producer, capture_ns, rects, n_rects, SRC_OTHER);
 }
 
 int b2v_flush(void* h) {
@@ -1006,6 +1113,21 @@ int b2v_csc_nv12(void* h, const void* bgra, int32_t stride, void* nv12) {
   if (!rc) rc = csc_to_host(s, packed_src(d_in, s->src_w * 4, B2V_PIX_BGRA), nv12);
   cudaFree(d_in);
   return rc;
+}
+
+int b2v_damage_tiles(int32_t src_w, int32_t src_h, int32_t dst_w, int32_t dst_h, const b2v_rect* rects, int32_t n_rects, uint8_t* map) {
+  if (!size_ok(src_w, src_h) || !size_ok(dst_w, dst_h)) return fail(B2V_EINVAL, "sizes %dx%d -> %dx%d unsupported", src_w, src_h, dst_w, dst_h);
+  if (!map || (!rects && n_rects)) return fail(B2V_EINVAL, "null argument");
+  if (n_rects < 0 || n_rects > B2V_MAX_DAMAGE_RECTS) return fail(B2V_EINVAL, "%d damage rectangles: 0 .. B2V_MAX_DAMAGE_RECTS (%d)", n_rects, B2V_MAX_DAMAGE_RECTS);
+  for (int i = 0; i < n_rects; i++)
+    if (rects[i].w < 0 || rects[i].h < 0) return fail(B2V_EINVAL, "damage rectangle %d has a negative size (%d x %d)", i, rects[i].w, rects[i].h);
+  std::vector<Tap> tx, ty;
+  if (dst_w != src_w || dst_h != src_h) {              // the taps alloc_geometry makes
+    tx.resize(dst_w); ty.resize(dst_h);
+    make_taps_host(tx.data(), dst_w, src_w);
+    make_taps_host(ty.data(), dst_h, src_h);
+  }
+  return damage_tiles(tx.empty() ? nullptr : tx.data(), ty.empty() ? nullptr : ty.data(), src_w, src_h, dst_w, dst_h, rects, n_rects, map);
 }
 
 int b2v_csc_nv12_tensor(void* h, const b2v_tensor* t, void* cuda_stream, void* nv12) {

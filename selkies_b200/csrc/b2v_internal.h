@@ -95,5 +95,10 @@ struct CscSource : CscParams {
 // returns number of kernel launches issued (1)
 int launch_csc(const CscSource& p, cudaStream_t st);
 void make_taps_host(Tap* t, int dn, int sn);
+// B2V_FLAG_DAMAGE (csc.cu): rectangles -> dirty-tile map of ceil(dst_w / 16) x ceil(dst_h / 16) bytes; returns the dirty count.
+// tx / ty: the host taps of the scale, null at 1:1.  Rectangles are checked by the caller.
+int damage_tiles(const Tap* tx, const Tap* ty, int src_w, int src_h, int dst_w, int dst_h, const b2v_rect* rects, int n, uint8_t* map);
+// converts only the n tiles listed in d_tiles (ty * ceil(dst_w / 16) + tx each), one launch even for n == 0; returns 1
+int launch_csc_tiles(const CscSource& p, const int* d_tiles, int n, cudaStream_t st);
 
 }  // namespace b2v

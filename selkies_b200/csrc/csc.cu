@@ -27,7 +27,9 @@
 //              per-pixel loader reads three strided elements and quantises them.
 #include <cuda_fp16.h>
 
+#include <cstring>
 #include <mutex>
+#include <vector>
 
 #include "b2v_internal.h"
 
@@ -312,10 +314,8 @@ __device__ __forceinline__ void fetch_bgr(const CscSource& p, int x, int y, int&
   B = out[0]; G = out[1]; R = out[2];
 }
 
-__global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscSource p) {
-  int bx = blockIdx.x * blockDim.x + threadIdx.x;   // 2x2 block column
-  int by = blockIdx.y * blockDim.y + threadIdx.y;
-  if (bx * 2 >= p.coded_w || by * 2 >= p.coded_h) return;
+// the 2x2 output block (bx, by): four pixels through fetch_bgr, their chroma from the sums.  Every source and scale.
+__device__ __forceinline__ void csc_block(const CscSource& p, int bx, int by) {
   const int* mx = c_mx[2 * p.matrix + (p.fmt & 1)];
   int sb = 0, sg = 0, sr = 0;
   unsigned yy[4];
@@ -332,6 +332,26 @@ __global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscSource p) {
   *(uint16_t*)(p.out_y + (size_t)(by * 2) * p.coded_w + bx * 2) = (uint16_t)(yy[0] | (yy[1] << 8));
   *(uint16_t*)(p.out_y + (size_t)(by * 2 + 1) * p.coded_w + bx * 2) = (uint16_t)(yy[2] | (yy[3] << 8));
   *(uint16_t*)(p.out_uv + (size_t)by * p.coded_w + bx * 2) = (uint16_t)(cb | (cr << 8));
+}
+
+__global__ void __launch_bounds__(256) csc_bgra_nv12_general(CscSource p) {
+  int bx = blockIdx.x * blockDim.x + threadIdx.x;   // 2x2 block column
+  int by = blockIdx.y * blockDim.y + threadIdx.y;
+  if (bx * 2 >= p.coded_w || by * 2 >= p.coded_h) return;
+  csc_block(p, bx, by);
+}
+
+// ---- tile-list path (B2V_FLAG_DAMAGE): only the listed 16x16 tiles of the output, the others keep the previous picture -------
+// blockDim (64, CT_TILES): one tile per 64 threads, one thread per 2x2 block of it.  tiles[k] = ty * tiles_w + tx, n of them (n
+// may be 0: the one launch of the picture then writes nothing).
+constexpr int CT_TILES = 4;
+__global__ void __launch_bounds__(64 * CT_TILES) csc_tiles(CscSource p, const int* __restrict__ tiles, int n, int tiles_w) {
+  const int k = blockIdx.x * CT_TILES + threadIdx.y;
+  if (k >= n) return;
+  const int t = tiles[k], tx = t % tiles_w, ty = t / tiles_w;
+  const int bx = tx * 8 + (threadIdx.x & 7), by = ty * 8 + (threadIdx.x >> 3);
+  if (bx * 2 >= p.coded_w || by * 2 >= p.coded_h) return;
+  csc_block(p, bx, by);
 }
 
 // ---- scaled path: fused bilinear scale + CSC through a shared-memory tile -----------------------------------------------------
@@ -413,6 +433,46 @@ void make_taps_host(Tap* t, int dn, int sn) {
     int i0 = (int)(pos >> 16);
     t[d] = Tap{i0, i0 + 1 < sn ? i0 + 1 : sn - 1, (int)((pos >> 8) & 255), 0};
   }
+}
+
+// B2V_FLAG_DAMAGE: rectangles -> dirty 16x16 tiles of a dst_w x dst_h output (include/b2video.h, b2v_damage_tiles).  tx / ty:
+// the taps of the scale (null at 1:1).  A tile's source footprint is the union of its pixels' taps, i0 of its first pixel to i1 of
+// its last (the taps are monotone); the chroma of a 2x2 block lies in the block's own tile, so no footprint crosses a tile.  Each
+// rectangle marks the tile columns and the tile rows its footprint meets; the map is their product, rectangle by rectangle.
+int damage_tiles(const Tap* tx, const Tap* ty, int src_w, int src_h, int dst_w, int dst_h, const b2v_rect* rects, int n, uint8_t* map) {
+  const int tw = (dst_w + 15) / 16, th = (dst_h + 15) / 16;
+  memset(map, 0, (size_t)tw * th);
+  std::vector<uint8_t> cols(tw), rows(th);
+  // footprint [lo, hi] of tile c of an axis of dn output and sn source pixels
+  auto span = [](const Tap* t, int c, int dn, int& lo, int& hi) {
+    const int a = 16 * c, b = 16 * c + 15 < dn ? 16 * c + 15 : dn - 1;
+    lo = t ? t[a].i0 : a; hi = t ? t[b].i1 : b;
+  };
+  int dirty = 0;
+  for (int r = 0; r < n; r++) {
+    const int x0 = rects[r].x > 0 ? rects[r].x : 0, y0 = rects[r].y > 0 ? rects[r].y : 0;
+    const int64_t x1e = (int64_t)rects[r].x + rects[r].w, y1e = (int64_t)rects[r].y + rects[r].h;   // exclusive ends
+    const int x1 = (int)(x1e < src_w ? x1e : src_w) - 1, y1 = (int)(y1e < src_h ? y1e : src_h) - 1;
+    if (x1 < x0 || y1 < y0) continue;
+    int c0 = tw, c1 = -1, r0 = th, r1 = -1;
+    for (int c = 0; c < tw; c++) {
+      int lo, hi; span(tx, c, dst_w, lo, hi);
+      if (lo <= x1 && hi >= x0) { c0 = c < c0 ? c : c0; c1 = c; }
+    }
+    for (int c = 0; c < th; c++) {
+      int lo, hi; span(ty, c, dst_h, lo, hi);
+      if (lo <= y1 && hi >= y0) { r0 = c < r0 ? c : r0; r1 = c; }
+    }
+    for (int y = r0; y <= r1; y++)
+      for (int x = c0; x <= c1; x++) { uint8_t& m = map[(size_t)y * tw + x]; dirty += !m; m = 1; }
+  }
+  return dirty;
+}
+
+int launch_csc_tiles(const CscSource& p, const int* d_tiles, int n, cudaStream_t st) {
+  const int tiles_w = (p.dst_w + 15) / 16;
+  csc_tiles<<<n > 0 ? (n + CT_TILES - 1) / CT_TILES : 1, dim3(64, CT_TILES), 0, st>>>(p, d_tiles, n, tiles_w);
+  return 1;
 }
 
 // Opt-in dynamic shared memory above 48 KB.  cudaFuncSetAttribute applies to the CURRENT device only, so the size already

@@ -119,6 +119,22 @@ class FrameSource:
         raise NotImplementedError
 
 
+class DamageFrameSource(FrameSource):
+    """Producer of BGRA frames that knows what changed (X11 XDamage, PipeWire's SPA_META_VideoDamage, wlroots screencopy
+    damage, DXGI dirty rects).  `fill_damage(view, index, whole)` writes frame `index` into the (H,W,4) view of a pinned ring
+    slot and returns the (x, y, w, h) rectangles that changed since the previous frame, or None to end the stream.  With
+    whole=False only those rectangles need writing: the slot holds stale pixels elsewhere, and only the rectangles are copied
+    to the GPU.  With whole=True (the first frame, after every update_resolution, and whenever the library needs a whole picture
+    or the list is longer than B2V_MAX_DAMAGE_RECTS) the whole frame must be written; the rectangles are then ignored.  The
+    rectangles must cover every pixel that changed: the stream is then exactly that of whole frames."""
+
+    def fill(self, view, index):
+        return self.fill_damage(view, index, True) is not None
+
+    def fill_damage(self, view: np.ndarray, index: int, whole: bool):   # pragma: no cover - interface
+        raise NotImplementedError
+
+
 class DeviceFrameSource:
     """Producer of frames in device memory.  `frame(index)` returns a device array (any object with `__cuda_array_interface__`,
     uint8 (H, W, 4) or (H, W, 3) as `pixel_format` says) covering the whole surface, or None to end the stream.  ScreenCapture
@@ -221,6 +237,7 @@ class ScreenCapture:
         self._fps = 60.0
         self._cursor_cb = None
         self._origin = (0, 0)
+        self._need_whole = True                  # a DamageFrameSource writes the whole next frame
         self.frames_emitted = 0
 
     # -- lifecycle ----------------------------------------------------------------------------------
@@ -255,6 +272,7 @@ class ScreenCapture:
             s.header_mode = N.B2V_HDR_PIXELFLUX       # callers strip / keep the 10-byte header themselves
             s.ring_slots = 4
             s.flags = 0
+            s.damage = isinstance(self._source, DamageFrameSource)
             s.quality = bool(getattr(settings, "quality_metrics", False))      # b2v_create refuses it in JPEG mode
             s.droppable = bool(getattr(settings, "h264_droppable_frames", False))
             if s.droppable and (jpeg or not bool(getattr(settings, "h264_fullframe", True))):
@@ -298,6 +316,7 @@ class ScreenCapture:
             if self._source is None:
                 self._source = SyntheticDesktopSource()
             self._source.configure(w, h)
+            self._need_whole = True
             self._stop.clear()
             self._thread = threading.Thread(target=self._capture_loop, name="b2v-capture", daemon=True)
             self._thread.start()
@@ -354,6 +373,7 @@ class ScreenCapture:
                 height -= height & 1
                 self._session.set_resolution(width, height)
                 self._source.configure(width, height)
+                self._need_whole = True
 
     def set_cursor_callback(self, fn) -> None:       # selkies.py:3166-3167 (guarded by hasattr)
         self._cursor_cb = fn
@@ -404,10 +424,33 @@ class ScreenCapture:
             slot, view = session.acquire()
         except N.B2VError:
             return False                          # the session is stopping
+        if isinstance(self._source, DamageFrameSource):
+            return self._encode_damage(session, slot, view, index)
         if not self._source.fill(view, index):
             session.release_slot(slot)            # end of the source: nothing to encode
             return False
         session.submit_slot(slot, time.monotonic_ns())
+        return True
+
+    def _encode_damage(self, session: Session, slot: int, view, index: int) -> bool:
+        """Frame `index` of a DamageFrameSource: its rectangles, or the whole frame when the session needs one."""
+        rects = self._source.fill_damage(view, index, self._need_whole)
+        if rects is None:
+            session.release_slot(slot)
+            return False
+        if not self._need_whole:
+            if len(rects) <= N.B2V_MAX_DAMAGE_RECTS:
+                try:
+                    session.submit_slot(slot, time.monotonic_ns(), damage=rects)
+                    return True
+                except N.B2VError as e:
+                    if e.code != N.B2V_ESTATE:
+                        raise
+            if self._source.fill_damage(view, index, True) is None:    # the slot is still ours: write the whole frame
+                session.release_slot(slot)
+                return False
+        session.submit_slot(slot, time.monotonic_ns())
+        self._need_whole = False
         return True
 
     def _on_frame(self, fptr):

@@ -164,6 +164,24 @@ def tensor_frame_args(frame, width: int, height: int, device: int, *, channels: 
     return t, _producer_stream(frame, cai, torch, stream)
 
 
+def normalize_rects(rects, width: int, height: int, cap: int = N.B2V_MAX_DAMAGE_RECTS) -> list:
+    """Damage rectangles (x, y, w, h) clipped to the width x height frame, empty ones dropped; a list longer than `cap` is merged
+    into `cap` bounding boxes of runs of rectangles in top-to-bottom order.  Every pixel of the input lies in the output."""
+    out = []
+    for r in rects:
+        x, y, w, h = (int(v) for v in r)
+        if w < 0 or h < 0:
+            raise ValueError(f"damage rectangle {tuple(r)} has a negative size")
+        x0, y0, x1, y1 = max(x, 0), max(y, 0), min(x + w, width), min(y + h, height)
+        if x1 > x0 and y1 > y0:
+            out.append((x0, y0, x1, y1))
+    if len(out) > cap:
+        out.sort(key=lambda b: (b[1], b[0]))
+        runs = [out[len(out) * k // cap: len(out) * (k + 1) // cap] for k in range(cap)]
+        out = [(min(b[0] for b in g), min(b[1] for b in g), max(b[2] for b in g), max(b[3] for b in g)) for g in runs]
+    return [(x0, y0, x1 - x0, y1 - y0) for x0, y0, x1, y1 in out]
+
+
 # the opt-in H.264 flags: Session keyword and attribute -> B2V_FLAG_* bit
 _OPT_IN_FLAGS = {"quality": N.B2V_FLAG_QUALITY, "droppable": N.B2V_FLAG_DROPPABLE, "wide_motion": N.B2V_FLAG_WIDE_MOTION,
                  "long_term_ref": N.B2V_FLAG_LONG_TERM_REF}
@@ -175,8 +193,10 @@ class Session:
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
                  collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False,
-                 long_term_ref: bool = False):
+                 long_term_ref: bool = False, damage: bool = False):
         self._lib = N.lib()
+        flags |= N.B2V_FLAG_DAMAGE if damage else 0
+        self.damage = bool(flags & N.B2V_FLAG_DAMAGE)      # the damage submits (damage=[...]) need it
         asked = dict(quality=quality, droppable=droppable, wide_motion=wide_motion, long_term_ref=long_term_ref)
         for name, bit in _OPT_IN_FLAGS.items():      # the attribute reports the bit, whether the keyword or `flags` set it
             flags |= bit if asked[name] else 0
@@ -224,15 +244,24 @@ class Session:
         return FrameQuality.from_native(q)
 
     # -- ingest ---------------------------------------------------------------------------------
-    def submit(self, bgra: np.ndarray, capture_ns: int = 0) -> None:
-        """Copy one (H,W,4) uint8 BGRA frame into the next pinned ring slot and enqueue it."""
+    def submit(self, bgra: np.ndarray, capture_ns: int = 0, damage=None) -> None:
+        """Copy one (H,W,4) uint8 BGRA frame into the next pinned ring slot and enqueue it.  `damage` (Session(damage=True)): the
+        (x, y, w, h) regions that changed since the previous picture; only they are written into the slot and copied to the
+        device (normalize_rects: clipped, merged past the cap).  When the library needs a whole picture first (B2V_ESTATE: the
+        first picture, after a resize or after a device picture) the whole frame is written and submitted instead."""
         assert bgra.dtype == np.uint8 and bgra.shape == (self.height, self.width, 4), bgra.shape
-        slot = C.c_int32(-1)
-        p = self._lib.b2v_ring_acquire(self._h, C.byref(slot))
-        if not p:
-            N.check(N.B2V_ESTATE)
-        C.memmove(p, np.ascontiguousarray(bgra).ctypes.data, self.width * self.height * 4)
-        N.check(self._lib.b2v_ring_submit(self._h, slot.value, self.width * 4, capture_ns))
+        slot, view = self.acquire()
+        if damage is not None:
+            rects = normalize_rects(damage, self.width, self.height)
+            for x, y, w, h in rects:
+                view[y:y + h, x:x + w] = bgra[y:y + h, x:x + w]
+            arr, n = N.rect_array(rects)
+            rc = self._lib.b2v_ring_submit_damage(self._h, slot, self.width * 4, arr, n, capture_ns)
+            if rc != N.B2V_ESTATE:
+                N.check(rc)
+                return
+        view[...] = bgra
+        N.check(self._lib.b2v_ring_submit(self._h, slot, self.width * 4, capture_ns))
 
     def acquire(self):
         """Zero-copy ingest: returns (slot, numpy view of the pinned slot) to fill in place."""
@@ -247,8 +276,11 @@ class Session:
         """Give the most recently acquired slot back without encoding it."""
         N.check(self._lib.b2v_ring_release(self._h, slot))
 
-    def submit_slot(self, slot: int, capture_ns: int = 0) -> None:
-        N.check(self._lib.b2v_ring_submit(self._h, slot, self.width * 4, capture_ns))
+    def submit_slot(self, slot: int, capture_ns: int = 0, damage=None) -> None:
+        """Enqueue an acquired slot.  `damage`: the rectangles written into it, passed through as they are (b2v_ring_submit_damage;
+        raises B2VError B2V_ESTATE with the slot still acquired when the library needs a whole picture first)."""
+        arr, n = N.rect_array(damage)
+        N.check(self._lib.b2v_ring_submit_damage(self._h, slot, self.width * 4, arr, n, capture_ns))
 
     def resident_upload(self, index: int, bgra: np.ndarray) -> None:
         bgra = np.ascontiguousarray(bgra)
@@ -257,23 +289,26 @@ class Session:
     def submit_resident(self, index: int, capture_ns: int = 0) -> None:
         N.check(self._lib.b2v_submit_resident(self._h, index, capture_ns))
 
-    def submit_device(self, frame, *, pixel_format: str = "BGRA", stream=None, origin=(0, 0), capture_ns: int = 0) -> None:
+    def submit_device(self, frame, *, pixel_format: str = "BGRA", stream=None, origin=(0, 0), capture_ns: int = 0, damage=None) -> None:
         """Encode the `width` x `height` window at `origin` = (x, y) of a frame in device memory of the session's GPU, without a
         copy: `frame` is any object with `__cuda_array_interface__` (torch, CuPy, Numba), uint8 (H, W, 4) for BGRA / RGBA or
         (H, W, 3) for BGR / RGB.  The conversion runs in stream order after the producer's stream (see device_frame_args), and
-        that stream waits for it in turn: the frame may be overwritten in stream order as soon as this returns."""
+        that stream waits for it in turn: the frame may be overwritten in stream order as soon as this returns.  `damage`: the
+        changed rectangles of the window, passed through (b2v_submit_device_damage)."""
         ptr, pitch, fmt, handle = device_frame_args(frame, self.width, self.height, self.device, pixel_format, origin, stream)
-        N.check(self._lib.b2v_submit_device(self._h, ptr, pitch, fmt, handle, capture_ns))
+        arr, n = N.rect_array(damage)
+        N.check(self._lib.b2v_submit_device_damage(self._h, ptr, pitch, fmt, arr, n, handle, capture_ns))
 
     def submit_tensor(self, frame, *, channels: str = "RGB", layout: str = "CHW", dtype=None, stream=None, origin=(0, 0),
-                      capture_ns: int = 0) -> None:
+                      capture_ns: int = 0, damage=None) -> None:
         """Encode the `width` x `height` window at `origin` of a 3-D tensor in device memory of the session's GPU as it is: uint8,
         or fp16 / bf16 / fp32 in [0, 1], planar or interleaved, any strides (tensor_frame_args).  The colour conversion
         quantises the elements as it reads them: no clamp / scale / cast / permute pass is needed in front.  Stream order as
-        submit_device."""
+        submit_device; `damage` as submit_device."""
         t, handle = tensor_frame_args(frame, self.width, self.height, self.device, channels=channels, layout=layout, dtype=dtype,
                                       origin=origin, stream=stream)
-        N.check(self._lib.b2v_submit_tensor(self._h, C.byref(t), handle, capture_ns))
+        arr, n = N.rect_array(damage)
+        N.check(self._lib.b2v_submit_tensor_damage(self._h, C.byref(t), arr, n, handle, capture_ns))
 
     def flush(self) -> None:
         N.check(self._lib.b2v_flush(self._h))
