@@ -412,9 +412,14 @@ TAP = np.array([1, -5, 20, 20, -5, 1], np.int64)
 def luma_inter(ref, x0, y0, mv, n=16, rows=None):
     """8.4.2.2.1: the n x n luma prediction at (x0, y0) for quarter-sample vector mv, reference coordinates clamped to the
     plane (rows = (first, last) row for a band-clamped reference)."""
+    return luma_planes(ref, x0 + (mv[0] >> 2), y0 + (mv[1] >> 2), n, rows)[(mv[0] & 3, mv[1] & 3)]
+
+
+def luma_planes(ref, xi, yi, n=16, rows=None):
+    """8.4.2.2.1: {(xFrac, yFrac): the n x n luma prediction whose full-sample part is the position (xi, yi)}, all sixteen from one
+    set of half-sample planes."""
     h, w = ref.shape
     r0, r1 = rows if rows is not None else (0, h - 1)
-    xi, yi, fx, fy = x0 + (mv[0] >> 2), y0 + (mv[1] >> 2), mv[0] & 3, mv[1] & 3
     ys = np.clip(np.arange(yi - 2, yi + n + 4), r0, r1)
     xs = np.clip(np.arange(xi - 2, xi + n + 4), 0, w - 1)
     W = ref[np.ix_(ys, xs)].astype(np.int64)             # W[r + 2, c + 2] = sample (xi + c, yi + r)
@@ -428,11 +433,10 @@ def luma_inter(ref, x0, y0, mv, n=16, rows=None):
 
     def avg(p, q):
         return (p + q + 1) >> 1
-    table = {(0, 0): G, (1, 0): avg(G, b), (2, 0): b, (3, 0): avg(Hs, b),
-             (0, 1): avg(G, hh), (1, 1): avg(b, hh), (2, 1): avg(b, j), (3, 1): avg(b, m),
-             (0, 2): hh, (1, 2): avg(hh, j), (2, 2): j, (3, 2): avg(j, m),
-             (0, 3): avg(M, hh), (1, 3): avg(hh, s), (2, 3): avg(j, s), (3, 3): avg(m, s)}
-    return table[(fx, fy)]
+    return {(0, 0): G, (1, 0): avg(G, b), (2, 0): b, (3, 0): avg(Hs, b),
+            (0, 1): avg(G, hh), (1, 1): avg(b, hh), (2, 1): avg(b, j), (3, 1): avg(b, m),
+            (0, 2): hh, (1, 2): avg(hh, j), (2, 2): j, (3, 2): avg(j, m),
+            (0, 3): avg(M, hh), (1, 3): avg(hh, s), (2, 3): avg(j, s), (3, 3): avg(m, s)}
 
 
 def chroma_inter(ref, xc0, yc0, mv, n=8, rows=None):
@@ -472,10 +476,10 @@ def mv_ok(vx, vy):
     return -MV_MAX_FULL <= vx <= MV_MAX_FULL and -MV_MAX_FULL <= vy <= MV_MAX_FULL
 
 
-def full_search(src_blk, ref, x0, y0, qp, rows=None, centre=(0, 0)):
-    """Brute force over the window centred on the full-sample vector `centre` — dx in [-16, 15], dy in [-16, 16] around it —
-    with clamped coordinates (8.4.2.2.1: a full-sample prediction is the reference sample at the clamped position), the vectors
-    outside mv_ok left out: {(vx, vy) full samples: (SAD, cost)}."""
+def full_search(src_blk, ref, x0, y0, qp, rows=None, centre=(0, 0), dy_range=16):
+    """Brute force over the window centred on the full-sample vector `centre` — dx in [-16, 15], dy in [-dy_range, dy_range]
+    around it — with clamped coordinates (8.4.2.2.1: a full-sample prediction is the reference sample at the clamped position), the
+    vectors outside mv_ok left out: {(vx, vy) full samples: (SAD, cost)}."""
     h, w = ref.shape
     r0, r1 = rows if rows is not None else (0, h - 1)
     cx, cy = centre
@@ -484,13 +488,49 @@ def full_search(src_blk, ref, x0, y0, qp, rows=None, centre=(0, 0)):
     win = sliding_window_view(ref[np.ix_(ys, xs)].astype(np.int64), (16, 16))      # win[16 + dy, 16 + dx] = the prediction
     sads = np.abs(win - np.asarray(src_blk, np.int64)).sum(axis=(2, 3))
     out = {}
-    for dy in range(-16, 17):
+    for dy in range(-dy_range, dy_range + 1):
         for dx in range(-16, 16):
             v = (cx + dx, cy + dy)
             if mv_ok(*v):
                 s = int(sads[16 + dy, 16 + dx])
                 out[v] = (s, motion_cost(s, (4 * v[0], 4 * v[1]), qp))
     return out
+
+
+def search(src_blk, ref, x0, y0, qp, centre=(0, 0), dy_range=16):
+    """§5.3: the exhaustive search (dy_range 16), or the reduced one on new content (dy_range 2), in the window centred on `centre`:
+    the full-sample vector of the lowest key cost << 11 | (vy − cy + 16)·32 + (vx − cx + 16), so that equal costs go to the lower
+    row, then the lower column.  Returns (vector, SAD, cost)."""
+    costs = full_search(src_blk, ref, x0, y0, qp, centre=centre, dy_range=dy_range)
+    v = min(costs, key=lambda v: (costs[v][1], v[1], v[0]))
+    return v, costs[v][0], costs[v][1]
+
+
+NB8 = [(-1, -1), (0, -1), (1, -1), (-1, 0), (1, 0), (-1, 1), (0, 1), (1, 1)]    # §5.3: the refinement's neighbour order
+
+
+def refine(src_blk, ref, x0, y0, v, centre, sad_int, qp):
+    """§5.3 quarter-sample refinement of the full-sample vector v, found in the window centred on `centre` with SAD sad_int.  The gate:
+    |v − centre| ≤ 13 per component (the 6-tap support stays inside the window) and 96·λ < sad_int < 8192; closed, v stands.  Stage H
+    scores v and its 8 half-sample neighbours, stage Q the stage-H winner and its 8 quarter-sample neighbours, each by motion_cost
+    (SAD + λ·(bits(mvx) + bits(mvy)), 4 bits more when fractional) of the real vector and the lowest (cost, i) wins, i = 0 the
+    centre and 1..8 the neighbours in NB8's order: the centre wins ties.  Predictions by 8.4.2.2.1 on the clamped reference.
+    Returns (quarter-sample vector, whether the gate was open)."""
+    mv = (4 * v[0], 4 * v[1])
+    if not (abs(v[0] - centre[0]) <= 13 and abs(v[1] - centre[1]) <= 13
+            and EARLY_SAD_PER_LAMBDA * LAMBDA[qp] < sad_int < REFINE_MAX_SAD):
+        return mv, False
+    planes = luma_planes(ref, x0 + v[0] - 1, y0 + v[1] - 1, 17)       # every offset in [-3, 3] quarter samples around v
+    blk = np.asarray(src_blk, np.int64)
+
+    def cost(q):
+        ox, oy = q[0] - 4 * v[0] + 4, q[1] - 4 * v[1] + 4             # quarter samples from (v − 1), in [1, 7]
+        pred = planes[(ox & 3, oy & 3)][oy >> 2:(oy >> 2) + 16, ox >> 2:(ox >> 2) + 16]
+        return motion_cost(sad(blk, pred), q, qp)
+    for step in (2, 1):
+        cands = [mv] + [(mv[0] + step * i, mv[1] + step * j) for i, j in NB8]
+        mv = cands[min(range(9), key=lambda i: (cost(cands[i]), i))]
+    return mv, True
 
 
 def anchor_of(mbx, mby, mbw, band_r0, band_r1):
@@ -581,7 +621,8 @@ def predictor_test(src_blk, ref, x0, y0, k, centre, sad0, qp):
     """§5.3: the 3x3 test of full-sample candidate k (real vector) in the window centred on `centre`.  Every position's key is
     cost << 11 | index, cost = SAD + λ·(bits(4x) + bits(4y)) of the real vector and index = (y − cy + 16)·32 + (x − cx + 16) relative
     to the window, so equal costs go to the lower row, then the lower column.  Taken when the candidate's SAD ≤ 4·96·λ, its key is
-    below all 8 neighbours' (a strict local minimum) and at most the zero vector's key0 = (sad0 + 2λ) << 11 | 528."""
+    below all 8 neighbours' (a strict local minimum) and at most the zero vector's key0 = (sad0 + 2λ) << 11 | 528.  Returns the
+    candidate's SAD when taken, None otherwise."""
     lam = LAMBDA[qp]
     keys = {}
     for j in (-1, 0, 1):
@@ -591,34 +632,20 @@ def predictor_test(src_blk, ref, x0, y0, k, centre, sad0, qp):
             keys[(i, j)] = (s, (s + lam * (se_bits(4 * v[0]) + se_bits(4 * v[1]))) << 11 | (v[1] - centre[1] + 16) * 32 + (v[0] - centre[0] + 16))
     sadc, kc = keys.pop((0, 0))
     key0 = (sad0 + 2 * lam) << 11 | (16 * 32 + 16)
-    return sadc <= PRED_SAD_FACTOR * EARLY_SAD_PER_LAMBDA * lam and all(kc < kk for _, kk in keys.values()) and kc <= key0
+    taken = sadc <= PRED_SAD_FACTOR * EARLY_SAD_PER_LAMBDA * lam and all(kc < kk for _, kk in keys.values()) and kc <= key0
+    return sadc if taken else None
 
 
 class Exit:
-    """The lean pass's class of one macroblock (lean_exit) and what it allows the coded macroblock to be.  cls: "zero", "predictor",
-    "long-term" or "searched".  k: the predictor's full-sample candidate (or None); frac: the previous vector was fractional;
-    lean: the lean pass took the predictor (otherwise the search pass did, on the clamped window, with its refinement)."""
+    """The lean pass's class of one macroblock (lean_exit).  cls: "zero", "predictor", "long-term" or "searched".  k: the
+    predictor's full-sample candidate (or None); frac: the previous vector was fractional; lean: the lean pass took the predictor
+    (otherwise the search pass did, on the clamped window, with its refinement).  For decide(): sad0, the co-located SAD; tried,
+    the temporal predictor's candidate when it was tested (hit or not); centre and sad, the window and the SAD of a hit."""
 
-    def __init__(self, cls, k=None, frac=False, lean=False, search_pred=False):
+    def __init__(self, cls, k=None, frac=False, lean=False, search_pred=False, sad0=0, tried=None, centre=(0, 0), sad=0):
         self.cls, self.k, self.frac, self.lean = cls, k, frac, lean
         self.search_pred = search_pred          # "long-term": the search pass's predictor test would have hit
-
-    def allows(self, kind, ref_idx, mv):
-        """True when a coded macroblock (parsed kind, refIdx, vector in quarter samples) is what this class allows.  I_PCM overrides
-        every class."""
-        if kind == "I_PCM":
-            return True
-        if self.cls == "long-term":
-            return kind == "P_L0_16x16" and ref_idx == 1 and mv == (0, 0)
-        if ref_idx != 0:
-            return False
-        if self.cls == "zero":
-            return mv == (0, 0)
-        if self.cls == "predictor":
-            if not self.frac:
-                return mv == (4 * self.k[0], 4 * self.k[1])
-            return abs(mv[0] - 4 * self.k[0]) <= 3 and abs(mv[1] - 4 * self.k[1]) <= 3
-        return True
+        self.sad0, self.tried, self.centre, self.sad = sad0, tried, centre, sad
 
 
 def lean_exit(src_blk, ref, lt, prev, x0, y0, qp, wide=False, dist=(1, 1)):
@@ -638,21 +665,86 @@ def lean_exit(src_blk, ref, lt, prev, x0, y0, qp, wide=False, dist=(1, 1)):
     thr = EARLY_SAD_PER_LAMBDA * lam
     sad0 = sad(src_blk, full_pred(ref, x0, y0, (0, 0)))
     if sad0 <= thr:
-        return Exit("zero")
-    hit = None
+        return Exit("zero", sad0=sad0)
+    hit, tried = None, None
     if prev is not None and prev.kind in ("P_L0_16x16", "P_Skip"):
         mv = tuple(scale_mv(c, *dist) for c in prev.mv)
         cand = predictor_candidate(mv, wide)
-        if cand is not None and predictor_test(src_blk, ref, x0, y0, cand[0], cand[1], sad0, qp):
-            inside = x0 - 16 + cand[1][0] >= 0 and x0 + 32 + cand[1][0] <= ref.shape[1]
-            hit = cand[0], bool((mv[0] | mv[1]) & 3), inside
+        if cand is not None:
+            tried = cand[0]
+            s = predictor_test(src_blk, ref, x0, y0, cand[0], cand[1], sad0, qp)
+            if s is not None:
+                inside = x0 - 16 + cand[1][0] >= 0 and x0 + 32 + cand[1][0] <= ref.shape[1]
+                hit = cand, bool((mv[0] | mv[1]) & 3), inside, s
     if hit is not None and hit[2] and not hit[1]:
-        return Exit("predictor", hit[0], False, lean=True)
+        return Exit("predictor", hit[0][0], False, lean=True, sad0=sad0, tried=tried, centre=hit[0][1], sad=hit[3])
     if lt is not None and sad(src_blk, full_pred(lt, x0, y0, (0, 0))) <= thr:
-        return Exit("long-term", search_pred=hit is not None)
+        return Exit("long-term", search_pred=hit is not None, sad0=sad0, tried=tried)
     if hit is not None:
-        return Exit("predictor", hit[0], hit[1], lean=False)
-    return Exit("searched")
+        return Exit("predictor", hit[0][0], hit[1], lean=False, sad0=sad0, tried=tried, centre=hit[0][1], sad=hit[3])
+    return Exit("searched", sad0=sad0, tried=tried)
+
+
+class Decision:
+    """What §5.3 decides for one macroblock: ref_idx and mv (quarter samples) — what it is coded with unless the I_PCM rule of §5.7
+    sends it raw; ex, its lean_exit; path, how the vector was found: "zero", "long-term", "predictor" (the temporal predictor),
+    "anchor predictor", "search" or "reduced search"; full, centre and sad: the full-sample vector before refinement, the centre of
+    its window and its SAD; src: the vector a predictor hit came from; refined, the refinement's gate was open; second, the anchor's
+    second window won; bad, the new-content flag an anchor publishes with its vector."""
+
+    def __init__(self, ex, path, ref_idx=0, mv=(0, 0), full=(0, 0), centre=(0, 0), sad=0, src=None, refined=False, second=False):
+        self.ex, self.path, self.ref_idx, self.mv = ex, path, ref_idx, mv
+        self.full, self.centre, self.sad, self.src = full, centre, sad, src
+        self.refined, self.second = refined, second
+        self.bad = path not in ("zero", "long-term") and sad >= REFINE_MAX_SAD
+
+
+def decide(src_blk, ref, lt, prev, x0, y0, qp, wide=False, dist=(1, 1), anchor=None, coarse=None):
+    """§5.3 / §5.12 / §5.13: the final refIdx and vector of the macroblock at (x0, y0), after lean_exit (same arguments).  anchor:
+    the Decision of the macroblock's anchor (None: the macroblock is an anchor; anchors are decided first); coarse: for a wide-motion
+    anchor, its group's coarse vector (coarse_search).
+      - zero: (0, 0).  long-term: refIdx 1, (0, 0); an anchor publishes the zero vector with the new-content flag clear.
+      - a temporal-predictor hit: its candidate k, refined (refine) when the previous vector was fractional.
+      - otherwise, a macroblock that is no anchor tests its anchor's vector v the same way (predictor_candidate(v), predictor_test),
+        except that the zero vector is not tested twice: a zero candidate is skipped when the temporal predictor tested zero.  A hit
+        is refined when v is fractional.  A miss, with the anchor's new-content flag set and SAD(0,0) ≥ 8192, shrinks the search to
+        dy in [-2, 2] (the reduced search).
+      - otherwise the search of the co-located window, refined; for a wide-motion anchor, also the search of the window centred on
+        second_window(coarse) when there is one, which wins when its cost is lower (equal: the co-located window), refined in its
+        window.
+    The new-content flag: the full-sample SAD of the vector before refinement ≥ 8192 for a hit or a search, clear for the zero and
+    long-term exits."""
+    ex = lean_exit(src_blk, ref, lt, prev, x0, y0, qp, wide, dist)
+    if ex.cls == "zero":
+        return Decision(ex, "zero")
+    if ex.cls == "long-term":
+        return Decision(ex, "long-term", ref_idx=1)
+
+    def hit(path, k, centre, s, src):
+        frac = bool((src[0] | src[1]) & 3)
+        mv, refined = refine(src_blk, ref, x0, y0, k, centre, s, qp) if frac else ((4 * k[0], 4 * k[1]), False)
+        return Decision(ex, path, mv=mv, full=k, centre=centre, sad=s, src=src, refined=refined)
+    if ex.cls == "predictor":
+        return hit("predictor", ex.k, ex.centre, ex.sad, tuple(scale_mv(c, *dist) for c in prev.mv))
+    dy_range = 16
+    if anchor is not None:
+        cand = predictor_candidate(anchor.mv, wide)
+        if cand is not None and not (cand[0] == (0, 0) and ex.tried == (0, 0)):
+            s = predictor_test(src_blk, ref, x0, y0, cand[0], cand[1], ex.sad0, qp)
+            if s is not None:
+                return hit("anchor predictor", cand[0], cand[1], s, anchor.mv)
+        if anchor.bad and ex.sad0 >= REFINE_MAX_SAD:
+            dy_range = 2
+    v, s, c = search(src_blk, ref, x0, y0, qp, dy_range=dy_range)
+    centre, second = (0, 0), False
+    far = second_window(coarse) if wide and anchor is None else None
+    if far is not None:
+        v2, s2, c2 = search(src_blk, ref, x0, y0, qp, centre=far)
+        if c2 < c:
+            v, s, centre, second = v2, s2, far, True
+    mv, refined = refine(src_blk, ref, x0, y0, v, centre, s, qp)
+    return Decision(ex, "search" if dy_range == 16 else "reduced search", mv=mv, full=v, centre=centre, sad=s, refined=refined,
+                    second=second)
 
 
 def changed_count(src_y, ref_y, qp):

@@ -1,6 +1,7 @@
 """The encoder's decisions, macroblock by macroblock, against a second statement of DESIGN.md §5 that shares no code with either
 encoder: tests/h264_syntax_refs.py (on tests/h264_syntax.py) parses the bytes and follows the decoded picture buffer,
-tests/h264_model.py restates prediction, quantisation, decimation, motion cost, the lean pass's exits and the long-term marking rule.
+tests/h264_model.py restates prediction, quantisation, decimation, motion cost, the lean pass's exits, the search after it (anchor
+predictor, reduced and exhaustive search, second window, quarter-sample refinement) and the long-term marking rule.
 Byte parity with the oracle and libavcodec's decode pin conformance; these checks pin what is coded.
 
 Per stream (one per band in striped mode) and picture:
@@ -11,7 +12,7 @@ Per stream (one per band in striped mode) and picture:
   - A.3.1: every non-PCM macroblock_layer() is at most 3200 bits, its header within the budget of §5.7, every I_PCM sample equals
     the source;
   - no refIdx-0 P_L0_16x16 macroblock has cbp 0 and its P_Skip vector;
-  - the lean pass's exits (§5.3, §5.13): every P macroblock's coded refIdx and vector are what its class allows;
+  - motion (§5.3, §5.12, §5.13): every P macroblock not sent as I_PCM carries exactly the refIdx and vector M.decide gives it;
   - the long-term reference (§5.13): the marks, their operations, the override and the picture the DPB names follow the model's
     rule on the model's own changed(k);
   - the SPS: profile, constraint flags, level against Table A-1, reference frames, cropping and the VUI of §5.1.
@@ -136,6 +137,7 @@ class Stats:
         self.skip_next_to_lt = 0          # refIdx-0 P_Skip macroblocks with a refIdx-1 neighbour left or above
         self.scaled = 0                   # predictor-class macroblocks of pictures whose reference distances differ, previous vector fractional
         self.pcm_two_refs = 0             # I_PCM macroblocks in pictures with two references
+        self.paths = {}                   # how M.decide found vectors ("refined search", "anchor predictor", ...) -> count
 
     def count(self, kind, d=None):
         d = self.kinds if d is None else d
@@ -273,31 +275,62 @@ def check_picture(pic, recs, src, where, stats, wide=False):
     return rec
 
 
-def check_exits(pic, prev, recs, src_y, where, stats, wide=False):
-    """Every macroblock of P picture `pic` against the lean pass's class (M.lean_exit) from the source luma `src_y`, the model's
-    reconstructions of refIdx 0 and of the long-term picture (refIdx 1, while the picture has two references) and the previous
-    picture's parsed records `prev` (the picture just before in decoding order, reference or not): its coded refIdx and vector must
-    be what the class allows."""
-    mbw = pic.sps.mbw
+def check_exits(pic, prev, recs, src_y, where, stats, wide=False, dec=None):
+    """Every macroblock of P picture `pic` against the model's decision (M.decide) from the source luma `src_y`, the model's
+    reconstructions of refIdx 0 and of the long-term picture (refIdx 1, while the picture has two references), the previous
+    picture's parsed records `prev` (the picture just before in decoding order, reference or not) and, with wide motion, dec: the
+    decimated luma of this picture's source and of its reference's.  Anchors are decided first, then the rest with their anchor's
+    decision.  Every macroblock not sent as I_PCM must carry exactly the model's refIdx and vector (P_Skip: its inferred vector)."""
+    mbw, mbh = pic.sps.mbw, pic.sps.mbh
     ref = recs[pic.ref_list[0]][0]
     lt = recs[pic.ref_list[1]][0] if len(pic.ref_list) > 1 else None
     dist = (pic.index - pic.ref_list[0], prev.index - prev.ref_list[0] if prev.ref_list else 1)
     y = src_y.astype(np.int64)
-    for m in pic.mbs:
+    anchor = {m.addr: M.anchor_of(m.addr % mbw, m.addr // mbw, mbw, 0, mbh) for m in pic.mbs}
+    decided = {}
+    for m in sorted(pic.mbs, key=lambda m: anchor[m.addr] != (m.addr % mbw, m.addr // mbw)):       # anchors first
         mbx, mby = m.addr % mbw, m.addr // mbw
         x0, y0 = 16 * mbx, 16 * mby
         pm = prev.mbs[m.addr]
-        ex = M.lean_exit(y[y0:y0 + 16, x0:x0 + 16], ref, lt, pm, x0, y0, pic.qp, wide, dist)
-        assert ex.allows(m.kind, m.ref_idx, m.mv), \
-            f"{where} mb ({mbx},{mby}): class {ex.cls} (k {ex.k}, fractional {ex.frac}, lean {ex.lean}) but coded {m.kind} refIdx {m.ref_idx} mv {m.mv}"
+        blk = y[y0:y0 + 16, x0:x0 + 16]
+        is_anchor = anchor[m.addr] == (mbx, mby)
+        coarse = None
+        if wide and is_anchor:
+            coarse = M.coarse_search(dec[0], dec[1], mbx, mby, mbw, 0, mbh, M.sad(blk, ref[y0:y0 + 16, x0:x0 + 16]), pic.qp)
+        d = M.decide(blk, ref, lt, pm, x0, y0, pic.qp, wide, dist, None if is_anchor else decided[anchor[m.addr]], coarse)
+        decided[(mbx, mby)] = d
+        ex = d.ex
+        if m.kind != "I_PCM":
+            assert (m.ref_idx, m.mv) == (d.ref_idx, d.mv), \
+                f"{where} mb ({mbx},{mby}): the model decides refIdx {d.ref_idx} mv {d.mv} ({d.path}, class {ex.cls}, k {ex.k}, " \
+                f"refined {d.refined}, second window {d.second}) but coded {m.kind} refIdx {m.ref_idx} mv {m.mv}"
         stats.count(ex.cls, stats.exits)
         if ex.cls == "predictor":
             stats.count("predictor lean" if ex.lean else "predictor search", stats.exits)
             if dist[0] != dist[1] and (pm.mv[0] | pm.mv[1]) & 3:
                 stats.scaled += 1
+                # the candidate halving toward zero would give: where it differs, only the rounding of §5.12 codes this vector
+                toward = M.predictor_candidate(tuple(int(c / 2) for c in pm.mv), wide) if dist[0] < dist[1] else None
+                if toward is not None and toward[0] != ex.k:
+                    stats.count("scaled rounding decides", stats.paths)
         if ex.cls == "long-term" and ex.search_pred:
             inside = 16 <= x0 and x0 + 32 <= ref.shape[1]
             stats.count("long-term over edge predictor" if not inside else "long-term over fractional predictor", stats.exits)
+        d13 = max(abs(d.full[0] - d.centre[0]), abs(d.full[1] - d.centre[1])) == 13
+        for name, on in (("refined search", d.path == "search" and d.refined),
+                         ("refined predictor", d.path == "predictor" and d.refined),
+                         ("anchor predictor", d.path == "anchor predictor"),
+                         ("reduced search", d.path == "reduced search"),
+                         ("second window", d.second),
+                         # where a mistake in one rule changes the vector: each names the rule it exposes
+                         ("refined at |d| = 13", d.refined and d13),
+                         ("refined with SAD >= 4096", d.refined and d.sad >= 4096),
+                         ("reduced search at |dy| = 2", d.path == "reduced search" and abs(d.full[1]) == 2),
+                         ("anchor candidate rounded up", d.path == "anchor predictor" and d.full != (d.src[0] >> 2, d.src[1] >> 2)),
+                         ("refinement moves an inside fractional hit", d.path == "predictor" and d.refined and d.mv != (4 * d.full[0], 4 * d.full[1])
+                          and x0 - 16 + d.centre[0] >= 0 and x0 + 32 + d.centre[0] <= ref.shape[1])):
+            if on:
+                stats.count(name, stats.paths)
         if m.ref_idx == 1 and pic.ref_frame_nums[0] == pic.ref_frame_nums[1]:
             stats.lt_fn_twin += 1
         stats.pcm_two_refs += m.kind == "I_PCM" and lt is not None
@@ -365,7 +398,11 @@ def check_encoded(e: Encoded, stripe_rows=0):
                 assert np.array_equal(r[: vh // s, : vw // s], d), f"{where}: model reconstruction of plane {c} != libavcodec's decode"
             # the exits need the previous picture's records: a band left unsent (all skipped) in between hides them
             if not pic.idr and k > 0 and items[k - 1][0] == index - 1:
-                check_exits(pic, pics[k - 1], recs, src[0], where, stats, e.wide)
+                dec = None
+                if e.wide:     # the coarse search's planes: the decimated sources of this picture and of its reference
+                    ref_src = e.sources[items[pic.ref_list[0]][0]][0][y_start:y_start + band_mbh * 16]
+                    dec = M.decimate(src[0]), M.decimate(ref_src)
+                check_exits(pic, pics[k - 1], recs, src[0], where, stats, e.wide, dec)
             if ltr is not None:
                 ltr.picture(pic, recs, src[0], stats, y_start)
             recs.append(rec)
@@ -425,7 +462,7 @@ def cases():
     out.append(("predictor_paths", S.Config(130, 70, qp=30), synth.predictor_paths(130, 70), (0,), None, 0))
     still = synth.desktop(96, 64, 0)
     out.append(("paintover_burst", S.Config(96, 64, qp=40, paint=(2, 20, 3)), [still] * 8, (0,), None, 0))
-    return out + wide_cases() + ltr_cases()
+    return out + wide_cases() + ltr_cases() + motion_cases()
 
 
 WIDE = WS.FLAG_WIDE_MOTION
@@ -439,16 +476,16 @@ def blocky_noise(w, h, x0, y0, seed=11):
     return grey(w, h, grey_table(), luma[y0:y0 + h, x0:x0 + w])
 
 
-def band_bottom_scroll(w, h, rows, seed=13):
-    """Two BGRA pictures of 2x2-blocky grey noise, the second scrolled up by 4 px, with the last 4 luma rows of every band of `rows`
-    macroblock rows dark in the second (the first 4 of the next band in the first): the bottom group of each band matches the
-    reference exactly one decimated row below the band, where the coarse search must not look."""
+def band_bottom_scroll(w, h, rows, sx=0, seed=13):
+    """Two BGRA pictures of 2x2-blocky grey noise, the second scrolled up by 4 px and left by sx px, with the last 4 luma rows of every
+    band of `rows` macroblock rows dark in the second (4 rows lower in the first, the first 4 of the next band): the bottom group of
+    each band matches the reference exactly one decimated row below the band, where the coarse search must not look."""
     rng = np.random.default_rng(seed)
-    luma = rng.integers(48, 208, ((h + 4) // 2 + 1, w // 2)).repeat(2, 0).repeat(2, 1)[:h + 4]
+    luma = rng.integers(48, 208, ((h + 4) // 2 + 1, (w + sx) // 2 + 1)).repeat(2, 0).repeat(2, 1)[:h + 4, :w + sx]
     for y in range(16 * rows, h, 16 * rows):
         luma[y:y + 4] = 16
     inv = grey_table()
-    return [grey(w, h, inv, luma[:h]), grey(w, h, inv, luma[4:4 + h])]
+    return [grey(w, h, inv, luma[:h, :w]), grey(w, h, inv, luma[4:4 + h, sx:sx + w])]
 
 
 def moving_noise(w, h, n, v, seed=3):
@@ -526,6 +563,71 @@ def ltr_cases():
             ("droppable_fractional_pan", S.Config(128, 64, qp=22, flags=LS.FLAG_DROPPABLE), pan, (0,), None, 0)]
 
 
+def bars_over_texture(w, h, shifts, period=3, amp=40, seed=7):
+    """BGRA pictures of vertical bars (a cosine of `period` px) over a weak non-periodic texture (random cosines of 5..40 px, about
+    ±12 levels), both constant down each column.  Picture t holds the bars shifted left by shifts[t][0] px and the texture by
+    shifts[t][1] px: where the two shifts of a step differ by a whole period, the bars alone match at a vector the texture does not."""
+    rng = np.random.default_rng(seed)
+    comps = [(rng.uniform(5, 40), rng.uniform(0, 2 * np.pi)) for _ in range(6)]
+    x = np.arange(w, dtype=np.float64)
+    out, inv = [], grey_table()
+    for a, b in shifts:
+        tex = sum(np.cos(2 * np.pi * (x + b) / p + ph) for p, ph in comps) * 4
+        row = 128 + amp * np.cos(2 * np.pi * (x + a) / period) + tex
+        out.append(grey(w, h, inv, np.repeat(np.rint(row).astype(np.int64)[None, :], h, 0)))
+    return out
+
+
+def smooth_texture_pan(w, h, n, v, seed=9):
+    """n BGRA pictures of a smooth 2-D texture (random plane waves of 6..30 px) moving by v px per picture, fractional allowed (content
+    at (x, y) was at (x, y) + v one picture earlier)."""
+    rng = np.random.default_rng(seed)
+    waves_ = [(rng.uniform(6, 30), rng.uniform(0, 2 * np.pi), rng.uniform(0, 2 * np.pi)) for _ in range(8)]
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    inv = grey_table()
+    out = []
+    for t in range(n):
+        X, Y = xx + t * v[0], yy + t * v[1]
+        luma = 128 + sum(12 * np.cos(2 * np.pi * (X * np.cos(th) + Y * np.sin(th)) / p + ph) for p, th, ph in waves_)
+        out.append(grey(w, h, inv, np.clip(np.rint(luma), 16, 235).astype(np.int64)))
+    return out
+
+
+def noise_window_scroll(w, h, n, box, seed=21):
+    """n BGRA desktop pictures scrolling up 3 px per picture with a window of fresh grey noise (new every picture) at box = (x, y,
+    width, height): new content next to moving content."""
+    rng = np.random.default_rng(seed)
+    inv = grey_table()
+    out = []
+    for t in range(n):
+        f = synth.desktop(w, h + 3 * n, 0)[3 * t:3 * t + h].copy()
+        x, y, bw, bh = box
+        f[y:y + bh, x:x + bw] = grey(bw, bh, inv, rng.integers(16, 236, (bh, bw)))
+        out.append(f)
+    return out
+
+
+def motion_cases():
+    """The motion search after the lean pass (§5.3): each reaches what assert_targets names for it."""
+    # droppable: picture 2 (two back from picture 0) moves 2.75 px, so its vectors are 11 quarter samples; picture 3 (from picture 2)
+    # moves the bars 2 px and the texture -1 px: the halved predictor 6 rounds to the candidate 2, where only the bars match — a strict
+    # local minimum whose refinement codes a vector the search (at -1) never finds; halving toward zero (5) gives the candidate 1
+    return [("droppable_scaled_alias", S.Config(128, 64, qp=30, flags=LS.FLAG_DROPPABLE),
+             bars_over_texture(128, 64, [(0, 0), (0, 0), (2.75, 2.75), (4.75, 1.75)]), (0,), None, 0),
+            # a fractional pan at QP 22: the previous vector is fractional, its full-sample candidate hits inside the picture, and the
+            # refinement moves it (the lean pass must leave such a hit to the search pass)
+            ("fractional_pan_qp22", S.Config(128, 64, qp=22), [waves(128, 64, t, [(0, 64, 24, 1.25)], amp=30) for t in range(5)],
+             (0,), None, 0),
+            # 13.25 px across and 5.5 px up per picture: searched vectors at the refinement gate's edge, |dx| = 13
+            ("texture_pan_13", S.Config(160, 96, qp=26), smooth_texture_pan(160, 96, 3, (13.25, -5.5)), (0,), None, 0),
+            # fresh noise next to a scroll: anchors inside the noise raise the new-content flag, their groups run the reduced search
+            ("noise_window_scroll", S.Config(192, 128, qp=26), noise_window_scroll(192, 128, 3, (48, 32, 96, 64)), (0,), None, 0),
+            # the coarse search's band edges with wide motion: each band's bottom group matches best one decimated row past its band,
+            # 20 px across, so that a coarse search looking there moves the anchor's second window (and its coded vector)
+            ("wide_band_bottoms", S.Config(128, 208, qp=26, stripe_rows=5, flags=WIDE), band_bottom_scroll(128, 208, 5, sx=20), (0,),
+             None, 5)]
+
+
 def assert_targets(name, st):
     """What each case is there for, from the parsed streams and the model: a case that drifts away from its target fails."""
     ex = st.exits
@@ -548,6 +650,15 @@ def assert_targets(name, st):
             (st.marks, st.mark_at_fn0, st.mmco1_wrap, st.lt_age, st.lt_fn_twin)
     if name == "droppable_fractional_pan":
         assert st.scaled > 0, ex
+    # the search half of §5.3: every path M.decide restates, and the rules whose mistakes only these cases expose
+    want = {"qp26": ["refined search", "anchor predictor"], "pcm_noise_qp0_4": ["reduced search"],
+            "wide_scroll250_tall": ["second window"], "wide_band_bottoms": ["second window"],
+            "droppable_scaled_alias": ["scaled rounding decides", "refined predictor"],
+            "fractional_pan_qp22": ["refined predictor", "refinement moves an inside fractional hit"],
+            "texture_pan_13": ["refined at |d| = 13", "anchor candidate rounded up"],
+            "noise_window_scroll": ["reduced search at |dy| = 2", "refined with SAD >= 4096"]}
+    for path in want.get(name, []):
+        assert st.paths.get(path, 0) > 0, (path, st.paths)
 
 
 CASES = cases()
@@ -756,9 +867,10 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28, wide=False, shift=(-
     """A cut to new structured content (a gradient with noise, or 2x2-blocky noise, still for one picture, then translated by
     `shift` px plus mild noise).  On the translated picture the anchors search (§5.3).  For every anchor the model shows did
     search — SAD(0,0) above 96·λ and the temporal predictor (its previous vector) more than 4·96·λ off — the documented cost of
-    the coded vector is at most the brute-force minimum over the window, and equal to it when the vector is full-sample.
+    the coded vector is at most the brute-force minimum over the window, and equal to it when the vector is full-sample; and the
+    coded vector is exactly the model's: the search's winner (M.search), refined (M.refine).
     wide: with wide-range motion, over the co-located window and the window around the model's coarse vector × 4 (when §5.3
-    searches it), vectors outside the range left out; and the coded vector's full-sample part lies in one of them."""
+    searches it), vectors outside the range left out, the winner of the two by cost, the co-located window on equal cost."""
     rng = np.random.default_rng(5)
     sx, sy = shift
     ox, oy = max(24, -sx), max(20, -sy)                                  # the still picture's corner in the content
@@ -808,16 +920,17 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28, wide=False, shift=(-
             if costs[(0, 0)][0] <= early or (pv in costs and costs[pv][0] <= 4 * early):
                 continue
             checked += 1
+            v, s_, c_ = M.search(blk, ref, 16 * mbx, 16 * mby, qp)
+            centre = (0, 0)
             if wide:
                 coarse = M.coarse_search(dec_cur, dec_ref, mbx, mby, mbw, 0, mbh, costs[(0, 0)][0], qp)
-                centre = M.second_window(coarse)
-                if centre is not None:
-                    costs.update(M.full_search(blk, ref, 16 * mbx, 16 * mby, qp, centre=centre))
+                far_centre = M.second_window(coarse)
+                if far_centre is not None:
+                    costs.update(M.full_search(blk, ref, 16 * mbx, 16 * mby, qp, centre=far_centre))
+                    v2, s2, c2 = M.search(blk, ref, 16 * mbx, 16 * mby, qp, centre=far_centre)
+                    if c2 < c_:
+                        v, s_, centre = v2, s2, far_centre
                     far += 1
-                # the full-sample position the refinement started from: within 3 quarter samples of the coded vector
-                near = [(fx, fy) for fx in {m.mv[0] >> 2, -(-m.mv[0] // 4)} for fy in {m.mv[1] >> 2, -(-m.mv[1] // 4)}
-                        if abs(m.mv[0] - 4 * fx) <= 3 and abs(m.mv[1] - 4 * fy) <= 3]
-                assert any(v in costs for v in near), (y0, mbx, mby, m.mv, coarse)
             best = min(c for _, c in costs.values())
             pred = M.luma_inter(ref, 16 * mbx, 16 * mby, m.mv)
             cost = M.motion_cost(M.sad(blk, pred), m.mv, qp)
@@ -825,6 +938,9 @@ def search_optimality(make_enc, w, h, stripe_rows=0, qp=28, wide=False, shift=(-
                 assert cost <= best, (y0, mbx, mby, m.mv, cost, best)
             else:
                 assert cost == best, (y0, mbx, mby, m.mv, cost, best)
+            # exactly the search's winner, refined in its window
+            want, _ = M.refine(blk, ref, 16 * mbx, 16 * mby, v, centre, s_, qp)
+            assert m.mv == want, (y0, mbx, mby, m.mv, want, v, centre)
     assert anchors and checked >= 0.75 * anchors, (checked, anchors)
     assert far or not wide
 
