@@ -150,7 +150,7 @@ enum {
                                    b2v_set_resolution rejects a size at which stripe_rows would stripe.  It costs one kernel launch
                                    per P picture (kernel_launches), a copy of one picture on the pictures that mark, and coded
                                    width x height x 1.5 bytes. */
-  B2V_FLAG_DAMAGE        = 1024 /* damage rectangles (an ingest flag, not a coding flag: it works with H.264 full-frame and striped,
+  B2V_FLAG_DAMAGE        = 1024,/* damage rectangles (an ingest flag, not a coding flag: it works with H.264 full-frame and striped,
                                    B2V_FLAG_JPEG, B2V_FLAG_NO_ENCODE and every coding flag).  The b2v_*_damage submits take the
                                    regions of the source that changed since the previous picture; only those are copied and
                                    colour-converted.  The contract: when the rectangles cover every pixel that changed since the
@@ -158,6 +158,35 @@ enum {
                                    exactly those of a whole-frame submit of the same picture.  The ring then copies into one
                                    persistent device frame (the mirror, src_w x src_h x 4 bytes) instead of one device buffer per
                                    ring slot: at 4K that is 33 MB of HBM instead of ring_slots x 33 MB. */
+  B2V_FLAG_SCENE_CUT     = 2048 /* scene cuts: a P picture whose content is all new (an application switch, a slide change, a cut in a
+                                   video) is coded as an intra picture instead of predicted from a picture it no longer resembles.
+                                   The GPU decides per P picture, after the P analysis, which runs unchanged:
+                                     cost_inter = the sum over macroblocks of the luma cost of the prediction the analysis chose:
+                                                  SAD + lambda(QP) x (se(v) bits of both vector components, + 4 when the vector is
+                                                  fractional), a long-term macroblock counting the zero vector's bits, and 0 for a
+                                                  macroblock whose SAD is at most 96 x lambda(QP) (the zero-motion exit's threshold:
+                                                  its residual is quantisation noise); while a long-term picture is a reference, the
+                                                  smaller of that and the same cost of the long-term picture's zero vector, for every
+                                                  macroblock, so that content that comes back stays P;
+                                     cost_intra = the sum over macroblocks of the smallest luma SAD of Intra16x16 vertical,
+                                                  horizontal and DC prediction from the SOURCE picture's neighbouring samples
+                                                  (neighbours outside the picture unavailable, 8.3.3; slices ignored), + 16 x
+                                                  lambda(QP) per macroblock;
+                                     the picture is cut when cost_intra < cost_inter (lambda: the motion-search table, DESIGN.md §5.3).
+                                   A cut picture is a non-IDR intra picture: NAL type 1, every slice of slice_type 7, in the IDR
+                                   slice grid (idr_slice_mbs), at the QP the P picture would have had, with the frame_num,
+                                   nal_ref_idc and dec_ref_pic_marking() the P picture would have had; its macroblocks are coded by
+                                   the intra coder of IDR pictures.  It carries no parameter sets, is_key stays 0, the gop count,
+                                   the droppable layers and the long-term picture go on as after a P picture, and the SPS does not
+                                   change.  The next picture predicts from its reconstruction and finds no temporal predictor in it,
+                                   as after an IDR.  A consumer tells a cut picture by the slice_type of its first slice
+                                   (h264_nal.is_intra).  Works with CQP and CBR, paint-over, scaling, cropping, B2V_FLAG_QUALITY,
+                                   B2V_FLAG_WIDE_MOTION, B2V_FLAG_DROPPABLE, B2V_FLAG_LONG_TERM_REF (whose long-term candidate is
+                                   part of cost_inter) and B2V_FLAG_DAMAGE.  H.264 full-frame only: b2v_create rejects it
+                                   (B2V_EINVAL) with B2V_FLAG_JPEG, B2V_FLAG_NO_ENCODE or in striped mode, and b2v_set_resolution
+                                   rejects a size at which stripe_rows would stripe.  It costs two kernel launches per P picture
+                                   (kernel_launches: k_scene_cut, and k_intra_rows, which returns at once unless the picture was
+                                   cut), flagged variants of the analysis and entropy kernels, and 4 bytes per macroblock. */
 };
 
 /* B2V_FLAG_DAMAGE: one changed region of the source, in source pixels of the frame (or the device window) the submit names.

@@ -21,6 +21,7 @@ B2V_FLAG_QUALITY = 64
 B2V_FLAG_DROPPABLE = 128
 B2V_FLAG_WIDE_MOTION = 256
 B2V_FLAG_LONG_TERM_REF = 512
+B2V_FLAG_SCENE_CUT = 2048
 B2V_FLAG_DAMAGE = 1024
 B2V_MAX_DAMAGE_RECTS = 64
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3

@@ -189,6 +189,7 @@ constexpr CodingFlagRule kCodingFlags[] = {
   {B2V_FLAG_WIDE_MOTION, "B2V_FLAG_WIDE_MOTION", "searches H.264 P pictures", false, 0, nullptr},
   {B2V_FLAG_LONG_TERM_REF, "B2V_FLAG_LONG_TERM_REF", "keeps an H.264 reference picture", true, B2V_FLAG_DROPPABLE,
    "a non-reference picture cannot mark a long-term picture, and its reference is two pictures back"},
+  {B2V_FLAG_SCENE_CUT, "B2V_FLAG_SCENE_CUT", "codes H.264 P pictures as intra pictures", true, 0, nullptr},
 };
 
 // `flags` against the table for a picture of dst_h rows: 0, or B2V_EINVAL naming the flag.  No CUDA call.

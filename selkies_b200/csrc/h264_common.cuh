@@ -16,6 +16,7 @@ constexpr int COEF_BLOCKS = 27;            // 0 luma DC | 1..16 luma | 17,18 chr
 constexpr int MB_BITS_LIMIT = 3200;         // A.3.1: bits of macroblock_layer() per macroblock
 constexpr int MB_WORDS = 128;              // per-macroblock bit scratch: 128 x u32 = 4096 bits
 constexpr unsigned FULL = 0xffffffffu;
+constexpr int ME_EARLY_SAD_PER_LAMBDA = 96;   // P pictures: skip the search when SAD(0,0) <= 96 * lambda(qp) (the quantisation noise of the QP)
 
 struct __align__(8) MbInfo {
   int16_t mvx, mvy;        // quarter-sample units
@@ -43,6 +44,20 @@ struct LtrState {
   int32_t pad;
   LtrPic pic[2];
 };
+
+// B2V_FLAG_SCENE_CUT (DESIGN.md §5.14; oracle/h264_scut_ref.c).  k_scene_cut of P picture k sums the intra estimate and the
+// analysis's costs of every macroblock into `intra` and `inter`; the block that finishes last decides, writes cut[k & 1] and
+// zeroes the sums and `done` for the next picture.  cut[k & 1] is read by k_intra_rows and the entropy stage of picture k
+// (double-buffered for the same reason as LtrState::pic).
+struct ScutState {
+  unsigned long long intra, inter;
+  uint32_t done;
+  int32_t cut[2];
+  int32_t pad;
+};
+// the rule (include/b2video.h): a P picture is cut when SCUT_INTRA_WEIGHT x cost_intra < SCUT_INTER_WEIGHT x cost_inter; every
+// macroblock's cost_intra carries lambda x SCUT_INTRA_MB_BITS
+constexpr int SCUT_INTRA_WEIGHT = 1, SCUT_INTER_WEIGHT = 1, SCUT_INTRA_MB_BITS = 16;
 
 // Feedback record of the rate controller / paint-over scheduler.  fb[k & 1] is written after picture k (rc_step, last block of
 // its slice scan); picture k is CODED from fb[k & 1] as it stood before that — the state after picture k-2 — because the entropy
@@ -77,6 +92,7 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   int slice_cols;          // this picture's slices are a grid of slice_rows x slice_cols macroblocks in raster order: P pictures
                            // slice_rows x mbw, IDR pictures 1 x slice_cols, never more than one row (DESIGN.md §5.2)
   int idr, rc_mode, qp_fixed;
+  int islice;              // every slice is an I slice: an IDR picture, or a cut picture (B2V_FLAG_SCENE_CUT, set on the device)
   int paint_trigger, paint_qp, paint_burst;   // paint-over: `paint_burst` refinement pictures after `paint_trigger` all-skipped pictures (0 = off)
   int pic;                 // picture counter of this encoder (parity selects the feedback record and the double-buffered side data)
   long long target_bits;
@@ -127,7 +143,21 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   uint8_t* lt;             // the long-term reference picture's reconstruction (NV12, coded size), valid while ltr->epoch == ltr_epoch
   int ltr_epoch;           // IDR pictures coded so far (>= 1 in every P picture)
   int prev_idr;            // the previous picture is an IDR picture: changed(k-1) = mbs
+  // B2V_FLAG_SCENE_CUT (h264_intra.cu k_scene_cut): null without the flag and in IDR pictures
+  ScutState* scut;
+  int32_t* scut_cost;      // [mbs] the luma cost of the prediction the analysis chose (finish_mb of the flagged analysis kernels)
+  int cut_slice_cols, cut_n_slices, cut_slice_words, cut_chunks;   // the IDR grid, in which a cut picture is coded
 };
+
+// B2V_FLAG_SCENE_CUT: a P picture that k_scene_cut cut is coded as a non-IDR intra picture in the IDR grid.  The flagged variants of
+// the entropy kernels take their context through this; it leaves every other picture's as it is.
+__device__ __forceinline__ void apply_scene_cut(FrameCtx& f) {
+  if (f.scut && !f.idr && *reinterpret_cast<const volatile int32_t*>(&f.scut->cut[f.pic & 1])) {
+    f.islice = 1;
+    f.slice_rows = 1; f.slice_cols = f.cut_slice_cols; f.n_slices = f.cut_n_slices;
+    f.slice_words = f.cut_slice_words; f.chunks_per_slice = f.cut_chunks;
+  }
+}
 
 __device__ __forceinline__ int clip3i(int lo, int hi, int v) { return min(hi, max(lo, v)); }
 __device__ __forceinline__ int clip255(int v) { return min(255, max(0, v)); }

@@ -41,6 +41,9 @@ struct Encoder {
   // k_ltr_mark), and the marking state
   uint8_t* lt = nullptr;
   LtrState* ltr = nullptr;
+  // B2V_FLAG_SCENE_CUT: k_scene_cut's sums and decisions, and the analysis's cost of every macroblock
+  ScutState* scut = nullptr;
+  int32_t* scut_cost = nullptr;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
   // of picture k (packing stream) overlaps the analysis of picture k+1 (main stream)
   MbInfo* mbinfo[2] = {nullptr, nullptr};
@@ -210,6 +213,12 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     ECK(cudaMalloc((void**)&e->ltr, sizeof(LtrState)));
     ECK(cudaMemset(e->ltr, 0, sizeof(LtrState)));     // epoch 0: no long-term picture (every P picture has ltr_epoch >= 1)
   }
+  if (cfg->flags & B2V_FLAG_SCENE_CUT) {
+    ECK(cudaMalloc((void**)&e->scut, sizeof(ScutState)));
+    ECK(cudaMemset(e->scut, 0, sizeof(ScutState)));
+    ECK(cudaMalloc((void**)&e->scut_cost, mbs * sizeof(int32_t)));
+    ECK(cudaMemset(e->scut_cost, 0, mbs * sizeof(int32_t)));
+  }
   for (int b = 0; b < 2; b++) {
     ECK(cudaMalloc((void**)&e->mbinfo[b], mbs * sizeof(MbInfo)));
     ECK(cudaMemset(e->mbinfo[b], 0, mbs * sizeof(MbInfo)));
@@ -288,7 +297,7 @@ void encoder_destroy(Encoder* e) {
   void* ptrs[] = {e->recon[0], e->recon[1], e->recon[2], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
-                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse, e->lt, e->ltr};
+                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse, e->lt, e->ltr, e->scut, e->scut_cost};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -317,7 +326,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.cw = e->cfg.coded_w; f.ch = e->cfg.coded_h; f.mbw = e->mbw; f.mbh = e->mbh;
   const SliceGrid& g = idr ? e->idr_grid : e->p_grid;
   f.slice_rows = g.rows; f.slice_cols = g.cols; f.n_slices = g.n; f.slice_words = g.words; f.chunks_per_slice = g.chunks;
-  f.idr = idr; f.rc_mode = p->rc_mode; f.qp_fixed = p->qp_fixed; f.target_bits = p->target_bits;
+  f.idr = idr; f.islice = idr; f.rc_mode = p->rc_mode; f.qp_fixed = p->qp_fixed; f.target_bits = p->target_bits;
   f.frame_num = e->frame_num; f.idr_pic_id = e->idr_count; f.pic = (int)(e->pic & 0x7fffffff);
   f.nal_ref_idc = idr ? 3 : is_ref ? 2 : 0; f.ref_dist = ref_dist; f.prev_ref_dist = e->last_ref_dist;
   f.cur = p->cur; f.ref = e->recon[e->ref_buf]; f.recon = e->recon[wb];
@@ -332,6 +341,11 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   f.param_sets = e->param_sets; f.param_len = e->param_len; f.csc_ts = p->csc_ts; f.au = p->au; f.overflow = e->overflow;
   if (e->cfg.flags & B2V_FLAG_WIDE_MOTION) { f.wide = 1; f.dec_cur = e->dec[wb]; f.dec_ref = e->dec[e->ref_buf]; f.coarse = e->coarse; }
   if (e->cfg.flags & B2V_FLAG_LONG_TERM_REF) { f.ltr = e->ltr; f.lt = e->lt; f.ltr_epoch = e->idr_count; f.prev_idr = e->since_idr == 1; }
+  if ((e->cfg.flags & B2V_FLAG_SCENE_CUT) && !idr) {
+    f.scut = e->scut; f.scut_cost = e->scut_cost;
+    const SliceGrid& gi = e->idr_grid;
+    f.cut_slice_cols = gi.cols; f.cut_n_slices = gi.n; f.cut_slice_words = gi.words; f.cut_chunks = gi.chunks;
+  }
   int n = 0;
   // Two-stream schedule (no per-stage events requested): ANALYSIS of picture k on `st` (CSC before it, by the caller), ENTROPY
   // coding of picture k (CAVLC, slice build with the rate-control step, pack) on `st_pack`, overlapping
@@ -357,11 +371,17 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   //  * the copy's source, f.ref, is picture k-1's reconstruction, which only the analysis of picture k+1 overwrites;
   //  * the decision record pic[k & 1] is read by the entropy stage of picture k (after ev_analysed) and rewritten by k_ltr_mark of
   //    picture k+2, whose analysis waits for the pack of picture k (ev_packed, or the single stream).
+  // B2V_FLAG_SCENE_CUT: k_scene_cut and k_intra_rows of P picture k run on `st` behind the analysis and before k_ltr_mark (which
+  // may replace the long-term picture k_scene_cut reads; neither touches what the other writes), k_quality and ev_analysed.  k_scene_cut reads the costs the analysis of picture k stored; the decision cut[k & 1] is read by
+  // k_intra_rows of picture k on `st` and by its entropy stage after ev_analysed, and rewritten by k_scene_cut of picture k+2, whose
+  // analysis waits for the pack of picture k.  A cut picture's k_intra_rows overwrites this picture's reconstruction and side data,
+  // which only this picture's entropy stage and the next picture's analysis read, both behind it.
   const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
   if (overlap) cudaStreamWaitEvent(st, e->ev_packed[par], 0);           // pack of picture k-2 (no-op before the first two)
   if (f.wide) n += launch_coarse(f, st);      // every picture: its decimated plane; P pictures: the coarse vectors
   if (f.ltr && !idr) cudaMemsetAsync(&e->ltr->changed[par], 0, sizeof(int32_t), st);
   n += idr ? launch_intra(f, st) : launch_inter(f, st);
+  if (f.scut) n += launch_scene_cut(f, st);
   if (f.ltr && !idr) n += launch_ltr_mark(f, st);
   if (e->quality_off) {
     QualityParams q{};

@@ -59,7 +59,7 @@ __device__ __forceinline__ void mv_pred_skip(const MvCtx& m, int& px, int& py) {
 // intra_chroma_pred_mode, coded_block_pattern (intra me(v) mapping), mb_qp_delta
 template <class S>
 __device__ __forceinline__ void mb_header_i4(S& h, const FrameCtx& f, const MbInfo& mi, int mb, int mbx, int mby) {
-  put_ue(h, f.idr ? 0u : 5u);
+  put_ue(h, f.islice ? 0u : 5u);
   const uint8_t* own = f.i4modes + (size_t)mb * 16;
   const bool availA = left_in_slice(f, mbx), availB = top_in_slice(f, mby);
   const bool a_i4 = availA && f.mbinfo[mb - 1].type == MB_I4, b_i4 = availB && f.mbinfo[mb - f.mbw].type == MB_I4;
@@ -84,7 +84,7 @@ __device__ __forceinline__ void mb_header(S& h, const FrameCtx& f, const MbInfo&
   if (mi.type == MB_I4) mb_header_i4(h, f, mi, mb, mbx, mby);
   else if (mi.type == MB_I16) {
     const int tcode = 1 + mi.i16_mode + 4 * (mi.cbp >> 4) + ((mi.cbp & 15) ? 12 : 0);
-    put_ue(h, (uint32_t)(f.idr ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
+    put_ue(h, (uint32_t)(f.islice ? tcode : tcode + 5)); put_ue(h, mi.chroma_mode); put_se(h, 0);
   } else {
     put_ue(h, 0);
     if (two_refs) h.put(1, mi.i16_mode ? 0u : 1u);
@@ -96,7 +96,11 @@ __device__ __forceinline__ void mb_header(S& h, const FrameCtx& f, const MbInfo&
 // ------------------------------------------------------------------------------------------------ k_cavlc_mb
 constexpr int CAVLC_WARPS = 4;
 
-__global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
+// CUT (B2V_FLAG_SCENE_CUT, P pictures): the picture may have been cut (apply_scene_cut)
+template <bool CUT>
+__global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx fp) {
+  FrameCtx f = fp;
+  if (CUT) apply_scene_cut(f);
   __shared__ __align__(16) uint32_t s_words[CAVLC_WARPS][MB_WORDS];
   __shared__ __align__(16) int16_t s_lv[CAVLC_WARPS][32][16];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -110,9 +114,9 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   // (most macroblocks of a desktop picture leave through the P_Skip exit: nothing that only a coded macroblock needs — the bit
   // scratch, the mvd — is touched before it)
   const int cbp_l = mi.cbp & 15, cbp_c = mi.cbp >> 4;
-  const bool two_refs = f.ltr && !f.idr && f.ltr->pic[f.pic & 1].active;     // B2V_FLAG_LONG_TERM_REF (k_ltr_mark)
+  const bool two_refs = f.ltr && !f.islice && f.ltr->pic[f.pic & 1].active;     // B2V_FLAG_LONG_TERM_REF (k_ltr_mark)
   int mvdx = 0, mvdy = 0;
-  if (!f.idr) {
+  if (!f.islice) {
     const MvCtx mc = mv_ctx(f, mbx, mby);
     if (mi.type == MB_P16 && mi.cbp == 0 && mi.i16_mode == 0) {
       int sx, sy;
@@ -130,7 +134,7 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
   for (int i = lane; i < MB_WORDS; i += 32) words[i] = 0;
   if (mi.type == MB_PCM) {                       // I_PCM: only mb_type here; alignment + 384 raw samples are placed by k_slice_build
     if (lane == 0) {
-      const uint32_t code = f.idr ? 25u : 30u;
+      const uint32_t code = f.islice ? 25u : 30u;
       const int len = 2 * (31 - __clz(code + 1)) + 1;
       f.mb_words[(size_t)mb * MB_WORDS] = (code + 1) << (32 - len);
       f.mb_nbits[mb] = (uint32_t)len | 0x40000000u;
@@ -199,14 +203,14 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx f) {
 template <class S>
 __device__ __forceinline__ void slice_header(S& s, const FrameCtx& f, int first_mb, int qp, int frame_num) {
   put_ue(s, (uint32_t)first_mb);
-  put_ue(s, f.idr ? 7u : 5u);
+  put_ue(s, f.islice ? 7u : 5u);
   put_ue(s, 0);
   s.put(8, (uint32_t)(frame_num & 255));
   if (f.idr) put_ue(s, (uint32_t)(f.idr_pic_id & 15));
   // B2V_FLAG_LONG_TERM_REF: what k_ltr_mark decided for this picture (nothing without the flag)
   LtrPic lp{0, 0, 0, 0};
   if (f.ltr && !f.idr) lp = f.ltr->pic[f.pic & 1];
-  if (!f.idr) {
+  if (!f.islice) {
     // num_ref_idx_active_override_flag (two references while a long-term picture is one: the previous picture, then the long-term
     // one, the initial list of 8.2.4.2.1), ref_pic_list_modification_flag_l0
     if (lp.active) { s.put(1, 1); put_ue(s, 1); } else s.put(1, 0);
@@ -318,7 +322,10 @@ __device__ __forceinline__ bool wait_flag(const volatile int* flag, int tag) {
   return true;
 }
 
-__global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
+template <bool CUT>
+__global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx fp) {
+  FrameCtx f = fp;
+  if (CUT) apply_scene_cut(f);      // a cut picture has fewer blocks than the grid: the rest only count for the rate-control step
   __shared__ long long s_warp_sum[SLICE_THREADS / 32];
   __shared__ int s_warp_max[SLICE_THREADS / 32];
   __shared__ uint32_t s_nb[SLICE_THREADS];       // nbits | I_PCM flag (bit 30), 0xffffffff = skipped
@@ -334,7 +341,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
   const int n_chunks = (geo.n_mb + SLICE_THREADS - 1) / SLICE_THREADS;
   const int tag = f.pic + 1, qp = frame_qp(f);
   uint32_t* out = f.slice_buf + (size_t)s * f.slice_words;
-  bool active = k < n_chunks;
+  bool active = k < n_chunks && (!CUT || s < f.n_slices);
   const int idx0 = k * SLICE_THREADS, n = active ? min(SLICE_THREADS, geo.n_mb - idx0) : 0, mb_first = geo.mb0 + idx0;
   const bool last_chunk = active && k == n_chunks - 1;
   if (active) {
@@ -357,7 +364,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
     __syncthreads();
     if (first_coded) s_first = tid;
     const int run_local = tid - 1 - excl_max;  // for every coded macroblock but the first: its mb_skip_run
-    const int pre = (!skip && !first_coded && !f.idr) ? ue_len((uint32_t)run_local) : 0;
+    const int pre = (!skip && !first_coded && !f.islice) ? ue_len((uint32_t)run_local) : 0;
     const long long tot = skip ? 0 : (long long)pre + nbits;
     long long incl = tot;
 #pragma unroll
@@ -420,7 +427,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
           const long long rb2 = __shfl_sync(FULL, rb, t), ib2 = __shfl_sync(FULL, ib, t); const int it2 = __shfl_sync(FULL, it, t);
           const int n_j = min(SLICE_THREADS, geo.n_mb - (base + t) * SLICE_THREADS);
           if (h2 & 2) { bits = ib2; trail = it2; }
-          else if (h2 & 1) { bits += (f.idr ? 0 : ue_len((uint32_t)(trail + fr2))) + rb2; trail = tr2; }
+          else if (h2 & 1) { bits += (f.islice ? 0 : ue_len((uint32_t)(trail + fr2))) + rb2; trail = tr2; }
           else trail += n_j;
         }
       }
@@ -431,7 +438,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
     const long long bits_in = s_bits_in; const int trail_in = s_trail_in;
     // ---- final offsets ----------------------------------------------------------------------------------------------------------
     const int run_first = trail_in + first;
-    const int pre_first = (last_coded >= 0 && !f.idr) ? ue_len((uint32_t)run_first) : 0;
+    const int pre_first = (last_coded >= 0 && !f.islice) ? ue_len((uint32_t)run_first) : 0;
     int run = first_coded ? run_first : run_local;
     long long my_off = bits_in + off_local + ((!skip && !first_coded) ? pre_first : 0);
     s_nb[tid] = skip ? 0xffffffffu : (nbits | (pcm ? 0x40000000u : 0u)); s_run[tid] = run; s_off[tid] = my_off;
@@ -443,7 +450,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
         const uint32_t nb = s_nb[j];
         if (nb == 0xffffffffu) continue;
         s_off[j] = pos;
-        pos += (f.idr ? 0 : ue_len((uint32_t)s_run[j])) + (nb & 0x3fffffffu);
+        pos += (f.islice ? 0 : ue_len((uint32_t)s_run[j])) + (nb & 0x3fffffffu);
         if (nb & 0x40000000u) pos = ((pos + 7) & ~7LL) + 384 * 8;
       }
       s_bits_out = pos;
@@ -461,7 +468,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       if (last_chunk) {                          // trailing mb_skip_run, rbsp_trailing_bits
         BitWriter g{out, s_bits_out};
         const int runt = s_trail_out;
-        if (!f.idr && runt > 0) put_ue(g, (uint32_t)runt);
+        if (!f.islice && runt > 0) put_ue(g, (uint32_t)runt);
         f.slice_bits[s] = g.pos;
         if (runt < geo.n_mb) {                   // the slice holds a coded macroblock (benign races: every writer stores the same value)
           f.rc->pic_coded = 1;
@@ -505,7 +512,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
       const uint32_t nbits = v & 0x3fffffffu;
       const int mb = mb_first + i, mby = mb / f.mbw, mbx = mb - mby * f.mbw;
       long long pos = s_off[i];
-      if (!f.idr) {
+      if (!f.islice) {
         const uint32_t run = (uint32_t)s_run[i];
         if (sub == 0) { BitWriter g{out, pos}; put_ue(g, run); }
         pos += ue_len(run);
@@ -553,9 +560,13 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx f) {
 // ------------------------------------------------------------------------------------------------ k_pack_au
 constexpr int PACK_THREADS = ESC_THREADS;
 
-__global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long au_cap) {
+template <bool CUT>
+__global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx fp, long long au_cap) {
   __shared__ int s_wsum[PACK_THREADS / 32];
+  FrameCtx f = fp;
+  if (CUT) apply_scene_cut(f);
   const int s = blockIdx.x, tid = threadIdx.x;
+  if (CUT && s >= f.n_slices) return;       // a cut picture has fewer slices than the grid
   const SliceGeo geo = slice_geo(f, s);
   const int row0 = geo.row0, band = row0 / f.band_rows;
   const bool band_first = row0 == band * f.band_rows && geo.x0 == 0;      // this slice opens its band's access unit
@@ -608,17 +619,22 @@ __global__ void __launch_bounds__(PACK_THREADS) k_pack_au(FrameCtx f, long long 
   }
 }
 
+// B2V_FLAG_SCENE_CUT, P pictures: the flagged variants, on grids that cover both the P grid and the IDR grid a cut picture is coded in
 int launch_cavlc(const FrameCtx& f, cudaStream_t st) {
   const int mbs = f.mbw * f.mbh;
-  k_cavlc_mb<<<(mbs + CAVLC_WARPS - 1) / CAVLC_WARPS, 32 * CAVLC_WARPS, 0, st>>>(f);
+  if (f.scut && !f.idr) k_cavlc_mb<true><<<(mbs + CAVLC_WARPS - 1) / CAVLC_WARPS, 32 * CAVLC_WARPS, 0, st>>>(f);
+  else k_cavlc_mb<false><<<(mbs + CAVLC_WARPS - 1) / CAVLC_WARPS, 32 * CAVLC_WARPS, 0, st>>>(f);
   return 1;
 }
 int launch_slice_build(const FrameCtx& f, cudaStream_t st) {
-  k_slice_build<<<f.n_slices * f.chunks_per_slice, SLICE_THREADS, 0, st>>>(f);      // scan + copy + emulation-prevention count
+  if (f.scut && !f.idr)
+    k_slice_build<true><<<max(f.n_slices * f.chunks_per_slice, f.cut_n_slices * f.cut_chunks), SLICE_THREADS, 0, st>>>(f);
+  else k_slice_build<false><<<f.n_slices * f.chunks_per_slice, SLICE_THREADS, 0, st>>>(f);      // scan + copy + emulation-prevention count
   return 1;
 }
 int launch_pack_cap(const FrameCtx& f, long long au_cap, cudaStream_t st) {
-  k_pack_au<<<f.n_slices, PACK_THREADS, 0, st>>>(f, au_cap);
+  if (f.scut && !f.idr) k_pack_au<true><<<max(f.n_slices, f.cut_n_slices), PACK_THREADS, 0, st>>>(f, au_cap);
+  else k_pack_au<false><<<f.n_slices, PACK_THREADS, 0, st>>>(f, au_cap);
   return 1;
 }
 

@@ -29,7 +29,6 @@ namespace b2v {
 constexpr int WIN_ROWS = 48, WIN_WORDS = 12;
 constexpr int PW_ROWS = 24, PW_WORDS = 8;      // the part of the window around a temporal predictor (k_inter_lean)
 constexpr int WARPS_PER_BLOCK = 4;
-constexpr int ME_EARLY_SAD_PER_LAMBDA = 96;   // skip the search when SAD(0,0) <= 96 * lambda(qp)
 
 struct alignas(16) InterSm {      // one per warp; the 16-byte size padding keeps t's uint4 accesses aligned for every array element
   MbTile t;
@@ -305,10 +304,24 @@ __device__ __forceinline__ void publish_anchor(const FrameCtx& f, int mb, int sa
 // 48 + WM_MVD_BITS.
 constexpr int LTR_MV = -32768;
 constexpr uint32_t LTR_MV_WORD = 0x80008000u;
-template <bool WIDE>
+// COST (B2V_FLAG_SCENE_CUT): the macroblock's cost_inter into f.scut_cost, the value the exits and the search compare: the luma SAD of
+// the prediction plus lambda x (bits of the vector's components, + ME_FRAC_PENALTY_BITS for a fractional vector); the zero vector's
+// for refIdx 1.  0 when the SAD is within the zero-motion exit's threshold: the residual is quantisation noise, there is nothing to
+// code.  Whichever path chose the prediction, t.pred_y holds it here.
+template <bool WIDE, bool COST>
 __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc, bool ltr = false) {
   const bool ref1 = ltr && mvx == LTR_MV;
   const size_t ysz = (size_t)f.cw * f.ch;
+  if (COST) {      // first, while little is live (t.pred_y was written by other lanes: __syncwarp)
+    __syncwarp();
+    const int r8 = lane >> 1, c8 = (lane & 1) * 8;
+    const uint2 c = *reinterpret_cast<const uint2*>(&t.cur_y[r8][c8]), pr = *reinterpret_cast<const uint2*>(&t.pred_y[r8][c8]);
+    const int sad = __reduce_add_sync(FULL, (int)sad4acc(c.x, pr.x, sad4acc(c.y, pr.y, 0u)));
+    const int vx = ref1 ? 0 : mvx, vy = ref1 ? 0 : mvy;
+    const int lambda = me_lambda[qp];
+    if (lane == 0) f.scut_cost[p.mb] = sad <= ME_EARLY_SAD_PER_LAMBDA * lambda ? 0 : sad + lambda * (se_bits_dev(vx) + se_bits_dev(vy) + (((vx | vy) & 3) ? ME_FRAC_PENALTY_BITS : 0));
+  }
+
   const uint8_t* __restrict__ ref_uv = f.ref + ysz;
   const int rc4 = lane >> 2, cc4 = (lane & 3) * 4;
   const int mb = p.mb, mbx = p.mbx, mby = p.mby;
@@ -369,7 +382,8 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 // the search do not cap the occupancy of the common case.
 // LTR (B2V_FLAG_LONG_TERM_REF): the block counts changed(k) for k_ltr_mark, and while a long-term picture is a reference, a
 // macroblock that both exits fail is tested at the zero vector in it before it is queued (DESIGN.md §5.13).
-template <bool SCALE, bool WIDE, bool LTR>
+// CUT (B2V_FLAG_SCENE_CUT): every macroblock it finishes stores its cost (finish_mb).
+template <bool SCALE, bool WIDE, bool LTR, bool CUT>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) {
   __shared__ __align__(16) LeanSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -437,7 +451,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
     }
   }
   if (p.anchor && lane == 0) publish_anchor<WIDE>(f, m, sad_int, LTR && mvx == LTR_MV ? 0 : mvx, LTR && mvy == LTR_MV ? 0 : mvy);   // sad_int 0 for refIdx 1
-  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc, LTR);
+  finish_mb<WIDE, CUT>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc, LTR);
 }
 
 // One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
@@ -446,7 +460,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
 // WIDE (B2V_FLAG_WIDE_MOTION): sm.win may hold the window centred on a full-sample vector (wx, wy) other than (0, 0) — a temporal or
 // anchor predictor outside the co-located window's test range, or an anchor's coarse vector x 4; candidate indices and (dx, dy) are
 // relative to that centre, costs are those of the real vector.
-template <bool SCALE, bool WIDE>
+template <bool SCALE, bool WIDE, bool CUT>
 __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int lane, const MbPos& p) {
   const int mb = p.mb, x0 = p.mbx * 16, y0 = p.mby * 16;
   const bool anchor = p.anchor;
@@ -646,19 +660,19 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   }
   if (anchor && lane == 0) publish_anchor<WIDE>(f, mb, sad_int, mvx, mvy);
   if (!refine) full_sample_pred(win, t, lane, dxi, dyi);
-  finish_mb<WIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
+  finish_mb<WIDE, CUT>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
 // Passes B and C: the queue k_inter_lean filled (0: anchors, 1: the rest), walked by a grid of the kernel's resident capacity.  No
 // decision here depends on another entry of the same queue, so the order inside a queue does not matter.
-template <bool SCALE, bool WIDE>
+template <bool SCALE, bool WIDE, bool CUT>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search(FrameCtx f, int queue) {
   __shared__ __align__(16) InterSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = f.me_queue[queue];
   const int* q = f.me_queue + 2 + (size_t)queue * f.mbw * f.mbh;
   for (int i = blockIdx.x * WARPS_PER_BLOCK + warp; i < n; i += gridDim.x * WARPS_PER_BLOCK) {
-    search_mb<SCALE, WIDE>(f, sm_all[warp], lane, mb_pos(f, q[i]));
+    search_mb<SCALE, WIDE, CUT>(f, sm_all[warp], lane, mb_pos(f, q[i]));
     __syncwarp();
   }
 }
@@ -667,30 +681,35 @@ cudaError_t inter_search_grid(int* blocks) {
   int dev = 0, sms = 0, per_sm = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search<false, false>, 32 * WARPS_PER_BLOCK, 0);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inter_search<false, false, false>, 32 * WARPS_PER_BLOCK, 0);
   *blocks = sms * per_sm;
   return e;
 }
 
 // The three passes of a P picture: SCALE, the previous picture's vectors span another reference distance than this picture's
-// (B2V_FLAG_DROPPABLE); WIDE, B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream); LTR, B2V_FLAG_LONG_TERM_REF.
-template <bool SCALE, bool WIDE, bool LTR>
+// (B2V_FLAG_DROPPABLE); WIDE, B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream); LTR, B2V_FLAG_LONG_TERM_REF; CUT,
+// B2V_FLAG_SCENE_CUT (k_scene_cut follows).
+template <bool SCALE, bool WIDE, bool LTR, bool CUT>
 void launch_passes(const FrameCtx& f, int lean_blocks, cudaStream_t st) {
-  k_inter_lean<SCALE, WIDE, LTR><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
-  k_inter_search<SCALE, WIDE><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
-  k_inter_search<SCALE, WIDE><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+  k_inter_lean<SCALE, WIDE, LTR, CUT><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+  k_inter_search<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
+  k_inter_search<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
+}
+template <bool CUT>
+void launch_passes_for(const FrameCtx& f, int lean_blocks, cudaStream_t st) {
+  // The long-term reference never comes with droppable pictures (check_coding_flags), so with it both distances are 1: LTR
+  // implies !SCALE, and no <true, *, true, *> variant is compiled.
+  const bool scale = f.ref_dist != f.prev_ref_dist;
+  if (f.ltr) f.wide ? launch_passes<false, true, true, CUT>(f, lean_blocks, st) : launch_passes<false, false, true, CUT>(f, lean_blocks, st);
+  else if (scale) f.wide ? launch_passes<true, true, false, CUT>(f, lean_blocks, st) : launch_passes<true, false, false, CUT>(f, lean_blocks, st);
+  else f.wide ? launch_passes<false, true, false, CUT>(f, lean_blocks, st) : launch_passes<false, false, false, CUT>(f, lean_blocks, st);
 }
 
 int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
   const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  // The long-term reference never comes with droppable pictures (check_coding_flags), so with it both distances are 1: LTR
-  // implies !SCALE, and no <true, *, true> variant is compiled.
-  const bool scale = f.ref_dist != f.prev_ref_dist;
-  if (f.ltr) f.wide ? launch_passes<false, true, true>(f, lean_blocks, st) : launch_passes<false, false, true>(f, lean_blocks, st);
-  else if (scale) f.wide ? launch_passes<true, true, false>(f, lean_blocks, st) : launch_passes<true, false, false>(f, lean_blocks, st);
-  else f.wide ? launch_passes<false, true, false>(f, lean_blocks, st) : launch_passes<false, false, false>(f, lean_blocks, st);
+  if (f.scut) launch_passes_for<true>(f, lean_blocks, st); else launch_passes_for<false>(f, lean_blocks, st);
   return 3;
 }
 

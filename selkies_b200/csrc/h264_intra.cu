@@ -105,11 +105,15 @@ struct I4Result { int tried, mode_bits, cbp, bits; long long d; };
 
 __device__ __forceinline__ void i4_pair_barrier() { asm volatile("bar.sync 1, 64;" ::: "memory"); }   // the two Intra4x4 warps
 
+// CUT (B2V_FLAG_SCENE_CUT): a P picture, launched behind k_scene_cut on the IDR grid; it codes the picture only when it was cut, at the
+// P picture's QP (f.idr is 0), over what the P analysis wrote.
+template <bool CUT>
 __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
   __shared__ __align__(16) MbTile t;
   __shared__ __align__(16) IntraNb nb;
   __shared__ __align__(16) I4State i4;
   __shared__ I4Result r4;
+  if (CUT && !f.scut->cut[f.pic & 1]) return;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const SliceGeo geo = slice_geo(f, blockIdx.x);        // columns [x0, x1) of row row0
   const int mby = geo.row0;
@@ -324,8 +328,70 @@ __global__ void __launch_bounds__(96) k_intra_rows(FrameCtx f) {
 }
 
 int launch_intra(const FrameCtx& f, cudaStream_t st) {
-  k_intra_rows<<<f.n_slices, 96, 0, st>>>(f);
+  k_intra_rows<false><<<f.n_slices, 96, 0, st>>>(f);
   return 1;
+}
+
+// ---- k_scene_cut (B2V_FLAG_SCENE_CUT): once per P picture, behind its analysis (DESIGN.md §5.14; oracle/h264_scut_ref.c) ----
+// One warp per macroblock: cost_intra(mb), the smallest luma SAD of Intra16x16 vertical, horizontal and DC prediction (8.3.3) formed
+// from the SOURCE picture's neighbouring samples, available at the picture's edges only (no slices: an estimate, no reconstruction),
+// + lambda x SCUT_INTRA_MB_BITS (no intra macroblock is free, a noise-level inter one is), and cost_inter(mb), which the analysis
+// stored; while a long-term picture is a reference (B2V_FLAG_LONG_TERM_REF), the smaller of that and the cost of the long-term
+// picture's zero vector, the same way (0 within the noise threshold, else SAD + 2 lambda), for every macroblock: the lean pass tries
+// it only within the noise threshold, and returning content must stay P.  It runs before k_ltr_mark, so the long-term picture and
+// its epoch are those this picture was analysed with.  Per block the two sums go into the picture's totals; the last block to finish
+// decides: cut = SCUT_INTRA_WEIGHT x cost_intra < SCUT_INTER_WEIGHT x cost_inter.
+constexpr int SCUT_WARPS = 8;
+__global__ void __launch_bounds__(32 * SCUT_WARPS) k_scene_cut(FrameCtx f) {
+  __shared__ unsigned long long s_intra[SCUT_WARPS], s_inter[SCUT_WARPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int mb = blockIdx.x * SCUT_WARPS + warp;
+  if (mb < f.mbw * f.mbh) {
+    const int mby = mb / f.mbw, mbx = mb - mby * f.mbw, r8 = lane >> 1, c8 = (lane & 1) * 8;
+    const bool top = mby > 0, left = mbx > 0;
+    const uint8_t* src = f.cur + (size_t)(mby * 16 + r8) * f.cw + mbx * 16 + c8;
+    const uint32_t s0 = *reinterpret_cast<const uint32_t*>(src), s1 = *reinterpret_cast<const uint32_t*>(src + 4);
+    uint32_t t0 = 0, t1 = 0, l = 0;
+    if (top) { const uint8_t* a = f.cur + (size_t)(mby * 16 - 1) * f.cw + mbx * 16 + c8; t0 = *reinterpret_cast<const uint32_t*>(a); t1 = *reinterpret_cast<const uint32_t*>(a + 4); }
+    if (left) l = src[-c8 - 1];
+    const int st = __reduce_add_sync(FULL, lane < 2 ? (int)(__vsadu4(t0, 0u) + __vsadu4(t1, 0u)) : 0);   // row 0's lanes hold the row above
+    const int sl = __reduce_add_sync(FULL, (lane & 1) == 0 ? (int)l : 0);                               // one lane per row: the left column
+    const uint32_t pd = rep4(top && left ? (st + sl + 16) >> 5 : top ? (st + 8) >> 4 : left ? (sl + 8) >> 4 : 128), ph = rep4((int)l);
+    int best = (int)__reduce_add_sync(FULL, __vsadu4(s0, pd) + __vsadu4(s1, pd));
+    if (top) best = min(best, (int)__reduce_add_sync(FULL, __vsadu4(s0, t0) + __vsadu4(s1, t1)));
+    if (left) best = min(best, (int)__reduce_add_sync(FULL, __vsadu4(s0, ph) + __vsadu4(s1, ph)));
+    const int lambda = me_lambda[frame_qp(f)];
+    int inter = f.scut_cost[mb];
+    if (f.ltr && f.ltr->epoch == f.ltr_epoch) {     // the long-term picture is a reference: its zero vector is every macroblock's candidate
+      const uint8_t* lt = f.lt + (src - f.cur);
+      const int s = (int)__reduce_add_sync(FULL, __vsadu4(s0, *reinterpret_cast<const uint32_t*>(lt)) + __vsadu4(s1, *reinterpret_cast<const uint32_t*>(lt + 4)));
+      inter = min(inter, s <= ME_EARLY_SAD_PER_LAMBDA * lambda ? 0 : s + 2 * lambda);
+    }
+    if (lane == 0) { s_intra[warp] = (unsigned long long)(best + lambda * SCUT_INTRA_MB_BITS); s_inter[warp] = (unsigned long long)inter; }
+  } else if (lane == 0) { s_intra[warp] = 0; s_inter[warp] = 0; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long a = 0, b = 0;
+    for (int w = 0; w < SCUT_WARPS; w++) { a += s_intra[w]; b += s_inter[w]; }
+    atomicAdd(&f.scut->intra, a); atomicAdd(&f.scut->inter, b);
+    __threadfence();
+    if (atomicAdd(&f.scut->done, 1u) == gridDim.x - 1) {
+      __threadfence();
+      const unsigned long long intra = atomicExch(&f.scut->intra, 0ull), inter = atomicExch(&f.scut->inter, 0ull);
+      f.scut->cut[f.pic & 1] = SCUT_INTRA_WEIGHT * intra < SCUT_INTER_WEIGHT * inter;
+      f.scut->done = 0;
+    }
+  }
+}
+
+// k_scene_cut, then k_intra_rows on the IDR grid, which codes the picture when it was cut: two launches per P picture
+int launch_scene_cut(const FrameCtx& f, cudaStream_t st) {
+  k_scene_cut<<<(f.mbw * f.mbh + SCUT_WARPS - 1) / SCUT_WARPS, 32 * SCUT_WARPS, 0, st>>>(f);
+  FrameCtx g = f;
+  g.slice_rows = 1; g.slice_cols = f.cut_slice_cols; g.n_slices = f.cut_n_slices;
+  g.slice_words = f.cut_slice_words; g.chunks_per_slice = f.cut_chunks;
+  k_intra_rows<true><<<g.n_slices, 96, 0, st>>>(g);
+  return 2;
 }
 
 }  // namespace b2v

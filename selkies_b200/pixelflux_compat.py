@@ -79,6 +79,7 @@ class CaptureSettings:
         self.h264_droppable_frames = False       # every second P picture a non-reference picture a lagging consumer may drop (full frame only)
         self.h264_wide_motion = False            # motion vectors up to 128 px across and 256 px down/up for fast scrolls and drags (H.264 only)
         self.h264_long_term_ref = False          # keep one earlier picture as a long-term reference: popups and app switches come back cheaply (full frame only)
+        self.h264_scene_cut = False              # code a P picture whose content is all new as an intra picture (full frame only)
 
 
 class StripeCallback:
@@ -286,6 +287,10 @@ class ScreenCapture:
                 raise ValueError("h264_long_term_ref needs full-frame H.264 (output_mode 1, h264_fullframe True) without "
                                  "h264_droppable_frames: JPEG has no reference pictures, every H.264 stripe is a stream of its own, "
                                  "and a droppable picture cannot mark a long-term one")
+            s.scene_cut = bool(getattr(settings, "h264_scene_cut", False))
+            if s.scene_cut and (jpeg or not bool(getattr(settings, "h264_fullframe", True))):
+                raise ValueError("h264_scene_cut needs full-frame H.264 (output_mode 1, h264_fullframe True): JPEG has no P pictures "
+                                 "and every H.264 stripe is a stream of its own")
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)

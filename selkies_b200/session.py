@@ -15,7 +15,7 @@ from typing import Callable, NamedTuple, Optional
 import numpy as np
 
 from . import _native as N
-from .h264_nal import is_droppable
+from .h264_nal import is_droppable, is_intra
 
 
 class FrameQuality(NamedTuple):
@@ -33,10 +33,10 @@ class FrameQuality(NamedTuple):
 
 
 class EncodedFrame:
-    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height", "quality", "droppable")
+    __slots__ = ("data", "frame_id", "is_key", "qp", "pts90k", "capture_ns", "y_start", "height", "quality", "droppable", "intra")
 
     def __init__(self, data: bytes, frame_id: int, is_key: bool, qp: int, pts90k: int, capture_ns: int, y_start: int = 0, height: int = 0,
-                 quality: Optional[FrameQuality] = None, droppable: bool = False):
+                 quality: Optional[FrameQuality] = None, droppable: bool = False, intra: bool = False):
         self.data = data
         self.frame_id = frame_id
         self.is_key = is_key
@@ -46,6 +46,7 @@ class EncodedFrame:
         self.y_start, self.height = y_start, height
         self.quality = quality          # None unless the session measures quality (Session(quality=True))
         self.droppable = droppable      # a non-reference picture a consumer may drop (Session(droppable=True)); read from the data
+        self.intra = intra              # a P picture coded as a non-IDR intra picture (Session(scene_cut=True)); read from the data
 
 
 # pixel formats of device frames: name -> (B2V_PIX_* code, bytes per pixel); the name is the byte order in memory
@@ -184,7 +185,7 @@ def normalize_rects(rects, width: int, height: int, cap: int = N.B2V_MAX_DAMAGE_
 
 # the opt-in H.264 flags: Session keyword and attribute -> B2V_FLAG_* bit
 _OPT_IN_FLAGS = {"quality": N.B2V_FLAG_QUALITY, "droppable": N.B2V_FLAG_DROPPABLE, "wide_motion": N.B2V_FLAG_WIDE_MOTION,
-                 "long_term_ref": N.B2V_FLAG_LONG_TERM_REF}
+                 "long_term_ref": N.B2V_FLAG_LONG_TERM_REF, "scene_cut": N.B2V_FLAG_SCENE_CUT}
 
 
 class Session:
@@ -193,11 +194,11 @@ class Session:
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
                  collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False,
-                 long_term_ref: bool = False, damage: bool = False):
+                 long_term_ref: bool = False, scene_cut: bool = False, damage: bool = False):
         self._lib = N.lib()
         flags |= N.B2V_FLAG_DAMAGE if damage else 0
         self.damage = bool(flags & N.B2V_FLAG_DAMAGE)      # the damage submits (damage=[...]) need it
-        asked = dict(quality=quality, droppable=droppable, wide_motion=wide_motion, long_term_ref=long_term_ref)
+        asked = dict(quality=quality, droppable=droppable, wide_motion=wide_motion, long_term_ref=long_term_ref, scene_cut=scene_cut)
         for name, bit in _OPT_IN_FLAGS.items():      # the attribute reports the bit, whether the keyword or `flags` set it
             flags |= bit if asked[name] else 0
             setattr(self, name, bool(flags & bit))
@@ -230,7 +231,8 @@ class Session:
             f = fptr.contents
             data = C.string_at(f.data, f.size)
             rec = EncodedFrame(data, f.frame_id, bool(f.is_key), f.qp, f.pts90k, f.capture_ns, f.y_start, f.height,
-                               self.frame_quality(), self.droppable and is_droppable(data, self._hdr_len))
+                               self.frame_quality(), self.droppable and is_droppable(data, self._hdr_len),
+                               self.scene_cut and not f.is_key and is_intra(data, self._hdr_len))
             with self._lock:
                 self.frames.append(rec)
 
