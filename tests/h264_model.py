@@ -1,7 +1,7 @@
-"""A numpy model of the encoder's operations, written from ITU-T H.264 (8.3, 8.4.2.2, 8.5) and DESIGN.md §5.3 (wide-range motion
-included) / §5.4, in int64.
+"""A numpy model of the encoder's operations, written from ITU-T H.264 (8.3, 8.4.2.2, 8.5) and DESIGN.md §5.2 (the intra decision) /
+§5.3 (wide-range motion included) / §5.4 / §5.7, in int64.
 It shares no code with oracle/ or selkies_b200/.  Planes are 2-D uint8 arrays of the coded size (chroma: one array per
-component); coordinates are in samples of the plane."""
+component); coordinates are in samples of the plane.  The 4x4 operations also take a stack of blocks (..., 4, 4)."""
 from __future__ import annotations
 
 import numpy as np
@@ -63,7 +63,7 @@ def dead_zone(qbits, intra):
 
 
 def inverse4x4(d):
-    """8.5.12.2: rows, then columns, then (x + 32) >> 6."""
+    """8.5.12.2: rows, then columns, then (x + 32) >> 6 (of each 4x4 block of a stack)."""
     d = np.asarray(d, np.int64)
 
     def one(v):                                          # v[..., 0..3]
@@ -71,7 +71,7 @@ def inverse4x4(d):
         e2, e3 = (v[..., 1] >> 1) - v[..., 3], v[..., 1] + (v[..., 3] >> 1)
         return np.stack([e0 + e3, e1 + e2, e1 - e2, e0 - e3], axis=-1)
     f = one(d)                                           # each row
-    h = one(f.T).T                                       # each column
+    h = np.swapaxes(one(np.swapaxes(f, -1, -2)), -1, -2)  # each column
     return (h + 32) >> 6
 
 
@@ -81,7 +81,7 @@ def dequant4x4(c, qp, skip_dc=False):
     c = np.asarray(c, np.int64)
     d = (c * ls) << (qp // 6 - 4) if qp >= 24 else (c * ls + (1 << (3 - qp // 6))) >> (4 - qp // 6)
     if skip_dc:
-        d[0, 0] = 0
+        d[..., 0, 0] = 0
     return d
 
 
@@ -105,7 +105,7 @@ def quant_block(res, qp, intra, with_dc=True):
     qbits = 15 + qp // 6
     lv = quant(w, mf_of(qp), dead_zone(qbits, intra), qbits)
     if not with_dc:
-        lv[0, 0] = 0
+        lv[..., 0, 0] = 0
     return lv, w
 
 
@@ -150,8 +150,12 @@ def decimate_levels(luma_scan):
     return out
 
 
+_ZX, _ZY = (np.array(c) for c in zip(*ZIGZAG_XY))
+
+
 def raster_to_scan(r):
-    return np.array([r[y, x] for x, y in ZIGZAG_XY], np.int64)
+    """The 16 levels of a 4x4 raster block (or of each block of a stack) in zig-zag scan order."""
+    return np.asarray(r, np.int64)[..., _ZY, _ZX]
 
 
 # ------------------------------------------------------------------------------------------------ the I_PCM rule (§5.7)
@@ -239,8 +243,10 @@ class Avail:
 
 
 def intra4x4_pred(mode, P):
-    """8.3.1.2.1-9: P(x, y) for x, y in -1..7 gives p[x, y] (None when not available).  Returns 4x4 raster."""
-    out = np.zeros((4, 4), np.int64)
+    """8.3.1.2.1-9: P(x, y) for x, y in -1..7 gives p[x, y] (None when not available): one sample, or an array of one sample per
+    block of a stack.  Returns the 4x4 raster (the stack of them, (..., 4, 4)); ValueError when the mode reads a sample that is not
+    available."""
+    vals = []
     for y in range(4):
         for x in range(4):
             if mode == 0:
@@ -250,11 +256,12 @@ def intra4x4_pred(mode, P):
             elif mode == 2:
                 top = [P(i, -1) for i in range(4)]
                 left = [P(-1, i) for i in range(4)]
-                if None not in top and None not in left:
+                has_top, has_left = all(t is not None for t in top), all(t is not None for t in left)
+                if has_top and has_left:
                     v = (sum(top) + sum(left) + 4) >> 3
-                elif None not in left:
+                elif has_left:
                     v = (sum(left) + 2) >> 2
-                elif None not in top:
+                elif has_top:
                     v = (sum(top) + 2) >> 2
                 else:
                     v = 128
@@ -305,15 +312,16 @@ def intra4x4_pred(mode, P):
                     v = (P(-1, y + (x >> 1)) + 2 * P(-1, y + (x >> 1) + 1) + P(-1, y + (x >> 1) + 2) + 2) >> 2
             if v is None:
                 raise ValueError(f"Intra4x4 mode {mode} uses an unavailable sample")
-            out[y, x] = v
-    return out
+            vals.append(np.asarray(v, np.int64))
+    out = np.stack(vals).reshape(4, 4, *vals[0].shape)
+    return np.moveaxis(out, (0, 1), (-2, -1))
 
 
-def intra4x4_neighbours(rec, mbx, mby, blk, av: Avail):
-    """p[x, y] accessor for luma block blk of macroblock (mbx, mby) reading the picture `rec` being decoded, with the
-    availability rules of 6.4.11.4 and the top-right substitution of 8.3.1.2."""
+def intra4x4_accessor(get, blk, av: Avail):
+    """p[x, y] accessor for luma block blk of a macroblock with the availability rules of 6.4.11.4 and the top-right substitution
+    of 8.3.1.2; get(nx, ny) reads the sample at offset (nx, ny) from the macroblock's top-left corner of the picture being
+    decoded."""
     bx, by = BLK_XY[blk]
-    x0, y0 = mbx * 16 + bx * 4, mby * 16 + by * 4
 
     def avail(nx, ny):                                   # (nx, ny): sample offset relative to the macroblock
         if nx < 0 and ny < 0:
@@ -338,8 +346,14 @@ def intra4x4_neighbours(rec, mbx, mby, blk, av: Avail):
             x = 3
         if not avail(bx * 4 + x, by * 4 + y):
             return None
-        return int(rec[y0 + y, x0 + x])
+        return get(bx * 4 + x, by * 4 + y)
     return P
+
+
+def intra4x4_neighbours(rec, mbx, mby, blk, av: Avail):
+    """intra4x4_accessor for luma block blk of macroblock (mbx, mby) reading the picture `rec` being decoded."""
+    x0, y0 = mbx * 16, mby * 16
+    return intra4x4_accessor(lambda nx, ny: int(rec[y0 + ny, x0 + nx]), blk, av)
 
 
 def intra16_pred(mode, top, left, tl):
@@ -764,3 +778,222 @@ def marking_ops(long_term_exists):
     """§5.13: the operations of a marking picture — MMCO 1 on the picture two back only while there is no long-term picture (the
     sliding window holds two short-term frames then), MMCO 4 (one long-term index), MMCO 3 (the previous picture to index 0)."""
     return ([] if long_term_exists else [(1, 1)]) + [(4, 1), (3, 0, 0)]
+
+
+# ------------------------------------------------------------------------------------------------ the intra decision (§5.2, §5.7)
+I4_SKIP_SAD_PER_LAMBDA = 32      # §5.2: Intra4x4 is tried only when the best Intra16x16 SAD exceeds 32·λ
+MB_BITS_LIMIT = 3200             # A.3.1 / §5.7: a macroblock sized above this is sent as I_PCM
+
+
+def rd_lambda(qp):
+    """§5.2: the Lagrangian of the Intra4x4 / Intra16x16 choice, round(0.85·2^((qp − 12)/3)), at least 1."""
+    return max(1, int(np.floor(0.85 * 2.0 ** ((qp - 12) / 3) + 0.5)))
+
+
+def _blocks(x):
+    """(..., 16, 16) -> (..., 16 blkIdx, 4, 4): the 4x4 luma blocks of a macroblock in decoding order."""
+    x = np.asarray(x, np.int64)
+    b = x.reshape(*x.shape[:-2], 4, 4, 4, 4).swapaxes(-3, -2)           # [..., by, bx, r, c]
+    return np.stack([b[..., by, bx, :, :] for bx, by in BLK_XY], axis=-3)
+
+
+def _unblocks(b):
+    """_blocks' inverse."""
+    out = np.zeros((*b.shape[:-3], 4, 4, 4, 4), np.int64)
+    for blk, (bx, by) in enumerate(BLK_XY):
+        out[..., by, bx, :, :] = b[..., blk, :, :]
+    return out.swapaxes(-3, -2).reshape(*b.shape[:-3], 16, 16)
+
+
+def _chroma_blocks(x):
+    """(..., 8, 8) -> (..., 4, 4, 4): the 4x4 blocks of one chroma component, raster order (= chroma4x4BlkIdx)."""
+    x = np.asarray(x, np.int64)
+    return x.reshape(*x.shape[:-2], 2, 4, 2, 4).swapaxes(-3, -2).reshape(*x.shape[:-2], 4, 4, 4)
+
+
+def _chroma_unblocks(b):
+    return b.reshape(*b.shape[:-3], 2, 2, 4, 4).swapaxes(-3, -2).reshape(*b.shape[:-3], 8, 8)
+
+
+def chroma_code(src, pred, qpc, intra):
+    """§5.4 for one chroma component of a stack of macroblocks ((N, 8, 8) source and prediction): (DC levels (N, 4), AC levels
+    (N, 4, 16) in scan order, position 0 unused, the reconstruction (N, 8, 8))."""
+    pb = _chroma_blocks(pred)
+    lv, w = quant_block(_chroma_blocks(src) - pb, qpc, intra, with_dc=False)
+    n = lv.shape[0]
+    dc = chroma_dc_levels(w[..., 0, 0].reshape(n, 2, 2), qpc, intra)
+    d = dequant4x4(lv, qpc)
+    d[..., 0, 0] = chroma_dc_dequant(dc, qpc).reshape(n, 4)
+    return dc.reshape(n, 4), raster_to_scan(lv), _chroma_unblocks(clip1(pb + inverse4x4(d)))
+
+
+def chroma_bits(dcs, acs):
+    """§5.7: the chroma bits of one macroblock from its two components' DC (4) and AC (4, 16) levels, and its coded_block_pattern
+    chroma part: 2 when an AC level is non-zero, 1 when only a DC level is."""
+    cc = 2 if any(np.any(a[:, 1:]) for a in acs) else 1 if any(np.any(d) for d in dcs) else 0
+    bits = sum(cavlc_bits(d, chroma_dc=True) for d in dcs) if cc else 0
+    if cc == 2:
+        bits += sum(cavlc_bits(a[b][1:]) for a in acs for b in range(4))
+    return bits, cc
+
+
+class IntraDecision:
+    """intra_decide's result for a stack of N macroblocks (arrays of N): kind ("I_16x16", "I_NxN" or "I_PCM"); i16_mode and
+    chroma_mode; i4_modes (N, 16) by blkIdx, those of the Intra4x4 pass; tried, the gate let Intra4x4 be tried; j16, j4 (the model
+    runs the Intra4x4 pass everywhere, so that j4 < j16 where it was not tried shows what the gate decided); size, the §5.7 size of the kind the comparison kept; i16_tie / chroma_tie, the two modes' SADs were
+    equal; rec, the reconstruction (Y (N, 16, 16), Cb, Cr (N, 8, 8)); right, what the next macroblock takes as its left neighbour."""
+
+
+def intra_decide(src_y, src_u, src_v, left, qp):
+    """§5.2: the intra decision of N macroblocks that have no neighbour above (src_y (N, 16, 16), src_u / src_v (N, 8, 8)).  left:
+    None at a slice start, else (y (N, 16), cb (N, 8), cr (N, 8), modes (N, 4)): the left neighbour's reconstructed right column and
+    the Intra4x4PredMode of its right-column blocks (2 where it is not I_NxN).
+      - Intra16x16: argmin of SAD·4 + mode over horizontal (1, with a left neighbour) and DC (2).
+      - chroma: argmin of (SAD Cb + SAD Cr)·4 + mode over DC (0) and horizontal (1, with a left neighbour).
+      - Intra4x4 is tried when the best Intra16x16 SAD exceeds 32·λ: per block in decoding order the key
+        (SAD + λ·(mode == predIntra4x4PredMode ? 1 : 4))·16 + mode over the modes whose samples are available, the block reconstructed
+        before the next is predicted.
+      - J = SSD(source, reconstruction) + rd_lambda(qp)·bits over the luma: Intra16x16 8 + the DC block + the 15-coefficient blocks
+        when any AC level is non-zero, Intra4x4 8 + the blocks of its cbp + its mode bits (1 or 4 per block), blocks by cavlc_bits;
+        Intra4x4 wins when its J is strictly smaller.
+      - §5.7: I_PCM when header_budget (48, 96 for I_NxN) + luma bits + chroma bits > 3200."""
+    sy, su, sv = (np.asarray(a, np.int64) for a in (src_y, src_u, src_v))
+    n, idx = sy.shape[0], np.arange(sy.shape[0])
+    lam, rdl, qpc = LAMBDA[qp], rd_lambda(qp), QPC[qp]
+    has_left = left is not None
+    ly, lu, lv_, lmodes = (np.asarray(a, np.int64) for a in left) if has_left else (None,) * 4
+    out = IntraDecision()
+    # ---- Intra16x16 mode
+    m16 = ([1] if has_left else []) + [2]
+    p16 = np.stack([np.stack([intra16_pred(m, None, None if ly is None else ly[i], None) for i in range(n)]) for m in m16])
+    sad16 = np.abs(sy - p16).sum(axis=(2, 3))
+    k = (sad16 * 4 + np.array(m16)[:, None]).argmin(0)
+    out.i16_mode, pred16 = np.array(m16)[k], p16[k, idx]
+    best16 = sad16[k, idx]
+    out.i16_tie = sad16[0] == sad16[1] if has_left else np.zeros(n, bool)
+    # ---- chroma mode
+    mc = [0] + ([1] if has_left else [])
+    pc = np.stack([np.stack([np.stack([chroma_pred(m, None, None if l_ is None else l_[i], None) for i in range(n)])
+                             for l_ in ((lu, lv_) if has_left else (None, None))]) for m in mc])       # (modes, 2, N, 8, 8)
+    sadc = (np.abs(np.stack([su, sv]) - pc).sum(axis=(3, 4))).sum(axis=1)
+    kc = (sadc * 4 + np.array(mc)[:, None]).argmin(0)
+    out.chroma_mode = np.array(mc)[kc]
+    out.chroma_tie = sadc[0] == sadc[1] if has_left else np.zeros(n, bool)
+    cbits = np.zeros(n, np.int64)
+    coded_c = [chroma_code(s_, pc[kc, c, idx], qpc, True) for c, s_ in enumerate((su, sv))]
+    for i in range(n):
+        cbits[i] = chroma_bits([coded_c[0][0][i], coded_c[1][0][i]], [coded_c[0][1][i], coded_c[1][1][i]])[0]
+    crec = [coded_c[0][2], coded_c[1][2]]
+    # ---- Intra16x16 coding
+    pb = _blocks(pred16)
+    lv, w = quant_block(_blocks(sy) - pb, qp, True, with_dc=False)
+    w_dc = np.zeros((n, 4, 4), np.int64)
+    for blk, (bx, by) in enumerate(BLK_XY):
+        w_dc[:, by, bx] = w[:, blk, 0, 0]
+    dc = i16_dc_levels(w_dc, qp)
+    dcy = luma_dc_dequant(dc, qp)
+    d = dequant4x4(lv, qp)
+    for blk, (bx, by) in enumerate(BLK_XY):
+        d[:, blk, 0, 0] = dcy[:, by, bx]
+    rec16 = _unblocks(clip1(pb + inverse4x4(d)))
+    ac, dcs = raster_to_scan(lv), raster_to_scan(dc)
+    bits16 = np.array([cavlc_bits(dcs[i]) + (sum(cavlc_bits(ac[i, b, 1:]) for b in range(16)) if np.any(ac[i]) else 0)
+                       for i in range(n)])
+    out.j16 = ((sy - rec16) ** 2).sum(axis=(1, 2)) + rdl * (8 + bits16)
+    # ---- Intra4x4: the gate, and the pass (on every macroblock)
+    out.tried = best16 > I4_SKIP_SAD_PER_LAMBDA * lam
+    rt = np.zeros((n, 17, 17), np.int64)            # rt[:, 1 + y, 1 + x]: sample (x, y) of the macroblock; column 0 the left one
+    if has_left:
+        rt[:, 1:, 0] = ly
+    av = Avail(has_left, False, False, False)
+    levels, modes, mode_bits = np.zeros((n, 16, 16), np.int64), np.zeros((n, 16), np.int64), np.zeros(n, np.int64)
+    for blk, (bx, by) in enumerate(BLK_XY):
+        P = intra4x4_accessor(lambda nx, ny: rt[:, 1 + ny, 1 + nx], blk, av)
+        cands, preds = [], []
+        for mode in range(9):
+            try:
+                preds.append(np.broadcast_to(intra4x4_pred(mode, P), (n, 4, 4)))
+                cands.append(mode)
+            except (ValueError, TypeError):          # the mode reads a sample that is not available
+                pass
+        if by == 0 or (bx == 0 and not has_left):    # 8.3.1.1: block A or B not available
+            pm = np.full(n, 2)
+        else:
+            ma = modes[:, BLK_IDX[(bx - 1, by)]] if bx > 0 else lmodes[:, by]
+            pm = np.minimum(ma, modes[:, BLK_IDX[(bx, by - 1)]])
+        src = sy[:, 4 * by:4 * by + 4, 4 * bx:4 * bx + 4]
+        keys = np.stack([(np.abs(src - p).sum(axis=(1, 2)) + lam * np.where(pm == m, 1, 4)) * 16 + m for m, p in zip(cands, preds)])
+        kk = keys.argmin(0)
+        mode, pred = np.array(cands)[kk], np.stack(preds)[kk, idx]
+        l4, _ = quant_block(src - pred, qp, True)
+        levels[:, blk], modes[:, blk] = raster_to_scan(l4), mode
+        mode_bits += np.where(mode == pm, 1, 4)
+        rt[:, 1 + 4 * by:5 + 4 * by, 1 + 4 * bx:5 + 4 * bx] = clip1(pred + inverse4x4(dequant4x4(l4, qp)))
+    bits4 = np.array([sum(cavlc_bits(levels[i, b]) for b in range(16) if np.any(levels[i, b & ~3:(b & ~3) + 4])) for i in range(n)])
+    rec4 = rt[:, 1:, 1:]
+    out.i4_modes = modes
+    out.j4 = ((sy - rec4) ** 2).sum(axis=(1, 2)) + rdl * (8 + bits4 + mode_bits)
+    use4 = out.tried & (out.j4 < out.j16)
+    out.size = np.where(use4, 2 * HEADER_BITS + bits4, HEADER_BITS + bits16) + cbits
+    pcm = out.size > MB_BITS_LIMIT
+    out.kind = np.where(pcm, "I_PCM", np.where(use4, "I_NxN", "I_16x16"))
+    ry = np.where(pcm[:, None, None], sy, np.where(use4[:, None, None], rec4, rec16))
+    ru, rv = (np.where(pcm[:, None, None], s_, r_) for s_, r_ in zip((su, sv), crec))
+    out.rec = (ry, ru, rv)
+    right_modes = np.full((n, 4), 2, np.int64)
+    nxn = out.kind == "I_NxN"
+    right_modes[nxn] = out.i4_modes[nxn][:, [BLK_IDX[(3, by)] for by in range(4)]]
+    out.right = (ry[:, :, 15], ru[:, :, 7], rv[:, :, 7], right_modes)
+    return out
+
+
+def intra_picture(src, slice_of, mbw, mbh, qp):
+    """§5.2 over a whole intra picture whose slices (slice_of[addr]: the slice of each macroblock) never span rows: the macroblocks
+    of all slices at the same position in their slice are decided together, each from the model's own reconstruction of its left
+    neighbour.  src: (Y, Cb, Cr) planes.  Returns ({addr: (IntraDecision, its index in the stack)}, at_slice_start {addr}, the
+    reconstruction (Y, Cb, Cr))."""
+    sy, su, sv = (np.asarray(p, np.int64) for p in src)
+    chains = {}
+    for a in range(mbw * mbh):
+        if a % mbw and slice_of[a - 1] == slice_of[a]:
+            chains[a] = chains.pop(a - 1) + [a]
+        else:
+            chains[a] = [a]
+    chains = list(chains.values())
+    rec = [np.zeros_like(sy), np.zeros_like(su), np.zeros_like(sv)]
+    out, left = {}, None
+    for j in range(max(len(c) for c in chains)):
+        live = [c for c in chains if len(c) > j]
+        addrs = [c[j] for c in live]
+        ys = np.stack([sy[16 * (a // mbw):16 * (a // mbw) + 16, 16 * (a % mbw):16 * (a % mbw) + 16] for a in addrs])
+        us, vs = (np.stack([p[8 * (a // mbw):8 * (a // mbw) + 8, 8 * (a % mbw):8 * (a % mbw) + 8] for a in addrs]) for p in (su, sv))
+        if j:
+            keep = [i for i, c in enumerate(prev_live) if len(c) > j]
+            left = tuple(x[keep] for x in left)
+        r = intra_decide(ys, us, vs, left, qp)
+        for i, a in enumerate(addrs):
+            out[a] = (r, i)
+            y0, x0 = 16 * (a // mbw), 16 * (a % mbw)
+            rec[0][y0:y0 + 16, x0:x0 + 16] = r.rec[0][i]
+            for c in (1, 2):
+                rec[c][y0 // 2:y0 // 2 + 8, x0 // 2:x0 // 2 + 8] = r.rec[c][i]
+        left, prev_live = r.right, live
+    return out, rec
+
+
+def p_mb_size(src, ref, x0, y0, mv, qp, wide=False):
+    """§5.7 / §5.4: the size of the P macroblock at (x0, y0) predicted from the reference planes `ref` (Y, Cb, Cr) at the quarter-
+    sample vector mv: its luma levels (dead zone of inter blocks, decimated) and chroma levels quantised by the model, the blocks its
+    cbp codes by cavlc_bits, plus 48 (and WM_MVD_BITS with wide motion).  Above 3200 the macroblock is I_PCM."""
+    sy, su, sv = (np.asarray(p, np.int64) for p in src)
+    pred = luma_inter(ref[0], x0, y0, mv)
+    lv, _ = quant_block(_blocks(sy - pred), qp, False)
+    scan = decimate_levels(raster_to_scan(lv))
+    bits = HEADER_BITS + (WM_MVD_BITS if wide else 0)
+    bits += sum(cavlc_bits(scan[b]) for b in range(16) if np.any(scan[b & ~3:(b & ~3) + 4]))
+    qpc, coded = QPC[qp], []
+    for c, s_ in ((1, su), (2, sv)):
+        pc = chroma_inter(ref[c], x0 // 2, y0 // 2, mv)
+        dc, ac, _ = chroma_code(s_[None], pc[None], qpc, False)
+        coded.append((dc[0], ac[0]))
+    return bits + chroma_bits([d for d, _ in coded], [a for _, a in coded])[0]

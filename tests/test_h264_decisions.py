@@ -1,7 +1,8 @@
 """The encoder's decisions, macroblock by macroblock, against a second statement of DESIGN.md §5 that shares no code with either
 encoder: tests/h264_syntax_refs.py (on tests/h264_syntax.py) parses the bytes and follows the decoded picture buffer,
-tests/h264_model.py restates prediction, quantisation, decimation, motion cost, the lean pass's exits, the search after it (anchor
-predictor, reduced and exhaustive search, second window, quarter-sample refinement) and the long-term marking rule.
+tests/h264_model.py restates prediction, quantisation, decimation, the intra decision of §5.2, the size rule of §5.7, motion cost, the
+lean pass's exits, the search after it (anchor predictor, reduced and exhaustive search, second window, quarter-sample refinement)
+and the long-term marking rule.
 Byte parity with the oracle and libavcodec's decode pin conformance; these checks pin what is coded.
 
 Per stream (one per band in striped mode) and picture:
@@ -10,9 +11,13 @@ Per stream (one per band in striped mode) and picture:
     macroblocks), blocks absent from cbp and P_Skip macroblocks included, each inter macroblock predicted from the model's
     reconstruction of the picture its refIdx names;
   - A.3.1: every non-PCM macroblock_layer() is at most 3200 bits, its header within the budget of §5.7, every I_PCM sample equals
-    the source;
+    the source, every I_PCM macroblock sized above 3200 bits by the model (intra: M.intra_decide; P: M.p_mb_size at M.decide's
+    vector);
+  - intra pictures (IDR pictures and scene cuts, §5.2): every macroblock's kind, Intra16x16, chroma and Intra4x4 modes are
+    M.intra_decide's, from the model's own reconstruction of its left neighbour;
   - no refIdx-0 P_L0_16x16 macroblock has cbp 0 and its P_Skip vector;
-  - motion (§5.3, §5.12, §5.13): every P macroblock not sent as I_PCM carries exactly the refIdx and vector M.decide gives it;
+  - motion (§5.3, §5.12, §5.13): every macroblock of a P picture (a scene cut is none) not sent as I_PCM carries exactly the refIdx
+    and vector M.decide gives it;
   - the long-term reference (§5.13): the marks, their operations, the override and the picture the DPB names follow the model's
     rule on the model's own changed(k);
   - the SPS: profile, constraint flags, level against Table A-1, reference frames, cropping and the VUI of §5.1.
@@ -33,6 +38,7 @@ from tests import layered_scenario as LS
 from tests import ltr_content as LC
 from tests import ltr_scenario as LTS
 from tests import scenario as S
+from tests import scut_scenario as SC
 from tests import synth
 from tests import wide_content as WC
 from tests import wide_scenario as WS
@@ -89,8 +95,10 @@ def source_nv12(frame, cw, ch):
 
 
 def oracle_side(cfg: S.Config) -> S.OracleSide:
-    """The oracle side for cfg.flags: the long-term reference (wide motion or not), wide-range motion (droppable or not), droppable
-    pictures, or none of them."""
+    """The oracle side for cfg.flags: scene cuts (with the long-term reference or not), the long-term reference (wide motion or not),
+    wide-range motion (droppable or not), droppable pictures, or none of them."""
+    if cfg.flags & SC.FLAG_SCENE_CUT:
+        return SC.ScutOracleSide(cfg)
     if cfg.flags & LTS.FLAG_LONG_TERM_REF:
         return LTS.LtrOracleSide(cfg)
     if cfg.flags & WS.FLAG_WIDE_MOTION:
@@ -138,10 +146,26 @@ class Stats:
         self.scaled = 0                   # predictor-class macroblocks of pictures whose reference distances differ, previous vector fractional
         self.pcm_two_refs = 0             # I_PCM macroblocks in pictures with two references
         self.paths = {}                   # how M.decide found vectors ("refined search", "anchor predictor", ...) -> count
+        # the intra decision (§5.2) and the I_PCM rule (§5.7), from the model where the stream carries what it decides
+        self.i4_row0, self.i4_rows = set(), set()     # Intra4x4 modes of I_NxN macroblocks in block row 0 / rows 1..3
+        self.i16_modes, self.chroma_modes = set(), set()
+        self.i4_untried = 0               # intra macroblocks whose Intra16x16 SAD kept the gate of 32·λ shut
+        self.gate_decides = 0             # ... where Intra4x4 would have won the comparison
+        self.compared = {}                # kind kept where Intra4x4 was tried ("I_NxN" / "I_16x16") -> count
+        self.ties = {}                    # SAD ties the mode index resolved: "I16 H over DC", "chroma DC over H" -> count
+        self.slice_starts = 0             # intra macroblocks that start a slice inside a row (no left neighbour)
+        self.min_dj = None                # the smallest |J4 − J16| where Intra4x4 was tried
+        self.max_coded = {"I": 0, "P": 0}           # the largest §5.7 size of a coded macroblock, intra / inter
+        self.min_pcm = {"I": None, "P": None}       # the smallest model size of an I_PCM macroblock, in intra / P pictures
+        self.cut_pictures = 0             # non-IDR pictures of I slices (scene cuts)
+        self.cut_pcm = 0                  # I_PCM macroblocks in them
 
     def count(self, kind, d=None):
         d = self.kinds if d is None else d
         d[kind] = d.get(kind, 0) + 1
+
+    def pcm_size(self, pic_type, size):
+        self.min_pcm[pic_type] = size if self.min_pcm[pic_type] is None else min(self.min_pcm[pic_type], size)
 
 
 def check_sps(sps, width, height, y_start, band_h, mbw, mbh_band, stats, flags=0):
@@ -200,6 +224,8 @@ def check_picture(pic, recs, src, where, stats, wide=False):
             assert m.bits <= est, f"{at}: {m.bits} bits coded, more than the {est} of the size rule"     # the rule only overstates
             assert est <= MAX_MB_BITS, f"{at}: sized {est} bits by the rule of §5.7 (wide {wide}), coded instead of I_PCM"
             stats.max_bits = max(stats.max_bits, m.bits)
+            t = "I" if m.intra else "P"
+            stats.max_coded[t] = max(stats.max_coded[t], est)
         if m.kind == "P_L0_16x16" and m.ref_idx == 0:
             assert not (m.cbp == 0 and m.mv == m.skip_mv), f"{at}: cbp 0 and the P_Skip vector {m.mv}, coded as P_L0_16x16"
         qp, intra = m.qp, m.intra
@@ -275,17 +301,70 @@ def check_picture(pic, recs, src, where, stats, wide=False):
     return rec
 
 
-def check_exits(pic, prev, recs, src_y, where, stats, wide=False, dec=None):
-    """Every macroblock of P picture `pic` against the model's decision (M.decide) from the source luma `src_y`, the model's
+def is_intra_picture(pic):
+    """An IDR picture or a scene cut (§5.14): every slice an I slice."""
+    return all(h["slice_type"] == 2 for h in pic.headers)
+
+
+def check_intra(pic, src, rec, where, stats):
+    """§5.2 on intra picture `pic` (an IDR picture or a scene cut): its slices never span rows, and every macroblock carries the kind
+    and the modes M.intra_picture decides from the source `src` (Y, U, V) on the model's own reconstruction, which must equal `rec`,
+    the reconstruction check_picture made from the parsed syntax.  A coded macroblock's model size is its size by the rule of §5.7;
+    an I_PCM one's exceeds 3200 bits."""
+    mbw, mbh = pic.sps.mbw, pic.sps.mbh
+    slice_of = [m.slice for m in pic.mbs]
+    for m in pic.mbs:
+        assert m.qp == pic.qp, f"{where}: mb {m.addr} at QP {m.qp} in a picture of QP {pic.qp}"
+        assert m.addr < mbw or slice_of[m.addr - mbw] != m.slice, f"{where}: the slice of mb {m.addr} spans rows"
+    decided, mrec = M.intra_picture(src, slice_of, mbw, mbh, pic.qp)
+    for m in pic.mbs:
+        r, i = decided[m.addr]
+        mbx, mby = m.addr % mbw, m.addr // mbw
+        at = f"{where} mb ({mbx},{mby}) {m.kind} qp {m.qp}"
+        why = f"model: {r.kind[i]}, size {r.size[i]}, Intra4x4 tried {r.tried[i]}, J16 {r.j16[i]}, J4 {r.j4[i]}"
+        assert m.kind == r.kind[i], f"{at}: {why}"
+        if m.kind == "I_PCM":
+            assert r.size[i] > M.MB_BITS_LIMIT
+            stats.pcm_size("I", int(r.size[i]))
+            stats.cut_pcm += not pic.idr
+        else:
+            assert r.size[i] == M.mb_size_estimate(m), f"{at}: size {M.mb_size_estimate(m)} by the parsed levels, {why}"
+            assert m.chroma_mode == r.chroma_mode[i], f"{at}: chroma mode {m.chroma_mode}, the model's {r.chroma_mode[i]}"
+            stats.chroma_modes.add(m.chroma_mode)
+            if r.chroma_tie[i]:
+                stats.count("chroma DC over H", stats.ties)
+            if m.kind == "I_16x16":
+                assert m.i16_mode == r.i16_mode[i], f"{at}: Intra16x16 mode {m.i16_mode}, the model's {r.i16_mode[i]} ({why})"
+                stats.i16_modes.add(m.i16_mode)
+                if r.i16_tie[i]:
+                    stats.count("I16 H over DC", stats.ties)
+            else:
+                assert list(m.i4_modes) == list(r.i4_modes[i]), f"{at}: Intra4x4 modes {m.i4_modes}, the model's {r.i4_modes[i].tolist()}"
+                for blk, mode in enumerate(m.i4_modes):
+                    (stats.i4_rows if BLK_XY[blk][1] else stats.i4_row0).add(mode)
+            if r.tried[i]:
+                stats.count(m.kind, stats.compared)
+                dj = abs(int(r.j4[i]) - int(r.j16[i]))
+                stats.min_dj = dj if stats.min_dj is None else min(stats.min_dj, dj)
+        stats.i4_untried += not r.tried[i]
+        stats.gate_decides += not r.tried[i] and m.kind != "I_PCM" and r.j4[i] < r.j16[i]
+        stats.slice_starts += mbx > 0 and slice_of[m.addr - 1] != m.slice
+    for c in range(3):
+        assert np.array_equal(mrec[c], rec[c]), f"{where}: the model's reconstruction of plane {c} != the parsed one"
+
+
+def check_exits(pic, prev, recs, src, where, stats, wide=False, dec=None):
+    """Every macroblock of P picture `pic` against the model's decision (M.decide) from the source `src` (Y, U, V), the model's
     reconstructions of refIdx 0 and of the long-term picture (refIdx 1, while the picture has two references), the previous
     picture's parsed records `prev` (the picture just before in decoding order, reference or not) and, with wide motion, dec: the
     decimated luma of this picture's source and of its reference's.  Anchors are decided first, then the rest with their anchor's
-    decision.  Every macroblock not sent as I_PCM must carry exactly the model's refIdx and vector (P_Skip: its inferred vector)."""
+    decision.  Every macroblock not sent as I_PCM must carry exactly the model's refIdx and vector (P_Skip: its inferred vector); every
+    I_PCM one must be sized above 3200 bits by the model at that vector (M.p_mb_size)."""
     mbw, mbh = pic.sps.mbw, pic.sps.mbh
     ref = recs[pic.ref_list[0]][0]
     lt = recs[pic.ref_list[1]][0] if len(pic.ref_list) > 1 else None
     dist = (pic.index - pic.ref_list[0], prev.index - prev.ref_list[0] if prev.ref_list else 1)
-    y = src_y.astype(np.int64)
+    y = src[0].astype(np.int64)
     anchor = {m.addr: M.anchor_of(m.addr % mbw, m.addr // mbw, mbw, 0, mbh) for m in pic.mbs}
     decided = {}
     for m in sorted(pic.mbs, key=lambda m: anchor[m.addr] != (m.addr % mbw, m.addr // mbw)):       # anchors first
@@ -300,7 +379,12 @@ def check_exits(pic, prev, recs, src_y, where, stats, wide=False, dec=None):
         d = M.decide(blk, ref, lt, pm, x0, y0, pic.qp, wide, dist, None if is_anchor else decided[anchor[m.addr]], coarse)
         decided[(mbx, mby)] = d
         ex = d.ex
-        if m.kind != "I_PCM":
+        if m.kind == "I_PCM":
+            size = M.p_mb_size([p[k * y0 // 16:k * (y0 + 16) // 16, k * x0 // 16:k * (x0 + 16) // 16] for p, k in zip(src, (16, 8, 8))],
+                               recs[pic.ref_list[d.ref_idx]], x0, y0, d.mv, pic.qp, wide)
+            assert size > M.MB_BITS_LIMIT, f"{where} mb ({mbx},{mby}): I_PCM, sized {size} bits at refIdx {d.ref_idx} mv {d.mv}"
+            stats.pcm_size("P", size)
+        else:
             assert (m.ref_idx, m.mv) == (d.ref_idx, d.mv), \
                 f"{where} mb ({mbx},{mby}): the model decides refIdx {d.ref_idx} mv {d.mv} ({d.path}, class {ex.cls}, k {ex.k}, " \
                 f"refined {d.refined}, second window {d.second}) but coded {m.kind} refIdx {m.ref_idx} mv {m.mv}"
@@ -355,11 +439,14 @@ class LtrModel:
             return
         changed = M.changed_count(src_y, recs[pic.index - 1][0], pic.qp)
         mark = M.marks(changed, self.prev_changed, self.mbs)
+        cut = is_intra_picture(pic)      # a scene cut keeps its P picture's marking; its I slices carry no override
         for h in pic.headers:
             assert h.get("mmco") == (M.marking_ops(self.lt is not None) if mark else None), \
                 f"{where}: operations {h.get('mmco')}, the rule says mark {mark} (changed {changed}, before {self.prev_changed})"
-            assert h.get("num_ref_idx_active", 1) == (2 if self.lt is not None else 1), f"{where}: override {h.get('num_ref_idx_active')}"
-        assert pic.ref_list == ([pic.index - 1] + ([self.lt] if self.lt is not None else [])), (where, pic.ref_list, self.lt)
+            if not cut:
+                assert h.get("num_ref_idx_active", 1) == (2 if self.lt is not None else 1), f"{where}: override {h.get('num_ref_idx_active')}"
+        if not cut:
+            assert pic.ref_list == ([pic.index - 1] + ([self.lt] if self.lt is not None else [])), (where, pic.ref_list, self.lt)
         if self.lt is not None:
             stats.lt_age = max(stats.lt_age, pic.index - self.lt)
         if mark:
@@ -392,17 +479,21 @@ def check_encoded(e: Encoded, stripe_rows=0):
             src = [p[y_start // k_: y_start // k_ + band_mbh * 16 // k_] for p, k_ in zip(e.sources[index], (1, 2, 2))]
             pic.ref_frame_nums = [pics[i].frame_num for i in pic.ref_list]
             rec = check_picture(pic, recs, src, where, stats, e.wide)
+            intra = is_intra_picture(pic)
+            if intra:
+                check_intra(pic, src, rec, where, stats)
+                stats.cut_pictures += not pic.idr
             vh, vw = pic.sps.height, pic.sps.width
             for c, (r, d) in enumerate(zip(rec, dec)):
                 s = 1 if c == 0 else 2
                 assert np.array_equal(r[: vh // s, : vw // s], d), f"{where}: model reconstruction of plane {c} != libavcodec's decode"
             # the exits need the previous picture's records: a band left unsent (all skipped) in between hides them
-            if not pic.idr and k > 0 and items[k - 1][0] == index - 1:
+            if not intra and k > 0 and items[k - 1][0] == index - 1:
                 dec = None
                 if e.wide:     # the coarse search's planes: the decimated sources of this picture and of its reference
                     ref_src = e.sources[items[pic.ref_list[0]][0]][0][y_start:y_start + band_mbh * 16]
                     dec = M.decimate(src[0]), M.decimate(ref_src)
-                check_exits(pic, pics[k - 1], recs, src[0], where, stats, e.wide, dec)
+                check_exits(pic, pics[k - 1], recs, src, where, stats, e.wide, dec)
             if ltr is not None:
                 ltr.picture(pic, recs, src[0], stats, y_start)
             recs.append(rec)
@@ -462,7 +553,7 @@ def cases():
     out.append(("predictor_paths", S.Config(130, 70, qp=30), synth.predictor_paths(130, 70), (0,), None, 0))
     still = synth.desktop(96, 64, 0)
     out.append(("paintover_burst", S.Config(96, 64, qp=40, paint=(2, 20, 3)), [still] * 8, (0,), None, 0))
-    return out + wide_cases() + ltr_cases() + motion_cases()
+    return out + wide_cases() + ltr_cases() + motion_cases() + intra_cases()
 
 
 WIDE = WS.FLAG_WIDE_MOTION
@@ -628,6 +719,84 @@ def motion_cases():
              None, 5)]
 
 
+def directional(w, h, seed=1, tile=16):
+    """BGRA picture of tile x tile squares, each an oriented pattern in two random colours: stripes of period 3..12 px, a step or a
+    ramp, at one of eight orientations (multiples of 22.5°) through a point near the tile's centre."""
+    rng = np.random.default_rng(seed)
+    f = np.zeros((h, w, 4), np.uint8)
+    f[..., 3] = 255
+    for ty in range(0, h, tile):
+        for tx in range(0, w, tile):
+            yy, xx = np.mgrid[0:min(tile, h - ty), 0:min(tile, w - tx)].astype(np.float64)
+            th = rng.integers(8) * np.pi / 8
+            u = (xx - tile / 2 + rng.uniform(-2, 2)) * np.cos(th) + (yy - tile / 2 + rng.uniform(-2, 2)) * np.sin(th)
+            kind = rng.integers(3)
+            if kind == 0:
+                v = 0.5 + 0.5 * np.cos(2 * np.pi * u / rng.uniform(3, 12))
+            elif kind == 1:
+                v = (u > 0).astype(np.float64)
+            else:
+                v = (u - u.min()) / max(np.ptp(u), 1)
+            c0, c1 = rng.integers(0, 256, 3), rng.integers(0, 256, 3)
+            f[ty:ty + tile, tx:tx + tile, :3] = np.rint(c0 + (c1 - c0) * v[..., None]).astype(np.uint8)
+    return f
+
+
+def flat(w, h):
+    """BGRA picture of flat areas: mid grey on the left, a flat colour on the right, a dark grey band across the bottom."""
+    f = np.full((h, w, 4), 255, np.uint8)
+    f[:, :w // 2, :3] = 128
+    f[:, w // 2:, :3] = (40, 160, 220)
+    f[h - 16:, :, :3] = 60
+    return f
+
+
+def dots(w, h):
+    """BGRA mid-grey picture with one 2x2 dot per macroblock, its amplitude rising by 1 from 1 in raster order: Intra16x16 SADs of
+    4 per level step, either side of the Intra4x4 gate at small λ."""
+    luma = np.full((h, w), 120, np.int64)
+    for a in range((h // 16) * (w // 16)):
+        y, x = 16 * (a // (w // 16)) + 5, 16 * (a % (w // 16)) + 9
+        luma[y:y + 2, x:x + 2] += a + 1
+    return grey(w, h, grey_table(), luma)
+
+
+def noise_ramp(w, h, amp, seed=0, base=None):
+    """BGRA grey picture: `base` (a luma plane; mid grey when None) plus uniform noise whose amplitude rises linearly from amp[0] at
+    the left edge to amp[1] at the right edge."""
+    rng = np.random.default_rng(seed)
+    a = np.linspace(amp[0], amp[1], w)[None, :]
+    luma = (np.full((h, w), 126, np.int64) if base is None else base) + np.rint(a * rng.uniform(-1, 1, (h, w))).astype(np.int64)
+    return grey(w, h, grey_table(), np.clip(luma, 16, 235)), luma
+
+
+def pcm_boundary_frames(w, h):
+    """An IDR picture and a P picture whose macroblocks reach the I_PCM limit of §5.7 in a ramp across the picture (coded at QP 4
+    and 0): noise of amplitude 50..110, then the same with fresh noise of amplitude 30..90 added."""
+    f0, luma = noise_ramp(w, h, (50, 110), seed=1)
+    f1, _ = noise_ramp(w, h, (30, 90), seed=2, base=np.clip(luma, 16, 235))
+    return [f0, f1]
+
+
+def intra_cases():
+    """The intra decision (§5.2) and the I_PCM rule (§5.7) in both directions: each reaches what assert_targets names for it."""
+    cut = SC.FLAG_SCENE_CUT
+    d64 = directional(64, 48, 3)
+    return [("intra_directional_qp26", S.Config(160, 96, qp=26), [directional(160, 96, 1)], (0,), None, 0),
+            ("intra_directional_qp40", S.Config(160, 96, qp=40), [directional(160, 96, 1)], (0,), None, 0),
+            ("intra_flat", S.Config(96, 64, qp=26), [flat(96, 64)], (0,), None, 0),
+            ("intra_gate_dots", S.Config(128, 80, qp=10), [dots(128, 80)], (0,), None, 0),
+            ("intra_slices3_crop", S.Config(136, 72, qp=30, idr_slice_mbs=3), [directional(136, 72, 2)] * 2, (0,), None, 0),
+            ("intra_qp0", S.Config(64, 48, qp=0), [d64], (0,), None, 0),
+            ("intra_qp10", S.Config(64, 48, qp=10), [d64], (0,), None, 0),
+            ("intra_qp51", S.Config(64, 48, qp=51), [d64], (0,), None, 0),
+            ("pcm_boundary", S.Config(320, 64, qp=0), pcm_boundary_frames(320, 64), (0,), [4, 0], 0),
+            ("scut_switches_qp26", S.Config(160, 96, qp=26, flags=cut), SC.switches(160, 96), (0,), None, 0),
+            ("scut_switches_ltr_qp36", S.Config(160, 96, qp=36, flags=cut | LTR), SC.switches(160, 96), (0,), None, 0),
+            ("scut_noise_qp0_4", S.Config(64, 48, qp=0, flags=cut),
+             [synth.desktop(64, 48)] * 2 + [synth.noise(64, 48, s) for s in (5, 6)], (0,), [0, 0, 2, 4], 0)]
+
+
 def assert_targets(name, st):
     """What each case is there for, from the parsed streams and the model: a case that drifts away from its target fails."""
     ex = st.exits
@@ -659,6 +828,29 @@ def assert_targets(name, st):
             "noise_window_scroll": ["reduced search at |dy| = 2", "refined with SAD >= 4096"]}
     for path in want.get(name, []):
         assert st.paths.get(path, 0) > 0, (path, st.paths)
+    # the intra decision: every mode and branch of §5.2 where a mistake in it changes what is coded
+    intra = (st.i4_row0, st.i4_rows, st.i16_modes, st.chroma_modes, st.i4_untried, st.compared, st.ties, st.slice_starts)
+    if name.startswith("intra_directional"):
+        assert st.i4_rows == set(range(9)) and st.i4_row0 == {1, 2, 8}, intra
+        assert st.i16_modes == {1, 2} and st.chroma_modes == {0, 1}, intra
+        assert st.compared.get("I_NxN", 0) > 0 and st.compared.get("I_16x16", 0) > 0, intra
+    if name == "intra_flat":
+        assert st.i4_untried > 0 and st.ties.get("I16 H over DC", 0) > 0 and st.ties.get("chroma DC over H", 0) > 0, intra
+    if name == "intra_gate_dots":                    # the gate shuts Intra4x4 out where it would have won
+        assert st.gate_decides > 0 and st.compared.get("I_NxN", 0) > 0, intra
+    if name == "intra_slices3_crop":
+        assert st.slice_starts >= 10, intra          # 9 macroblocks a row in slices of 3: two slice starts inside each of 5 rows
+    if name in ("intra_qp0", "intra_qp10"):          # rd_lambda 1, λ 1: both kinds kept after a comparison
+        assert st.compared.get("I_NxN", 0) > 0 and st.compared.get("I_16x16", 0) > 0, intra
+    if name == "intra_qp51":                           # rd_lambda 6963, λ 57: the comparison made, Intra16x16 kept
+        assert st.compared.get("I_16x16", 0) > 0, intra
+    if name == "pcm_boundary":     # coded and I_PCM macroblocks within 100 bits of the limit, on either side of it, intra and inter
+        for t in "IP":
+            assert 3100 <= st.max_coded[t] and st.min_pcm[t] is not None and st.min_pcm[t] <= 3300, (t, st.max_coded, st.min_pcm, st.kinds)
+    if name.startswith("scut_"):
+        assert st.cut_pictures > 0, st.kinds
+    if name == "scut_noise_qp0_4":
+        assert st.cut_pcm > 0, st.kinds
 
 
 CASES = cases()

@@ -60,3 +60,13 @@ def test_tables_match_libavcodec(path):
         assert blob.count(bytes(inv)) >= 1
     assert sorted(t["zigzag4x4"]) == list(range(16))
     assert blob.count(bytes(t["chroma_qp_tab"])) >= 1
+
+
+@pytest.mark.parametrize("path", ["oracle/h264_tables_ref.h", "selkies_b200/csrc/h264_tables.cuh"])
+def test_lambda_tables_follow_the_model(path):
+    """The encoders' λ tables are the ones tests/h264_model.py states: the motion λ table, and rd_lambda of the intra decision
+    (DESIGN.md §5.2), round(0.85·2^((qp − 12)/3)) and at least 1, which the model derives from the formula."""
+    from tests import h264_model as M
+    t = parse_tables(os.path.join(ROOT, path))
+    assert t["me_lambda"] == M.LAMBDA
+    assert t["rd_lambda"] == [M.rd_lambda(qp) for qp in range(52)]
