@@ -158,7 +158,7 @@ enum {
                                    exactly those of a whole-frame submit of the same picture.  The ring then copies into one
                                    persistent device frame (the mirror, src_w x src_h x 4 bytes) instead of one device buffer per
                                    ring slot: at 4K that is 33 MB of HBM instead of ring_slots x 33 MB. */
-  B2V_FLAG_SCENE_CUT     = 2048 /* scene cuts: a P picture whose content is all new (an application switch, a slide change, a cut in a
+  B2V_FLAG_SCENE_CUT     = 2048,/* scene cuts: a P picture whose content is all new (an application switch, a slide change, a cut in a
                                    video) is coded as an intra picture instead of predicted from a picture it no longer resembles.
                                    The GPU decides per P picture, after the P analysis, which runs unchanged:
                                      cost_inter = the sum over macroblocks of the luma cost of the prediction the analysis chose:
@@ -187,6 +187,33 @@ enum {
                                    rejects a size at which stripe_rows would stripe.  It costs two kernel launches per P picture
                                    (kernel_launches: k_scene_cut, and k_intra_rows, which returns at once unless the picture was
                                    cut), flagged variants of the analysis and entropy kernels, and 4 bytes per macroblock. */
+  B2V_FLAG_SIZE_CAP      = 4096 /* picture size cap: a P picture larger than b2v_set_max_picture_bytes is coded once more at a
+                                   coarser QP, decided on the GPU with no host round trip.  In a low-latency stream the size of a
+                                   picture is the time it holds the link; this bounds the spikes the CBR controller (which feeds
+                                   back two pictures late and repays a spike afterwards) lets through.
+                                     size: the sum of the picture's macroblock-layer bits (mb_type to the last residual block of
+                                           every coded macroblock; an I_PCM macroblock's mb_type and 384 samples), rounded up to
+                                           bytes.  Slice headers, mb_skip_run, I_PCM alignment bits (at most 7 per macroblock),
+                                           parameter sets, start codes and emulation-prevention bytes are not counted.
+                                     rule:  when size > cap, the picture is coded again once at QP' = QP + d, d the smallest value in
+                                           1..51-QP with bits <= (8 x cap x T[d]) >> 16, T[d] = round(65536 x 2^(d/6)) (integers
+                                           only); 51 when none qualifies.  A picture at QP 51 is not recoded.
+                                   There is one recode and no second pass: the cap is a target, and a recoded picture can still
+                                   exceed it (the rule assumes bits halve every 6 QP steps).  A recode keeps the analysis's vectors,
+                                   reference indices and exits; every macroblock gets the same motion-compensated prediction and a
+                                   new residual at QP' (transform, quantisation, reconstruction, levels); P_Skip and the I_PCM
+                                   fallback are decided again on the new levels, in both directions.  Every slice's slice_qp_delta
+                                   carries QP', b2v_frame.qp reports it, and the CBR controller and the paint-over scheduler see
+                                   the picture as finally coded.  Only P pictures are capped (the macroblocks coded from the
+                                   long-term picture included); IDR pictures and scene-cut intra pictures are not.  In striped mode
+                                   the cap applies to the whole access unit, all bands together (the QP is the picture's).
+                                   With cap 0 (the default) the flag changes no output byte.  Works with CQP and CBR, paint-over,
+                                   scaling, cropping, striped mode and every other coding flag.  H.264 only: b2v_create rejects it
+                                   (B2V_EINVAL) with B2V_FLAG_JPEG or B2V_FLAG_NO_ENCODE.  It costs three kernel launches per P
+                                   picture (kernel_launches: k_size_cap, k_requant and a second CAVLC pass, which return at once
+                                   unless the picture is recoded), 388 bytes per macroblock, and the overlap of a picture's entropy
+                                   coding with the next picture's analysis: a recode rewrites the reconstruction the next picture
+                                   predicts from, so entropy coding runs on the analysis stream. */
 };
 
 /* B2V_FLAG_DAMAGE: one changed region of the source, in source pixels of the frame (or the device window) the submit names.
@@ -360,6 +387,9 @@ int  b2v_set_gop(void* h, int32_t frames);               /* b2v_settings.gop, li
                                                             SECONDS, settings.py:163, with the current fps) */
 int  b2v_set_resolution(void* h, int32_t src_w, int32_t src_h, int32_t dst_w, int32_t dst_h);
 int  b2v_request_idr(void* h);
+int  b2v_set_max_picture_bytes(void* h, int32_t bytes);  /* B2V_FLAG_SIZE_CAP: the cap of every P picture from the next submit on
+                                                            (0 = none, the default).  B2V_ESTATE without the flag, B2V_EINVAL
+                                                            for a negative value. */
 
 /* ---- quality of the record being delivered (B2V_FLAG_QUALITY) --------------
  * Valid only inside this session's frame callback, on its output thread: fills *out with the measurement of the record the

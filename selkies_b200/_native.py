@@ -22,6 +22,7 @@ B2V_FLAG_DROPPABLE = 128
 B2V_FLAG_WIDE_MOTION = 256
 B2V_FLAG_LONG_TERM_REF = 512
 B2V_FLAG_SCENE_CUT = 2048
+B2V_FLAG_SIZE_CAP = 4096
 B2V_FLAG_DAMAGE = 1024
 B2V_MAX_DAMAGE_RECTS = 64
 B2V_PIX_BGRA, B2V_PIX_RGBA, B2V_PIX_BGR, B2V_PIX_RGB = 0, 1, 2, 3
@@ -109,6 +110,7 @@ SYMBOLS = [
     ("b2v_set_bitrate_kbps", C.c_int, [C.c_void_p, C.c_int32]),
     ("b2v_set_qp", C.c_int, [C.c_void_p, C.c_int32]),
     ("b2v_set_gop", C.c_int, [C.c_void_p, C.c_int32]),
+    ("b2v_set_max_picture_bytes", C.c_int, [C.c_void_p, C.c_int32]),
     ("b2v_set_resolution", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("b2v_request_idr", C.c_int, [C.c_void_p]),
     ("b2v_frame_quality", C.c_int, [C.c_void_p, C.POINTER(B2VQuality)]),

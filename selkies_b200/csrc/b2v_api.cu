@@ -151,6 +151,7 @@ struct Session {
   double fps = 60.0;
   int bitrate_kbps = 8000;
   int qp_fixed = 26;
+  int max_picture_bytes = 0;     // B2V_FLAG_SIZE_CAP
 
   // timing events (B2V_FLAG_TIMING): 6 per output slot, read back by the output thread
   cudaEvent_t ev_t[kMaxSlots][6] = {};
@@ -190,6 +191,7 @@ constexpr CodingFlagRule kCodingFlags[] = {
   {B2V_FLAG_LONG_TERM_REF, "B2V_FLAG_LONG_TERM_REF", "keeps an H.264 reference picture", true, B2V_FLAG_DROPPABLE,
    "a non-reference picture cannot mark a long-term picture, and its reference is two pictures back"},
   {B2V_FLAG_SCENE_CUT, "B2V_FLAG_SCENE_CUT", "codes H.264 P pictures as intra pictures", true, 0, nullptr},
+  {B2V_FLAG_SIZE_CAP, "B2V_FLAG_SIZE_CAP", "recodes H.264 P pictures", false, 0, nullptr},
 };
 
 // `flags` against the table for a picture of dst_h rows: 0, or B2V_EINVAL naming the flag.  No CUDA call.
@@ -526,6 +528,7 @@ int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStrea
     fp.idr = idr;
     fp.rc_mode = s->cfg.rc_mode;
     fp.qp_fixed = s->qp_fixed;
+    fp.max_picture_bytes = s->max_picture_bytes;
     fp.paint_trigger = s->cfg.paintover_trigger_frames > 0 ? s->cfg.paintover_trigger_frames : 0;
     fp.paint_qp = s->cfg.paintover_crf;
     fp.paint_burst = s->cfg.paintover_burst_frames > 0 ? s->cfg.paintover_burst_frames : 1;
@@ -569,7 +572,8 @@ int submit_common(Session* s, const CscSource& src, int in_slot, const cudaStrea
     nl += jpeg_encode(s->jenc, s->d_cur, s->d_au[out_idx], j.is_key, s->st_enc);
   } else if (s->encode) {
     fp.cur = s->d_cur; fp.au = s->d_au[out_idx]; fp.ev = s->timing_csc_only ? nullptr : ev; fp.csc_ts = cp.ts;
-    fp.st_pack = fp.ev ? nullptr : s->st_pack;      // per-stage events need the serial schedule
+    // per-stage events need the serial schedule; so does B2V_FLAG_SIZE_CAP (h264_encoder.cu encoder_encode)
+    fp.st_pack = fp.ev || (s->cfg.flags & B2V_FLAG_SIZE_CAP) ? nullptr : s->st_pack;
     nl += encoder_encode(s->enc, &fp, s->st_enc);
     if (fp.st_pack) st_done = fp.st_pack;
   }
@@ -1024,6 +1028,15 @@ int b2v_set_gop(void* h, int32_t frames) {
   if (!s) return fail(B2V_EINVAL, "null handle");
   std::lock_guard<std::mutex> lk(s->mu);
   s->cfg.gop = frames;
+  return 0;
+}
+int b2v_set_max_picture_bytes(void* h, int32_t bytes) {
+  Session* s = (Session*)h;
+  if (!s) return fail(B2V_EINVAL, "null handle");
+  if (!(s->cfg.flags & B2V_FLAG_SIZE_CAP)) return fail(B2V_ESTATE, "the session was created without B2V_FLAG_SIZE_CAP");
+  if (bytes < 0) return fail(B2V_EINVAL, "max_picture_bytes must be >= 0");
+  std::lock_guard<std::mutex> lk(s->mu);
+  s->max_picture_bytes = bytes;
   return 0;
 }
 int b2v_request_idr(void* h) {

@@ -59,6 +59,21 @@ struct ScutState {
 // macroblock's cost_intra carries lambda x SCUT_INTRA_MB_BITS
 constexpr int SCUT_INTRA_WEIGHT = 1, SCUT_INTER_WEIGHT = 1, SCUT_INTRA_MB_BITS = 16;
 
+// B2V_FLAG_SIZE_CAP (DESIGN.md §5.15; oracle/h264_cap_ref.c).  k_size_cap of P picture k writes qp[k & 1], the QP the picture is
+// finally coded at, and recode[k & 1], set when that is a coarser QP' than the analysis used; k_requant, the second CAVLC pass and
+// the slice build of picture k read them.  Double-buffered by parity like ScutState::cut.
+struct CapState {
+  int32_t qp[2];
+  int32_t recode[2];
+};
+// the rule (include/b2video.h): T[d] = round(65536 x 2^(d / 6)); a picture of `bits` over the cap is recoded at QP + d for the
+// smallest d in 1..51-QP with bits <= (cap_bits x T[d]) >> 16, or at 51
+__device__ const int32_t cap_t[52] = {
+  65536, 73562, 82570, 92682, 104032, 116772, 131072, 147123, 165140, 185364, 208064, 233544, 262144, 294247, 330281, 370728,
+  416128, 467088, 524288, 588493, 660561, 741455, 832255, 934175, 1048576, 1176987, 1321123, 1482910, 1664511, 1868350, 2097152,
+  2353974, 2642246, 2965821, 3329021, 3736700, 4194304, 4707947, 5284492, 5931642, 6658043, 7473400, 8388608, 9415894, 10568984,
+  11863283, 13316085, 14946800, 16777216, 18831788, 21137968, 23726566};
+
 // Feedback record of the rate controller / paint-over scheduler.  fb[k & 1] is written after picture k (rc_step, last block of
 // its slice scan); picture k is CODED from fb[k & 1] as it stood before that — the state after picture k-2 — because the entropy
 // coding of picture k-1, where its size becomes known, overlaps the analysis of picture k on another stream.  The two records
@@ -147,6 +162,11 @@ struct FrameCtx {          // everything a kernel needs about the picture being 
   ScutState* scut;
   int32_t* scut_cost;      // [mbs] the luma cost of the prediction the analysis chose (finish_mb of the flagged analysis kernels)
   int cut_slice_cols, cut_n_slices, cut_slice_words, cut_chunks;   // the IDR grid, in which a cut picture is coded
+  // B2V_FLAG_SIZE_CAP (h264_cap.cu): null without the flag and in IDR pictures
+  CapState* cap;
+  uint8_t* cap_pred;       // [mbs][384] the prediction the analysis chose: 16 x 16 luma, then 8 rows of 16 interleaved chroma bytes
+  uint32_t* cap_mv;        // [mbs] its vector word (finish_mb: LTR_MV_WORD for refIdx 1)
+  int cap_bytes;           // this picture's cap (0 = none)
 };
 
 // B2V_FLAG_SCENE_CUT: a P picture that k_scene_cut cut is coded as a non-IDR intra picture in the IDR grid.  The flagged variants of

@@ -44,6 +44,10 @@ struct Encoder {
   // B2V_FLAG_SCENE_CUT: k_scene_cut's sums and decisions, and the analysis's cost of every macroblock
   ScutState* scut = nullptr;
   int32_t* scut_cost = nullptr;
+  // B2V_FLAG_SIZE_CAP: k_size_cap's decisions, and the analysis's prediction and vector word of every macroblock
+  CapState* cap = nullptr;
+  uint8_t* cap_pred = nullptr;
+  uint32_t* cap_mv = nullptr;
   // side data the analysis kernels write and the entropy kernels read: double-buffered by picture parity, so the entropy coding
   // of picture k (packing stream) overlaps the analysis of picture k+1 (main stream)
   MbInfo* mbinfo[2] = {nullptr, nullptr};
@@ -219,6 +223,12 @@ int encoder_create(const EncoderConfig* cfg_in, Encoder** out) {
     ECK(cudaMalloc((void**)&e->scut_cost, mbs * sizeof(int32_t)));
     ECK(cudaMemset(e->scut_cost, 0, mbs * sizeof(int32_t)));
   }
+  if (cfg->flags & B2V_FLAG_SIZE_CAP) {
+    ECK(cudaMalloc((void**)&e->cap, sizeof(CapState)));
+    ECK(cudaMemset(e->cap, 0, sizeof(CapState)));
+    ECK(cudaMalloc((void**)&e->cap_pred, mbs * 384));
+    ECK(cudaMalloc((void**)&e->cap_mv, mbs * sizeof(uint32_t)));
+  }
   for (int b = 0; b < 2; b++) {
     ECK(cudaMalloc((void**)&e->mbinfo[b], mbs * sizeof(MbInfo)));
     ECK(cudaMemset(e->mbinfo[b], 0, mbs * sizeof(MbInfo)));
@@ -297,7 +307,8 @@ void encoder_destroy(Encoder* e) {
   void* ptrs[] = {e->recon[0], e->recon[1], e->recon[2], e->mbinfo[0], e->mbinfo[1], e->coef[0], e->coef[1], e->nnz[0], e->nnz[1], e->mb_words, e->mb_nbits, e->slice_buf,
                   e->slice_size, e->slice_rbsp, e->slice_bits, e->overflow, e->rc, e->param_sets, e->i4modes[0],
                   e->i4modes[1], e->band_fn, e->band_coded, e->me_pub, e->me_queue, e->chunk_agg, e->chunk_inc, e->slice_done,
-                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse, e->lt, e->ltr, e->scut, e->scut_cost};
+                  e->q_acc, e->q_done, e->dec[0], e->dec[1], e->dec[2], e->coarse, e->lt, e->ltr, e->scut, e->scut_cost,
+                  e->cap, e->cap_pred, e->cap_mv};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (e->ev_analysed[b]) cudaEventDestroy(e->ev_analysed[b]);
@@ -346,6 +357,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
     const SliceGrid& gi = e->idr_grid;
     f.cut_slice_cols = gi.cols; f.cut_n_slices = gi.n; f.cut_slice_words = gi.words; f.cut_chunks = gi.chunks;
   }
+  if ((e->cfg.flags & B2V_FLAG_SIZE_CAP) && !idr) { f.cap = e->cap; f.cap_pred = e->cap_pred; f.cap_mv = e->cap_mv; f.cap_bytes = p->max_picture_bytes; }
   int n = 0;
   // Two-stream schedule (no per-stage events requested): ANALYSIS of picture k on `st` (CSC before it, by the caller), ENTROPY
   // coding of picture k (CAVLC, slice build with the rate-control step, pack) on `st_pack`, overlapping
@@ -376,13 +388,20 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
   // k_intra_rows of picture k on `st` and by its entropy stage after ev_analysed, and rewritten by k_scene_cut of picture k+2, whose
   // analysis waits for the pack of picture k.  A cut picture's k_intra_rows overwrites this picture's reconstruction and side data,
   // which only this picture's entropy stage and the next picture's analysis read, both behind it.
-  const bool overlap = p->st_pack != nullptr && p->ev == nullptr;
+  // B2V_FLAG_SIZE_CAP: the entropy stage of every picture runs on `st`, whatever `st_pack` is (the caller, b2v_api.cu submit_common,
+  // passes none, since the access unit is complete on `st`).  A recode (k_requant) rewrites the reconstruction, levels and records of picture k after its first CAVLC pass, and picture
+  // k+1's analysis reads that reconstruction: it has to wait for the whole entropy stage of picture k, not only for its analysis.
+  // The P-picture sequence runs behind k_ltr_mark, whose decision the CAVLC passes read (two references), and before k_quality,
+  // which measures the reconstruction as finally coded; k_requant reads the prediction the analysis stored, never the long-term
+  // picture k_ltr_mark may have replaced.
+  const bool overlap = p->st_pack != nullptr && p->ev == nullptr && !(e->cfg.flags & B2V_FLAG_SIZE_CAP);
   if (overlap) cudaStreamWaitEvent(st, e->ev_packed[par], 0);           // pack of picture k-2 (no-op before the first two)
   if (f.wide) n += launch_coarse(f, st);      // every picture: its decimated plane; P pictures: the coarse vectors
   if (f.ltr && !idr) cudaMemsetAsync(&e->ltr->changed[par], 0, sizeof(int32_t), st);
   n += idr ? launch_intra(f, st) : launch_inter(f, st);
   if (f.scut) n += launch_scene_cut(f, st);
   if (f.ltr && !idr) n += launch_ltr_mark(f, st);
+  if (f.cap) n += launch_size_cap(f, st);
   if (e->quality_off) {
     QualityParams q{};
     q.src = p->cur; q.recon = f.recon;
@@ -398,7 +417,7 @@ int encoder_encode(Encoder* e, const EncodeFrameParams* p, cudaStream_t st) {
     cudaEventRecord(e->ev_analysed[par], st);
     cudaStreamWaitEvent(sp, e->ev_analysed[par], 0);
   }
-  n += launch_cavlc(f, sp);
+  if (!f.cap) n += launch_cavlc(f, sp);
   if (p->ev) cudaEventRecord(p->ev[3], st);
   n += launch_slice_build(f, sp);
   if (p->ev) cudaEventRecord(p->ev[4], st);

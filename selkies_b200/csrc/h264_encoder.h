@@ -22,6 +22,7 @@ struct EncoderConfig {
                            //   B2V_FLAG_DROPPABLE: every P picture at an odd count from the IDR is a non-reference picture
                            //   B2V_FLAG_WIDE_MOTION: coarse vectors per anchor group (k_coarse) and windows centred on far candidates
                            //   B2V_FLAG_LONG_TERM_REF: one long-term reference picture, marked on the GPU (k_ltr_mark)
+                           //   B2V_FLAG_SIZE_CAP: P pictures over max_picture_bytes coded again at a coarser QP (k_size_cap)
 };
 
 struct EncodeFrameParams {
@@ -33,7 +34,8 @@ struct EncodeFrameParams {
   int paint_trigger, paint_qp, paint_burst;   // paint-over: `paint_burst` pictures at paint_qp after `paint_trigger` all-skipped pictures (0 = off)
   int64_t target_bits;     // per frame, CBR
   cudaEvent_t* ev;         // null, or 6 timing events: encoder records ev[2..5] after each stage (forces the serial schedule)
-  cudaStream_t st_pack;    // null = everything on `st`; else the entropy coding of this picture (k_cavlc_mb ... k_pack_au) runs here,
+  int max_picture_bytes;   // B2V_FLAG_SIZE_CAP: this picture's cap (0 = none)
+  cudaStream_t st_pack;    // null = everything on `st` (always with B2V_FLAG_SIZE_CAP); else the entropy coding of this picture (k_cavlc_mb ... k_pack_au) runs here,
                            // overlapping the analysis of the next picture on `st`.  The access unit is complete on st_pack.
   const unsigned long long* csc_ts;   // null, or the CSC launch's device stamps to forward in the AuHeader
 };

@@ -98,7 +98,7 @@ constexpr int CAVLC_WARPS = 4;
 
 // CUT (B2V_FLAG_SCENE_CUT, P pictures): the picture may have been cut (apply_scene_cut)
 template <bool CUT>
-__global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx fp) {
+__device__ __forceinline__ void cavlc_mb(const FrameCtx& fp) {
   FrameCtx f = fp;
   if (CUT) apply_scene_cut(f);
   __shared__ __align__(16) uint32_t s_words[CAVLC_WARPS][MB_WORDS];
@@ -197,6 +197,14 @@ __global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx fp) {
   uint32_t* dst = f.mb_words + (size_t)mb * MB_WORDS;
   for (int i = lane; i < (nb + 31) >> 5; i += 32) dst[i] = words[i];
   if (lane == 0) f.mb_nbits[mb] = (uint32_t)nb;
+}
+template <bool CUT>
+__global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_mb(FrameCtx fp) { cavlc_mb<CUT>(fp); }
+// B2V_FLAG_SIZE_CAP, P pictures: the same pass over the records k_requant rewrote, when k_size_cap recoded the picture.  A recoded
+// picture was not cut (k_size_cap), so the P-picture context is the one to code in.
+__global__ void __launch_bounds__(32 * CAVLC_WARPS) k_cavlc_recode(FrameCtx fp) {
+  if (!*reinterpret_cast<const volatile int32_t*>(&fp.cap->recode[fp.pic & 1])) return;
+  cavlc_mb<false>(fp);
 }
 
 // ------------------------------------------------------------------------------------------------ slice header (7.3.3)
@@ -322,10 +330,10 @@ __device__ __forceinline__ bool wait_flag(const volatile int* flag, int tag) {
   return true;
 }
 
-template <bool CUT>
-__global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx fp) {
-  FrameCtx f = fp;
-  if (CUT) apply_scene_cut(f);      // a cut picture has fewer blocks than the grid: the rest only count for the rate-control step
+// CAP (B2V_FLAG_SIZE_CAP, P pictures): the QP is the one k_size_cap recorded, which every slice header carries and the rate-control
+// step is told
+template <bool CUT, bool CAP>
+__device__ __forceinline__ void slice_build(const FrameCtx& f) {
   __shared__ long long s_warp_sum[SLICE_THREADS / 32];
   __shared__ int s_warp_max[SLICE_THREADS / 32];
   __shared__ uint32_t s_nb[SLICE_THREADS];       // nbits | I_PCM flag (bit 30), 0xffffffff = skipped
@@ -339,7 +347,7 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx fp) {
   const int band = geo.row0 / f.band_rows, first_mb = geo.mb0 - band * f.band_rows * f.mbw;
   const int fn = f.idr ? 0 : f.striped ? f.band_fn[band] : f.frame_num;
   const int n_chunks = (geo.n_mb + SLICE_THREADS - 1) / SLICE_THREADS;
-  const int tag = f.pic + 1, qp = frame_qp(f);
+  const int tag = f.pic + 1, qp = CAP ? *reinterpret_cast<const volatile int32_t*>(&f.cap->qp[f.pic & 1]) : frame_qp(f);
   uint32_t* out = f.slice_buf + (size_t)s * f.slice_words;
   bool active = k < n_chunks && (!CUT || s < f.n_slices);
   const int idx0 = k * SLICE_THREADS, n = active ? min(SLICE_THREADS, geo.n_mb - idx0) : 0, mb_first = geo.mb0 + idx0;
@@ -556,6 +564,18 @@ __global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx fp) {
     }
   }
 }
+template <bool CUT>
+__global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build(FrameCtx fp) {
+  FrameCtx f = fp;
+  if (CUT) apply_scene_cut(f);      // a cut picture has fewer blocks than the grid: the rest only count for the rate-control step
+  slice_build<CUT, false>(f);
+}
+template <bool CUT>
+__global__ void __launch_bounds__(SLICE_THREADS, 8) k_slice_build_cap(FrameCtx fp) {
+  FrameCtx f = fp;
+  if (CUT) apply_scene_cut(f);
+  slice_build<CUT, true>(f);
+}
 
 // ------------------------------------------------------------------------------------------------ k_pack_au
 constexpr int PACK_THREADS = ESC_THREADS;
@@ -626,9 +646,19 @@ int launch_cavlc(const FrameCtx& f, cudaStream_t st) {
   else k_cavlc_mb<false><<<(mbs + CAVLC_WARPS - 1) / CAVLC_WARPS, 32 * CAVLC_WARPS, 0, st>>>(f);
   return 1;
 }
+int launch_cavlc_recode(const FrameCtx& f, cudaStream_t st) {
+  const int mbs = f.mbw * f.mbh;
+  k_cavlc_recode<<<(mbs + CAVLC_WARPS - 1) / CAVLC_WARPS, 32 * CAVLC_WARPS, 0, st>>>(f);
+  return 1;
+}
+// B2V_FLAG_SIZE_CAP, P pictures: the variants that take the QP from k_size_cap, on the same grids
 int launch_slice_build(const FrameCtx& f, cudaStream_t st) {
-  if (f.scut && !f.idr)
-    k_slice_build<true><<<max(f.n_slices * f.chunks_per_slice, f.cut_n_slices * f.cut_chunks), SLICE_THREADS, 0, st>>>(f);
+  const bool cap = f.cap && !f.idr;
+  if (f.scut && !f.idr) {
+    const int blocks = max(f.n_slices * f.chunks_per_slice, f.cut_n_slices * f.cut_chunks);
+    if (cap) k_slice_build_cap<true><<<blocks, SLICE_THREADS, 0, st>>>(f);
+    else k_slice_build<true><<<blocks, SLICE_THREADS, 0, st>>>(f);
+  } else if (cap) k_slice_build_cap<false><<<f.n_slices * f.chunks_per_slice, SLICE_THREADS, 0, st>>>(f);
   else k_slice_build<false><<<f.n_slices * f.chunks_per_slice, SLICE_THREADS, 0, st>>>(f);      // scan + copy + emulation-prevention count
   return 1;
 }

@@ -304,15 +304,20 @@ __device__ __forceinline__ void publish_anchor(const FrameCtx& f, int mb, int sa
 // 48 + WM_MVD_BITS.
 constexpr int LTR_MV = -32768;
 constexpr uint32_t LTR_MV_WORD = 0x80008000u;
-// COST (B2V_FLAG_SCENE_CUT): the macroblock's cost_inter into f.scut_cost, the value the exits and the search compare: the luma SAD of
-// the prediction plus lambda x (bits of the vector's components, + ME_FRAC_PENALTY_BITS for a fractional vector); the zero vector's
-// for refIdx 1.  0 when the SAD is within the zero-motion exit's threshold: the residual is quantisation noise, there is nothing to
-// code.  Whichever path chose the prediction, t.pred_y holds it here.
-template <bool WIDE, bool COST>
+template <bool WIDE>
+__device__ __forceinline__ void code_p_mb(const FrameCtx& f, MbTile& t, int lane, int mb, int qp, uint32_t mv, bool ltr, size_t ysz);
+// SIDE: what the picture-level decisions after the analysis need of the macroblock.
+//  * SIDE_COST (B2V_FLAG_SCENE_CUT): its cost_inter into f.scut_cost, the value the exits and the search compare: the luma SAD of the prediction plus
+//    lambda x (bits of the vector's components, + ME_FRAC_PENALTY_BITS for a fractional vector); the zero vector's for refIdx 1.
+//    0 when the SAD is within the zero-motion exit's threshold: the residual is quantisation noise, there is nothing to code.
+//  * SIDE_CAP (B2V_FLAG_SIZE_CAP): its prediction and vector word into f.cap_pred and f.cap_mv, from which k_requant codes it again at a coarser QP.
+// Whichever path chose the prediction, t.pred_y holds it here.
+constexpr int SIDE_COST = 1, SIDE_CAP = 2;      // SIDE: f.scut is set, f.cap is set
+template <bool WIDE, int SIDE>
 __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane, const MbPos& p, int qp, int ylo, int yhi, int mvx, int mvy, uint32_t uv_coloc, bool ltr = false) {
   const bool ref1 = ltr && mvx == LTR_MV;
   const size_t ysz = (size_t)f.cw * f.ch;
-  if (COST) {      // first, while little is live (t.pred_y was written by other lanes: __syncwarp)
+  if (SIDE & SIDE_COST) {      // first, while little is live (t.pred_y was written by other lanes: __syncwarp)
     __syncwarp();
     const int r8 = lane >> 1, c8 = (lane & 1) * 8;
     const uint2 c = *reinterpret_cast<const uint2*>(&t.cur_y[r8][c8]), pr = *reinterpret_cast<const uint2*>(&t.pred_y[r8][c8]);
@@ -360,6 +365,19 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
   // the vector as MbInfo's first word and the macroblock index are all that stays live across the transform: anything more
   // spills inside it at k_inter_lean's 64 registers.  So ref_idx 1 travels as a vector no macroblock can have, LTR_MV_WORD.
   const uint32_t mv = ref1 ? LTR_MV_WORD : (uint32_t)(mvx & 0xffff) | ((uint32_t)mvy << 16);
+  if (SIDE & SIDE_CAP) {
+    uint8_t* d = f.cap_pred + (size_t)mb * 384;
+    *reinterpret_cast<uint2*>(d + (lane >> 1) * 16 + (lane & 1) * 8) = *reinterpret_cast<const uint2*>(&t.pred_y[lane >> 1][(lane & 1) * 8]);
+    reinterpret_cast<uint32_t*>(d + 256)[lane] = reinterpret_cast<const uint32_t*>(&t.pred_uv[0][0])[lane];
+    if (lane == 0) f.cap_mv[mb] = mv;
+  }
+  code_p_mb<WIDE>(f, t, lane, mb, qp, mv, ltr, ysz);
+}
+
+// The residual of P macroblock mb, whose source and prediction are in the tile, at `qp`; the I_PCM fallback; its reconstruction and
+// record.  mv: finish_mb's vector word.  finish_mb, and k_requant at a picture's QP'.
+template <bool WIDE>
+__device__ __forceinline__ void code_p_mb(const FrameCtx& f, MbTile& t, int lane, int mb, int qp, uint32_t mv, bool ltr, size_t ysz) {
   int luma_bits, chroma_bits;
   int cbp = transform_mb<false>(t, lane, qp, f.coef + (size_t)mb * COEF_BLOCKS * 16, f.nnz + (size_t)mb * 32, luma_bits, chroma_bits);
   if ((WIDE ? 48 + WM_MVD_BITS : 48) + luma_bits + chroma_bits > MB_BITS_LIMIT) { apply_pcm(t, lane, f.nnz + (size_t)mb * 32); cbp = -1; }   // A.3.1: send raw
@@ -382,9 +400,9 @@ __device__ __forceinline__ void finish_mb(const FrameCtx& f, MbTile& t, int lane
 // the search do not cap the occupancy of the common case.
 // LTR (B2V_FLAG_LONG_TERM_REF): the block counts changed(k) for k_ltr_mark, and while a long-term picture is a reference, a
 // macroblock that both exits fail is tested at the zero vector in it before it is queued (DESIGN.md §5.13).
-// CUT (B2V_FLAG_SCENE_CUT): every macroblock it finishes stores its cost (finish_mb).
-template <bool SCALE, bool WIDE, bool LTR, bool CUT>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) {
+// SIDE: every macroblock it finishes stores what B2V_FLAG_SCENE_CUT and B2V_FLAG_SIZE_CAP need of it (finish_mb).
+template <bool SCALE, bool WIDE, bool LTR, int SIDE>
+__device__ __forceinline__ void inter_lean(const FrameCtx& f) {
   __shared__ __align__(16) LeanSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int mbs = f.mbw * f.mbh;
@@ -451,8 +469,13 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
     }
   }
   if (p.anchor && lane == 0) publish_anchor<WIDE>(f, m, sad_int, LTR && mvx == LTR_MV ? 0 : mvx, LTR && mvy == LTR_MV ? 0 : mvy);   // sad_int 0 for refIdx 1
-  finish_mb<WIDE, CUT>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc, LTR);
+  finish_mb<WIDE, SIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc, LTR);
 }
+// CUT: B2V_FLAG_SCENE_CUT; the _cap variant: B2V_FLAG_SIZE_CAP
+template <bool SCALE, bool WIDE, bool LTR, bool CUT>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx f) { inter_lean<SCALE, WIDE, LTR, CUT ? SIDE_COST : 0>(f); }
+template <bool SCALE, bool WIDE, bool LTR, bool CUT>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean_cap(FrameCtx f) { inter_lean<SCALE, WIDE, LTR, SIDE_CAP | (CUT ? SIDE_COST : 0)>(f); }
 
 // One macroblock that k_inter_lean queued, from the start, through the same functions on the same inputs (source, reference and the
 // previous picture's records are not written during the analysis of a picture).  Its co-located block failed the zero-motion test
@@ -460,7 +483,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 8) k_inter_lean(FrameCtx
 // WIDE (B2V_FLAG_WIDE_MOTION): sm.win may hold the window centred on a full-sample vector (wx, wy) other than (0, 0) — a temporal or
 // anchor predictor outside the co-located window's test range, or an anchor's coarse vector x 4; candidate indices and (dx, dy) are
 // relative to that centre, costs are those of the real vector.
-template <bool SCALE, bool WIDE, bool CUT>
+template <bool SCALE, bool WIDE, int SIDE>
 __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int lane, const MbPos& p) {
   const int mb = p.mb, x0 = p.mbx * 16, y0 = p.mby * 16;
   const bool anchor = p.anchor;
@@ -660,21 +683,57 @@ __device__ __forceinline__ void search_mb(const FrameCtx& f, InterSm& sm, int la
   }
   if (anchor && lane == 0) publish_anchor<WIDE>(f, mb, sad_int, mvx, mvy);
   if (!refine) full_sample_pred(win, t, lane, dxi, dyi);
-  finish_mb<WIDE, CUT>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
+  finish_mb<WIDE, SIDE>(f, t, lane, p, qp, ylo, yhi, mvx, mvy, s.uv_coloc);
 }
 
 // Passes B and C: the queue k_inter_lean filled (0: anchors, 1: the rest), walked by a grid of the kernel's resident capacity.  No
 // decision here depends on another entry of the same queue, so the order inside a queue does not matter.
-template <bool SCALE, bool WIDE, bool CUT>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search(FrameCtx f, int queue) {
+template <bool SCALE, bool WIDE, int SIDE>
+__device__ __forceinline__ void inter_search(const FrameCtx& f, int queue) {
   __shared__ __align__(16) InterSm sm_all[WARPS_PER_BLOCK];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = f.me_queue[queue];
   const int* q = f.me_queue + 2 + (size_t)queue * f.mbw * f.mbh;
   for (int i = blockIdx.x * WARPS_PER_BLOCK + warp; i < n; i += gridDim.x * WARPS_PER_BLOCK) {
-    search_mb<SCALE, WIDE, CUT>(f, sm_all[warp], lane, mb_pos(f, q[i]));
+    search_mb<SCALE, WIDE, SIDE>(f, sm_all[warp], lane, mb_pos(f, q[i]));
     __syncwarp();
   }
+}
+template <bool SCALE, bool WIDE, bool CUT>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search(FrameCtx f, int queue) { inter_search<SCALE, WIDE, CUT ? SIDE_COST : 0>(f, queue); }
+template <bool SCALE, bool WIDE, bool CUT>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, 5) k_inter_search_cap(FrameCtx f, int queue) {
+  inter_search<SCALE, WIDE, SIDE_CAP | (CUT ? SIDE_COST : 0)>(f, queue);
+}
+
+// ---- k_requant (B2V_FLAG_SIZE_CAP): P picture k once more at the QP' k_size_cap chose, when it chose one; one warp per macroblock ----
+// Every macroblock keeps the prediction and vector the analysis stored (finish_mb) and is coded again from them by the code the
+// analysis ran (code_p_mb): transform, quantisation, the I_PCM fallback in both directions, reconstruction, levels, nnz, record.
+// The second CAVLC pass then evaluates P_Skip again.  oracle/h264_cap_ref.c requant.
+constexpr int REQUANT_WARPS = 4;
+__global__ void __launch_bounds__(32 * REQUANT_WARPS) k_requant(FrameCtx f) {
+  if (!*reinterpret_cast<const volatile int32_t*>(&f.cap->recode[f.pic & 1])) return;
+  __shared__ __align__(16) MbTile tiles[REQUANT_WARPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int mb = blockIdx.x * REQUANT_WARPS + warp;
+  if (mb >= f.mbw * f.mbh) return;
+  MbTile& t = tiles[warp];
+  const size_t ysz = (size_t)f.cw * f.ch;
+  const int mby = mb / f.mbw, mbx = mb - mby * f.mbw;
+  stage_source(f, t, lane, mbx * 16, mby, ysz);
+  const uint8_t* d = f.cap_pred + (size_t)mb * 384;
+  *reinterpret_cast<uint2*>(&t.pred_y[lane >> 1][(lane & 1) * 8]) = *reinterpret_cast<const uint2*>(d + (lane >> 1) * 16 + (lane & 1) * 8);
+  reinterpret_cast<uint32_t*>(&t.pred_uv[0][0])[lane] = reinterpret_cast<const uint32_t*>(d + 256)[lane];
+  const uint32_t mv = f.cap_mv[mb];
+  const int qp = f.cap->qp[f.pic & 1];
+  __syncwarp();
+  if (f.wide) code_p_mb<true>(f, t, lane, mb, qp, mv, f.ltr != nullptr, ysz);
+  else code_p_mb<false>(f, t, lane, mb, qp, mv, f.ltr != nullptr, ysz);
+}
+
+int launch_requant(const FrameCtx& f, cudaStream_t st) {
+  k_requant<<<(f.mbw * f.mbh + REQUANT_WARPS - 1) / REQUANT_WARPS, 32 * REQUANT_WARPS, 0, st>>>(f);
+  return 1;
 }
 
 cudaError_t inter_search_grid(int* blocks) {
@@ -688,28 +747,35 @@ cudaError_t inter_search_grid(int* blocks) {
 
 // The three passes of a P picture: SCALE, the previous picture's vectors span another reference distance than this picture's
 // (B2V_FLAG_DROPPABLE); WIDE, B2V_FLAG_WIDE_MOTION (k_coarse ran first on this stream); LTR, B2V_FLAG_LONG_TERM_REF; CUT,
-// B2V_FLAG_SCENE_CUT (k_scene_cut follows).
-template <bool SCALE, bool WIDE, bool LTR, bool CUT>
+// B2V_FLAG_SCENE_CUT (k_scene_cut follows); CAP, B2V_FLAG_SIZE_CAP (k_size_cap follows).
+template <bool SCALE, bool WIDE, bool LTR, bool CUT, bool CAP>
 void launch_passes(const FrameCtx& f, int lean_blocks, cudaStream_t st) {
+  if (CAP) {
+    k_inter_lean_cap<SCALE, WIDE, LTR, CUT><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
+    k_inter_search_cap<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);
+    k_inter_search_cap<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);
+    return;
+  }
   k_inter_lean<SCALE, WIDE, LTR, CUT><<<lean_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f);
   k_inter_search<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 0);   // anchors
   k_inter_search<SCALE, WIDE, CUT><<<f.search_blocks, 32 * WARPS_PER_BLOCK, 0, st>>>(f, 1);   // the rest: read the anchors' vectors
 }
-template <bool CUT>
+template <bool CUT, bool CAP>
 void launch_passes_for(const FrameCtx& f, int lean_blocks, cudaStream_t st) {
   // The long-term reference never comes with droppable pictures (check_coding_flags), so with it both distances are 1: LTR
   // implies !SCALE, and no <true, *, true, *> variant is compiled.
   const bool scale = f.ref_dist != f.prev_ref_dist;
-  if (f.ltr) f.wide ? launch_passes<false, true, true, CUT>(f, lean_blocks, st) : launch_passes<false, false, true, CUT>(f, lean_blocks, st);
-  else if (scale) f.wide ? launch_passes<true, true, false, CUT>(f, lean_blocks, st) : launch_passes<true, false, false, CUT>(f, lean_blocks, st);
-  else f.wide ? launch_passes<false, true, false, CUT>(f, lean_blocks, st) : launch_passes<false, false, false, CUT>(f, lean_blocks, st);
+  if (f.ltr) f.wide ? launch_passes<false, true, true, CUT, CAP>(f, lean_blocks, st) : launch_passes<false, false, true, CUT, CAP>(f, lean_blocks, st);
+  else if (scale) f.wide ? launch_passes<true, true, false, CUT, CAP>(f, lean_blocks, st) : launch_passes<true, false, false, CUT, CAP>(f, lean_blocks, st);
+  else f.wide ? launch_passes<false, true, false, CUT, CAP>(f, lean_blocks, st) : launch_passes<false, false, false, CUT, CAP>(f, lean_blocks, st);
 }
 
 int launch_inter(const FrameCtx& f, cudaStream_t st) {
   // both queues empty; the counters are only read by the two k_inter_search launches that follow
   cudaMemsetAsync(f.me_queue, 0, 2 * sizeof(int), st);
   const int lean_blocks = (f.mbw * f.mbh + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  if (f.scut) launch_passes_for<true>(f, lean_blocks, st); else launch_passes_for<false>(f, lean_blocks, st);
+  if (f.cap) f.scut ? launch_passes_for<true, true>(f, lean_blocks, st) : launch_passes_for<false, true>(f, lean_blocks, st);
+  else f.scut ? launch_passes_for<true, false>(f, lean_blocks, st) : launch_passes_for<false, false>(f, lean_blocks, st);
   return 3;
 }
 

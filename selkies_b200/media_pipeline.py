@@ -91,7 +91,7 @@ class MediaPipelineB200(MediaPipeline):
                  video_bitrate: int = 8, audio_bitrate: int = 128000, width: int = 1920, height: int = 1080,
                  audio_channels: int = 2, audio_enabled: bool = False, audio_device_name="output.monitor",
                  crf: int = 23, rc_mode: RateControlMode = RateControlMode.CBR, gpu_id: int = 0, frame_source=None,
-                 droppable_frames: bool = False, wide_motion: bool = False, scene_cut: bool = False):
+                 droppable_frames: bool = False, wide_motion: bool = False, scene_cut: bool = False, max_picture_bytes: int = 0):
         self.async_event_loop = async_event_loop
         self.async_lock = asyncio.Lock()
         # what selkies reads back
@@ -105,6 +105,8 @@ class MediaPipelineB200(MediaPipeline):
         self.wide_motion = wide_motion
         # a P picture whose content is all new (an application switch, a slide change) coded as an intra picture (B2V_FLAG_SCENE_CUT)
         self.scene_cut = scene_cut
+        # a P picture over this many bytes coded once more at a coarser QP (B2V_FLAG_SIZE_CAP); 0 = no cap
+        self.max_picture_bytes = max_picture_bytes
         self.last_resize_success = True
         # audio parameters are only carried
         self.audio_bitrate, self.audio_channels = audio_bitrate, audio_channels
@@ -213,6 +215,7 @@ class MediaPipelineB200(MediaPipeline):
             cs.h264_droppable_frames = bool(self.droppable_frames)
             cs.h264_wide_motion = bool(self.wide_motion)
             cs.h264_scene_cut = bool(self.scene_cut)
+            cs.h264_max_picture_kb = int(self.max_picture_bytes) / 1000      # read back as round(1000 * kb): the exact byte count
         return cs
 
     def _on_encoded(self, result_ptr, _user) -> None:

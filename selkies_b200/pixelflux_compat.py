@@ -80,6 +80,7 @@ class CaptureSettings:
         self.h264_wide_motion = False            # motion vectors up to 128 px across and 256 px down/up for fast scrolls and drags (H.264 only)
         self.h264_long_term_ref = False          # keep one earlier picture as a long-term reference: popups and app switches come back cheaply (full frame only)
         self.h264_scene_cut = False              # code a P picture whose content is all new as an intra picture (full frame only)
+        self.h264_max_picture_kb = 0             # cap of a P picture in KB (1000 bytes; fractions count): one recode at a coarser QP above it; 0 = off (H.264 only)
 
 
 class StripeCallback:
@@ -291,6 +292,9 @@ class ScreenCapture:
             if s.scene_cut and (jpeg or not bool(getattr(settings, "h264_fullframe", True))):
                 raise ValueError("h264_scene_cut needs full-frame H.264 (output_mode 1, h264_fullframe True): JPEG has no P pictures "
                                  "and every H.264 stripe is a stream of its own")
+            s.max_picture_bytes = round(1000 * float(getattr(settings, "h264_max_picture_kb", 0) or 0))
+            if s.max_picture_bytes > 0 and jpeg:
+                raise ValueError("h264_max_picture_kb needs H.264 (output_mode 1): JPEG has no P pictures")
             if bool(getattr(settings, "use_paint_over_quality", False)):
                 # selkies.py:3217, 3226-3229: after paint_over_trigger_frames static pictures, h264_paintover_burst_frames pictures
                 # are coded at h264_paintover_crf (in CBR mode only when that is finer than the rate controller's QP)

@@ -194,9 +194,12 @@ class Session:
                  gop: int = -1, slice_rows: int = 0, paintover_trigger_frames: int = 0, paintover_crf: int = 18, paintover_burst_frames: int = 1, idr_slice_mbs: int = 0, stripe_rows: int = 0, header_mode: int = N.B2V_HDR_NONE, ring_slots: int = 4,
                  flags: int = 0, on_frame: Optional[Callable[[C.POINTER(N.B2VFrame)], None]] = None,
                  collect: bool = True, quality: bool = False, droppable: bool = False, wide_motion: bool = False,
-                 long_term_ref: bool = False, scene_cut: bool = False, damage: bool = False):
+                 long_term_ref: bool = False, scene_cut: bool = False, damage: bool = False, max_picture_bytes: int = 0):
         self._lib = N.lib()
+        if max_picture_bytes < 0:
+            raise N.B2VError(N.B2V_EINVAL, "max_picture_bytes must be >= 0")
         flags |= N.B2V_FLAG_DAMAGE if damage else 0
+        flags |= N.B2V_FLAG_SIZE_CAP if max_picture_bytes > 0 else 0
         self.damage = bool(flags & N.B2V_FLAG_DAMAGE)      # the damage submits (damage=[...]) need it
         asked = dict(quality=quality, droppable=droppable, wide_motion=wide_motion, long_term_ref=long_term_ref, scene_cut=scene_cut)
         for name, bit in _OPT_IN_FLAGS.items():      # the attribute reports the bit, whether the keyword or `flags` set it
@@ -222,6 +225,8 @@ class Session:
         h = C.c_void_p()
         N.check(self._lib.b2v_create(C.byref(s), self._cb, None, C.byref(h)))
         self._h = h
+        if max_picture_bytes > 0:
+            self.set_max_picture_bytes(max_picture_bytes)
 
     # -- native callback (fires on the library's output thread) ------------------------------
     def _callback(self, fptr, _user):
@@ -333,6 +338,11 @@ class Session:
     def set_gop(self, frames: int) -> None:
         """Key-frame distance in pictures from the next submit on (<= 0: key frames only on request)."""
         N.check(self._lib.b2v_set_gop(self._h, int(frames)))
+
+    def set_max_picture_bytes(self, nbytes: int) -> None:
+        """The cap of every P picture from the next submit on (0 = none); needs B2V_FLAG_SIZE_CAP (Session(max_picture_bytes=...)
+        sets it when > 0).  A P picture whose macroblock layer exceeds it is coded once more at a coarser QP (include/b2video.h)."""
+        N.check(self._lib.b2v_set_max_picture_bytes(self._h, int(nbytes)))
 
     def request_idr(self) -> None:
         N.check(self._lib.b2v_request_idr(self._h))
